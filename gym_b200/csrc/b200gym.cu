@@ -62,12 +62,15 @@ struct b200gym {
     } ep;
     int sm_count = 132;
     int occ[B200GYM_NUM_KINDS][3][4] = {};  // cached CTAs/SM of step_kernel_persistent per (kind, action width, lean + 2 * deep)
+    int occ_bulk[B200GYM_NUM_KINDS][3] = {};  // ... of step_kernel_persistent_bulk per (kind, action width)
     int p_depth = 1;                        // kernel P/L: tiles in flight per thread (B200GYM_P_DEPTH=1|2)
     int p_ctas = -1;                        // kernel P/L: resident CTAs per SM; -1 = occupancy limit, 0 = balance the tile
                                             // rounds (see launch_step_typed), k > 0 = exactly k (B200GYM_P_CTAS, tuning runs)
-    int kernel_choice = 2;                  // 0: kernel A (one tile per CTA), 1: kernel P (resident grid, asynchronous
-                                            // prefetch, deferred resets), 2: P's lean instantiation where it applies
-                                            // (else P); B200GYM_KERNEL=a|p|l overrides
+    int kernel_choice = -1;                 // -1: kernel B (bulk copies) where bulk_by_default picks it, else P's lean
+                                            // instantiation; 0: kernel A (one tile per CTA), 1: kernel P (resident grid,
+                                            // asynchronous prefetch, deferred resets), 2: P's lean instantiation where it
+                                            // applies (else P), 3: kernel B where it applies (else lean P);
+                                            // B200GYM_KERNEL=a|p|l|b overrides
     int gather_bulk = 1;                    // multi-GPU step: 1 = kernel G (staged tile + bulk pushes), 0 = per-thread
                                             // peer stores from kernel A; B200GYM_GATHER=bulk|direct overrides
     int block_a = 256;                      // CTA size of kernel A (B200GYM_BLOCK_A=64|128|256, tuning runs)
@@ -309,14 +312,23 @@ struct DirectSinkT {
         if constexpr (PEERS) store_scalars_all(a, i, reward, term, trunc);
         else { a.reward[i] = reward; a.terminated[i] = term; a.truncated[i] = trunc; }
     }
+    template <int S, typename I>
+    __device__ __forceinline__ void state(I i, const double (&s)[S]) const {
+#pragma unroll
+        for (int k = 0; k < S; k++) a.state[k * a.n + i] = s[k];
+    }
+    template <typename I>
+    __device__ __forceinline__ void elapsed(I i, int32_t e) const { a.elapsed[i] = e; }
 };
 using DirectSink = DirectSinkT<true>;
 
+// kernel G: the outputs are staged, the persistent state goes straight back to HBM
 struct StagedSink {
     float *s_obs;
     double *s_reward;
     uint8_t *s_term, *s_trunc;
     int64_t base;   // env index of row 0 of the tile
+    const StepArgs &a;
     template <int D, typename I>
     __device__ __forceinline__ void obs(I i, const float (&v)[D]) const { store_row<D>(s_obs, (int)(i - base), v); }
     template <typename I>
@@ -324,6 +336,40 @@ struct StagedSink {
         const int r = (int)(i - base);
         s_reward[r] = reward; s_term[r] = term; s_trunc[r] = trunc;
     }
+    template <int S, typename I>
+    __device__ __forceinline__ void state(I i, const double (&s)[S]) const {
+#pragma unroll
+        for (int k = 0; k < S; k++) a.state[k * a.n + i] = s[k];
+    }
+    template <typename I>
+    __device__ __forceinline__ void elapsed(I i, int32_t e) const { a.elapsed[i] = e; }
+};
+
+// kernel B: every row that the tile's bulk stores cover is written into the tile's stage -- the new state and
+// TimeLimit counter in place over the inputs, so that a row nobody writes (an invalid action, an env left for the
+// deferred reset) goes back to HBM unchanged
+struct InPlaceSink {
+    double *s_state;   // [S][kThreads]
+    int32_t *s_elapsed;
+    float *s_obs;
+    double *s_reward;
+    uint8_t *s_term, *s_trunc;
+    uint32_t base;     // env index of row 0 of the tile
+    template <int D, typename I>
+    __device__ __forceinline__ void obs(I i, const float (&v)[D]) const { store_row<D>(s_obs, (int)(i - base), v); }
+    template <typename I>
+    __device__ __forceinline__ void scalars(I i, double reward, uint8_t term, uint8_t trunc) const {
+        const int r = (int)(i - base);
+        s_reward[r] = reward; s_term[r] = term; s_trunc[r] = trunc;
+    }
+    template <int S, typename I>
+    __device__ __forceinline__ void state(I i, const double (&s)[S]) const {
+        const int r = (int)(i - base);
+#pragma unroll
+        for (int k = 0; k < S; k++) s_state[k * kThreads + r] = s[k];
+    }
+    template <typename I>
+    __device__ __forceinline__ void elapsed(I i, int32_t e) const { s_elapsed[(int)(i - base)] = e; }
 };
 
 // Tuning knobs (overridable at build time for A/B measurements).
@@ -343,6 +389,9 @@ struct Tuning {
     // without a spill, which would make BASELINE's 2^18 envs one round of tiles instead of two; at 2^18 envs they are
     // latency-bound either way, so they keep the common budget.)
     static constexpr int kMinCtas = (KIND == B200GYM_ACROBOT) ? 3 : B200_MIN_CTAS;
+    // kernel B (288 threads): 4 CTAs/SM = 32 compute warps and 56 registers a thread; the CTA's 3 stages of ~18 KB
+    // (CartPole) leave 4 CTAs inside the SM's 228 KB of shared memory.  Acrobot: 2 CTAs, 113 registers
+    static constexpr int kBulkMinCtas = (KIND == B200GYM_ACROBOT) ? 2 : 4;
 };
 
 // Phase 1, by the thread that owns env i (its inputs are in registers): Env.step, TimeLimit,
@@ -394,9 +443,8 @@ __device__ __forceinline__ bool advance_env(const StepArgs &a, const Sink &sink,
     if (needs_reset) {
         if (a.final_obs) store_row<E::D>(a.final_obs, i, obs);           // info["final_observation"]
     } else {
-#pragma unroll
-        for (int k = 0; k < E::S; k++) a.state[k * a.n + i] = s[k];
-        a.elapsed[i] = elapsed;
+        sink.template state<E::S>(i, s);
+        sink.elapsed(i, elapsed);
         sink.template obs<E::D>(i, obs);
     }
     return needs_reset;
@@ -414,9 +462,8 @@ __device__ __forceinline__ void reset_env(const StepArgs &a, const Sink &sink, I
     E::default_bounds(lo, hi);
     E::reset(s, g, lo, hi, obs);
     pcg64_store(a.rng + 4 * (size_t)i, g);
-#pragma unroll
-    for (int k = 0; k < E::S; k++) a.state[k * a.n + i] = s[k];
-    a.elapsed[i] = 0;                                                    // time_limit.py:67
+    sink.template state<E::S>(i, s);
+    sink.elapsed(i, 0);                                                  // time_limit.py:67
     sink.template obs<E::D>(i, obs);
 }
 
@@ -485,6 +532,38 @@ __device__ __forceinline__ void st_bulk_wait_read() { asm volatile("cp.async.bul
 __device__ __forceinline__ void st_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // generic-proxy writes to shared memory -> visible to the async proxy that executes the bulk copy
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// completed bulk-copy writes to global memory -> ordered before the generic-proxy stores that follow
+__device__ __forceinline__ void fence_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// mbarrier in shared memory: `count` arrivals plus the transaction bytes announced by expect_tx complete a phase
+__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+// the initialised barriers -> visible to the async proxy (the bulk copies complete transactions on them)
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// until the phase of parity `parity` has completed
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
+    uint32_t ok;
+    do {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(ok)
+                     : "r"(smem_u32(bar)), "r"(parity)
+                     : "memory");
+    } while (!ok);
+}
+// bulk (TMA, SASS UBLKCP) global -> shared load of a contiguous block; its bytes complete on `bar`
+__device__ __forceinline__ void ld_bulk(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                     smem_u32(smem_dst)),
+                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
 
 }  // namespace acp
 
@@ -604,6 +683,150 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
     for (int q = tid; q < cnt; q += kThreads) reset_env<KIND>(a, sink, (Idx)(first + (Idx)reset_list[q]));
 }
 
+// --- kernel B: kernel P's resident grid with every HBM row moved by bulk copies -------------------------------
+// In kernel P each compute warp is also its own memory engine: per tile it issues S + 2 per-thread cp.async and
+// S + 5 per-thread stores, and when HBM is saturated those instructions queue behind each other in the LSU, so the
+// arithmetic advances only as fast as memory accepts requests.  Here one extra warp (one elected thread) moves the
+// tiles: a ring of kBulkStages stages per CTA, each filled by S + 2 bulk loads (state rows, TimeLimit counters,
+// actions) that complete on the stage's `full` mbarrier.  The 8 compute warps read their env's inputs from the
+// stage, write every result back INTO the stage (new state and counter in place, obs / reward / flags in the
+// stage's output block: InPlaceSink), fence the writes to the async proxy and arrive on the stage's `done`
+// mbarrier; the copy thread then pushes the whole tile out with S + 5 bulk stores and, once they have read the
+// stage, refills it with the tile kBulkStages rounds ahead.  So the compute warps execute only shared-memory loads and
+// stores on the common path.  Resets as in kernel P: dense warps reset inline (through the stage), the others go
+// onto the CTA's list, which is drained with direct stores after every bulk store of the CTA has COMPLETED -- a
+// reset's rows must land after the tile's bulk store of the same rows.
+// Whole tiles only, every row 16-byte aligned (launch_step_typed checks), 32-bit env indices.
+constexpr int kBulkStages = 3;   // 2 stages at 5 CTAs/SM measured slower (DESIGN §4.1)
+constexpr int kBulkResetCap = 512;   // 4 CTAs x ~8 tiles x 256 envs / CTA, ~4.5 % finishing: ~90 entries typical
+
+template <int KIND, typename ActT>
+struct BulkLayout {
+    using E = Env<KIND>;
+    static constexpr int kActPerEnv = E::A == 0 ? 1 : E::A;
+    static constexpr int kStateOff = 0;                                       // [S][256] float64, in place
+    static constexpr int kElapsedOff = E::S * kThreads * 8;                   // [256] int32, in place
+    static constexpr int kActOff = kElapsedOff + kThreads * 4;                // [256][A] actions
+    static constexpr int kObsOff = kActOff + kThreads * kActPerEnv * (int)sizeof(ActT);   // [256][D] float32
+    static constexpr int kRewardOff = kObsOff + kThreads * E::D * 4;          // [256] float64
+    static constexpr int kTermOff = kRewardOff + kThreads * 8;                // [256] uint8
+    static constexpr int kTruncOff = kTermOff + kThreads;                     // [256] uint8
+    static constexpr int kBytes = kTruncOff + kThreads;
+    static constexpr uint32_t kLoadBytes = kObsOff;                           // the bulk loads fill [0, kObsOff)
+    static_assert(kActOff % 16 == 0 && kObsOff % 16 == 0 && kBytes % 128 == 0, "bulk copies need 16-byte rows");
+};
+
+template <int KIND, typename ActT>
+__global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
+    step_kernel_persistent_bulk(const StepArgs a, const int num_tiles) {
+    using E = Env<KIND>;
+    using L = BulkLayout<KIND, ActT>;
+    extern __shared__ __align__(128) unsigned char stage_mem[];   // [kBulkStages][L::kBytes]
+    __shared__ __align__(8) uint64_t full[kBulkStages], done[kBulkStages];
+    __shared__ int reset_list[kBulkResetCap];
+    __shared__ int reset_count;
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        reset_count = 0;
+        for (int q = 0; q < kBulkStages; q++) {
+            acp::mbar_init(&full[q], 1);
+            acp::mbar_init(&done[q], kThreads / 32);
+        }
+        acp::fence_mbar_init();
+    }
+    __syncthreads();
+    const uint32_t first = (uint32_t)a.first, n = (uint32_t)a.n;
+
+    if (tid >= kThreads) {
+        if (tid == kThreads) {   // the copy thread
+            auto load = [&](int tile, int q) {
+                unsigned char *b = stage_mem + q * L::kBytes;
+                const uint32_t i0 = first + (uint32_t)tile * kThreads;
+                acp::mbar_arrive_expect_tx(&full[q], L::kLoadBytes);
+#pragma unroll
+                for (int k = 0; k < E::S; k++)
+                    acp::ld_bulk(b + L::kStateOff + k * kThreads * 8, a.state + k * n + i0, kThreads * 8, &full[q]);
+                acp::ld_bulk(b + L::kElapsedOff, a.elapsed + i0, kThreads * 4, &full[q]);
+                acp::ld_bulk(b + L::kActOff, reinterpret_cast<const ActT *>(a.actions) + i0 * L::kActPerEnv,
+                             L::kObsOff - L::kActOff, &full[q]);
+            };
+            auto store = [&](int tile, int q) {
+                const unsigned char *b = stage_mem + q * L::kBytes;
+                const uint32_t i0 = first + (uint32_t)tile * kThreads;
+#pragma unroll
+                for (int k = 0; k < E::S; k++) acp::st_bulk(a.state + k * n + i0, b + L::kStateOff + k * kThreads * 8, kThreads * 8);
+                acp::st_bulk(a.elapsed + i0, b + L::kElapsedOff, kThreads * 4);
+                acp::st_bulk(a.obs + i0 * E::D, b + L::kObsOff, kThreads * E::D * 4);
+                acp::st_bulk(a.reward + i0, b + L::kRewardOff, kThreads * 8);
+                acp::st_bulk(a.terminated + i0, b + L::kTermOff, kThreads);
+                acp::st_bulk(a.truncated + i0, b + L::kTruncOff, kThreads);
+                acp::st_bulk_commit();
+            };
+            int q = 0;
+            for (int t = blockIdx.x; q < kBulkStages && t < num_tiles; t += gridDim.x) load(t, q++);
+            q = 0;
+            uint32_t parity = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                acp::mbar_wait(&done[q], parity);
+                store(tile, q);
+                const int next = tile + kBulkStages * (int)gridDim.x;
+                if (next < num_tiles) {
+                    // the stage is free once the stores have READ it (a few hundred ns); waiting right away keeps
+                    // kBulkStages - 1 tiles of loads ahead of the compute warps instead of kBulkStages - 2
+                    acp::st_bulk_wait_read();
+                    load(next, q);
+                }
+                if (++q == kBulkStages) { q = 0; parity ^= 1u; }
+            }
+            acp::st_bulk_wait_all();     // the drain below overwrites rows of these stores
+            acp::fence_async_global();
+        }
+    } else {
+        const int lane = tid & 31;
+        int q = 0;
+        uint32_t parity = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            unsigned char *b = stage_mem + q * L::kBytes;
+            const uint32_t j = (uint32_t)tile * kThreads + tid;
+            const uint32_t i = first + j;
+            const InPlaceSink sink{reinterpret_cast<double *>(b + L::kStateOff), reinterpret_cast<int32_t *>(b + L::kElapsedOff),
+                                   reinterpret_cast<float *>(b + L::kObsOff), reinterpret_cast<double *>(b + L::kRewardOff),
+                                   b + L::kTermOff, b + L::kTruncOff, i - tid};
+            acp::mbar_wait(&full[q], parity);
+            double s[E::S];
+#pragma unroll
+            for (int k = 0; k < E::S; k++) s[k] = sink.s_state[k * kThreads + tid];
+            const int32_t elapsed = sink.s_elapsed[tid];
+            const ActT av = reinterpret_cast<const ActT *>(b + L::kActOff)[tid * L::kActPerEnv];
+            long long action_int = 0;
+            float a0 = 0.0f;
+            if constexpr (E::A == 0) action_int = (long long)av;
+            else a0 = (float)av;
+            const bool need = advance_env<KIND, false>(a, sink, i, s, elapsed, action_int, a0);
+            const unsigned m = __ballot_sync(0xffffffffu, need);
+            if (m != 0u) {
+                bool inline_reset = __popc(m) >= 12;
+                if (need && !inline_reset) {
+                    const int slot = atomicAdd(&reset_count, 1);
+                    if (slot < kBulkResetCap) {
+                        reset_list[slot] = (int)j;
+                        asm volatile("prefetch.global.L2 [%0];" ::"l"(a.rng + 4 * (size_t)i));
+                    } else inline_reset = true;
+                }
+                if (need && inline_reset) reset_env<KIND>(a, sink, i);
+            }
+            acp::fence_async_smem();
+            __syncwarp();
+            if (lane == 0) acp::mbar_arrive(&done[q]);
+            if (++q == kBulkStages) { q = 0; parity ^= 1u; }
+        }
+    }
+    __syncthreads();
+    const int cnt = min(reset_count, kBulkResetCap);
+    const DirectSinkT<false> direct{a};
+    for (int q = tid; q < cnt; q += kThreads + 32) reset_env<KIND>(a, direct, first + (uint32_t)reset_list[q]);
+}
+
 // --- kernel G: one tile per CTA, results staged in shared memory and pushed with bulk stores ---------
 // The multi-GPU step (b200gym_step_p2p): every result must land in this rank's rows of EVERY rank's gather
 // buffers.  Per-thread peer stores put 16-, 8- and 1-byte writes on NVLink; here the 256-env tile of
@@ -624,7 +847,7 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
     __syncthreads();
     const int64_t j0 = (int64_t)blockIdx.x * kThreads;      // full tiles only: no bound check
     const int64_t i0 = a.first + j0;
-    const StagedSink sink{s_obs, s_reward, s_term, s_trunc, i0};
+    const StagedSink sink{s_obs, s_reward, s_term, s_trunc, i0, a};
     {
         const int64_t i = i0 + threadIdx.x;
         double s[E::S];
@@ -1333,6 +1556,11 @@ static inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads -
 // ---------------------------------------------------------------------------
 // dispatch
 // ---------------------------------------------------------------------------
+// Kernel B by default where it measured faster than lean P (DESIGN §4.1): CartPole, at 2^18, 2^20 and 2^23 envs.  The other
+// kinds are slower with it at 2^18 envs -- one partly filled wave, latency-bound, where B's 32 compute warps per SM
+// (P: 48) cost more than moving the memory traffic off the compute warps saves
+static bool bulk_by_default(int kind) { return kind == B200GYM_CARTPOLE; }
+
 template <int KIND, typename ActT>
 static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
     int64_t done = 0;
@@ -1357,14 +1585,40 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
             h->p2p_barrier_fused = fused_barrier;
         }
     }
-    if (done == 0 && h->kernel_choice >= 1 && a.npeer == 0 && a.count >= (int64_t)h->sm_count * kThreads) {
+    const bool resident = a.npeer == 0 && a.count >= (int64_t)h->sm_count * kThreads;
+    const bool bulk = h->kernel_choice == 3 || (h->kernel_choice == -1 && bulk_by_default(KIND));
+    if (done == 0 && resident && bulk && !a.ep_acc && h->n < (int64_t)1 << 30) {
+        // kernel B: whole tiles, every row a bulk copy touches 16-byte aligned
+        using L = BulkLayout<KIND, ActT>;
+        const auto al = [](const void *p) { return (uintptr_t)p % 16 == 0; };
+        bool aligned = h->n % 2 == 0 && al(a.state + a.first) && al(a.elapsed + a.first) && al(a.obs + a.first * Env<KIND>::D) &&
+                       al(a.reward + a.first) && al(a.terminated + a.first) && al(a.truncated + a.first) &&
+                       al(reinterpret_cast<const ActT *>(a.actions) + a.first * L::kActPerEnv);
+        if (aligned) {
+            const int smem = kBulkStages * L::kBytes;
+            int &occ = h->occ_bulk[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2];
+            if (occ == 0) {
+                CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+                CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                           (int)cudaSharedmemCarveoutMaxShared));
+                CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent_bulk<KIND, ActT>, kThreads + 32, smem));
+                if (occ < 1) occ = 1;
+            }
+            int64_t grid = (int64_t)h->sm_count * occ;
+            if (grid > tiles) grid = tiles;
+            step_kernel_persistent_bulk<KIND, ActT><<<(unsigned)grid, kThreads + 32, smem, st>>>(a, (int)tiles);
+            CK(h, cudaGetLastError());
+            done = tiles * kThreads;   // a ragged tail goes to kernel A below
+        }
+    }
+    if (done == 0 && h->kernel_choice != 0 && resident) {
         // kernel P: resident grid; needs naturally aligned input words for cp.async (always true for the
         // handle's own arrays; the caller's action pointer is checked)
         using L = PrefetchLayout<KIND, ActT>;
         const bool aligned = !L::kActAsync || ((uintptr_t)a.actions % L::kActBytes == 0);
         if (aligned) {
             // the lean instantiation: no fused episode statistics, every index fits 32 bits
-            const bool lean = h->kernel_choice == 2 && !a.ep_acc && h->n < (int64_t)1 << 30;
+            const bool lean = h->kernel_choice != 1 && !a.ep_acc && h->n < (int64_t)1 << 30;
             const bool deep = h->p_depth == 2;
             int &occ = h->occ[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2][(lean ? 1 : 0) + (deep ? 2 : 0)];
             if (occ == 0) {
@@ -1630,7 +1884,8 @@ extern "C" int b200gym_create(const b200gym_config *cfg, int64_t num_envs, int d
     {
         const char *fs = getenv("B200GYM_SIMPLE_KERNEL");
         const char *kc = getenv("B200GYM_KERNEL");
-        if (kc && (kc[0] == 'a' || kc[0] == 'p' || kc[0] == 'l')) h->kernel_choice = kc[0] == 'a' ? 0 : kc[0] == 'p' ? 1 : 2;
+        if (kc && (kc[0] == 'a' || kc[0] == 'p' || kc[0] == 'l' || kc[0] == 'b'))
+            h->kernel_choice = kc[0] == 'a' ? 0 : kc[0] == 'p' ? 1 : kc[0] == 'l' ? 2 : 3;
         const char *pd = getenv("B200GYM_P_DEPTH");
         if (pd && (pd[0] == '1' || pd[0] == '2')) h->p_depth = pd[0] - '0';
         const char *pc = getenv("B200GYM_P_CTAS");
