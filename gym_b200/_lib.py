@@ -92,6 +92,11 @@ SIGNATURES = {
     "b200gym_reset_host": (_i32, [_vp, _vp, _vp, _vp]),
     "b200gym_get_state": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "b200gym_set_state": (_i32, [_vp, _vp, _vp, _vp, _vp]),
+    "b200gym_snapshot_row_bytes": (_i64, [_i32]),
+    "b200gym_snapshot_save": (_i32, [_vp, _vp, _i64, _vp, _vp]),
+    "b200gym_snapshot_load": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "b200gym_clone": (_i32, [_vp, _vp, _vp]),
+    "b200gym_snapshot_index_error": (_i32, [_vp]),
     "b200gym_lunar_get_bodies": (_i32, [_vp, _vp, _vp, _vp]),
     "b200gym_lunar_wind_idx": (_i32, [_vp, _vp, _vp, _i32]),
     "b200gym_walker_get_bodies": (_i32, [_vp, _vp, _vp, _vp]),

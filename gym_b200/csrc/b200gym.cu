@@ -125,6 +125,10 @@ struct b200gym {
                                             // launch save -- so the separate launch stays the default
     cudaStream_t hstream[2] = {nullptr, nullptr};
     bool host_ready = false;
+    // env snapshots (lazily created)
+    unsigned long long *snap_bad = nullptr;       // page-locked, device-mapped word: an out-of-range snapshot index was met
+    unsigned long long *snap_bad_dev = nullptr;   // device alias
+    unsigned char *snap_scratch = nullptr;        // b200gym_clone: n rows
     mutable std::string err;
 };
 
@@ -159,6 +163,8 @@ extern "C" int b200gym_obs_dim(int kind) { return kind_ok(kind) ? k_obs_dim[kind
 extern "C" int b200gym_act_dim(int kind) { return kind_ok(kind) ? k_act_dim[kind] : -1; }
 extern "C" int b200gym_num_actions(int kind) { return kind_ok(kind) ? k_nact[kind] : -1; }
 extern "C" int b200gym_state_dim(int kind) { return kind_ok(kind) ? k_state_dim[kind] : -1; }
+static int snap_row_bytes(int kind);
+extern "C" int64_t b200gym_snapshot_row_bytes(int kind) { return kind_ok(kind) ? snap_row_bytes(kind) : -1; }
 extern "C" int b200gym_version(void) { return B200GYM_VERSION; }
 extern "C" const char *b200gym_last_error(const b200gym_t *h) {
     return h ? h->err.c_str() : g_create_err.c_str();
@@ -963,6 +969,155 @@ __global__ void __launch_bounds__(kThreads) state_set_kernel(double *soa, const 
     const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
     if (i >= n) return;
     for (int k = 0; k < S; k++) soa[k * n + i] = aos[i * S + k];
+}
+
+// ---- env snapshots (b200gym_snapshot_*, b200gym_clone) ---------------------------------------------
+// One AoS row per env holding every per-env word a later step reads, as 32-bit words:
+//   [0, 8)              PCG64 record {state_hi, state_lo, inc_hi, inc_lo}
+//   [8, 8 + 2S)         float64 state[S]
+//   [8 + 2S, .. + W)    Box2D solver record rec[W] (wind counters and the walker's buffered 32-bit draw included)
+//   then elapsed, flags (low byte of a word) and zeros up to a multiple of 32 B (one DRAM sector).
+// The transient per-step buffers (toi_mid, the reset / TOI lists) are not state and stay out of the row.
+// A CTA moves a tile of T envs through shared memory in 16-byte chunks: thread e takes chunk e / T of env e % T, so
+// the lanes of a warp share a chunk (warp-uniform field branches) and read / write each SoA word of 32 consecutive
+// envs with one coalesced access.  The tile is contiguous rows of R bytes; R / 16 is even, so a quarter warp's 16-byte
+// shared accesses at stride R hit each bank group at most twice (2-way: half the shared bandwidth, still several
+// times what HBM can feed).
+constexpr int kSnapMaxTileBytes = 96 * 1024;   // opt-in shared memory: 2 CTAs / SM even for the 2 KB hardcore rows
+
+static int snap_record_words(int kind) {
+    switch (kind) {
+    case B200GYM_LUNARLANDER: case B200GYM_LUNARLANDER_CONT: return lunar::kWords;
+    case B200GYM_BIPEDALWALKER: return walker::kWords;
+    case B200GYM_BIPEDALWALKER_HARDCORE: return walker::kWordsHC;
+    default: return 0;
+    }
+}
+static int snap_unpadded_bytes(int kind) { return 32 + 8 * k_state_dim[kind] + 4 * snap_record_words(kind) + 4 + 1; }
+static int snap_row_bytes(int kind) { return (snap_unpadded_bytes(kind) + 31) / 32 * 32; }
+static int snap_tile(int row_bytes) {
+    int t = kThreads;
+    while (t > 32 && t * row_bytes > kSnapMaxTileBytes) t /= 2;
+    return t;
+}
+
+struct SnapArgs {
+    uint32_t *rng, *state, *rec;   // the handle's arrays as 32-bit words
+    int32_t *elapsed;
+    uint8_t *flags;
+    int64_t n;
+    int S2, W;                     // 32-bit words of state and of the Box2D record
+    int chunks;                    // row bytes / 16
+    int tile_log2;                 // T = 1 << tile_log2 envs per CTA
+    unsigned long long *bad;       // page-locked, device-mapped word: set by a kernel that meets an out-of-range index
+};
+
+__device__ __forceinline__ uint32_t snap_get(const SnapArgs &a, int w, int64_t i) {
+    if (w < 8) return a.rng[8 * i + w];
+    w -= 8;
+    if (w < a.S2) return a.state[2 * ((int64_t)(w >> 1) * a.n + i) + (w & 1)];
+    w -= a.S2;
+    if (w < a.W) return a.rec[(int64_t)w * a.n + i];
+    w -= a.W;
+    if (w == 0) return (uint32_t)a.elapsed[i];
+    if (w == 1) return a.flags[i];
+    return 0u;
+}
+__device__ __forceinline__ void snap_put(const SnapArgs &a, int w, int64_t i, uint32_t v) {
+    if (w < 8) { a.rng[8 * i + w] = v; return; }
+    w -= 8;
+    if (w < a.S2) { a.state[2 * ((int64_t)(w >> 1) * a.n + i) + (w & 1)] = v; return; }
+    w -= a.S2;
+    if (w < a.W) { a.rec[(int64_t)w * a.n + i] = v; return; }
+    w -= a.W;
+    if (w == 0) a.elapsed[i] = (int32_t)v;
+    else if (w == 1) a.flags[i] = (uint8_t)v;
+}
+__device__ __forceinline__ void snap_raise(const SnapArgs &a) {
+    *reinterpret_cast<volatile unsigned long long *>(a.bad) = 1ULL;
+}
+
+// env idx[k] (idx == NULL: k) -> row k of snap, for k < m.  Out-of-range envs leave a zero row and raise a.bad.
+__global__ void __launch_bounds__(kThreads) snapshot_save_kernel(const SnapArgs a, const int64_t *idx, int64_t m,
+                                                                 unsigned char *snap) {
+    extern __shared__ __align__(128) unsigned char s_tile[];
+    const int T = 1 << a.tile_log2, C = a.chunks, R = 16 * C;
+    int64_t *s_env = reinterpret_cast<int64_t *>(s_tile + (size_t)T * R);
+    const int64_t k0 = (int64_t)blockIdx.x * T;
+    const int rows = (int)(m - k0 < T ? m - k0 : T);
+    for (int t = threadIdx.x; t < rows; t += kThreads) {
+        int64_t i = idx ? idx[k0 + t] : k0 + t;
+        if (i < 0 || i >= a.n) { snap_raise(a); i = -1; }
+        s_env[t] = i;
+    }
+    __syncthreads();
+    uint4 *tile = reinterpret_cast<uint4 *>(s_tile);
+    for (int e = threadIdx.x; e < T * C; e += kThreads) {
+        const int t = e & (T - 1), c = e >> a.tile_log2;
+        if (t >= rows) continue;
+        const int64_t i = s_env[t];
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (i >= 0) {
+            v.x = snap_get(a, 4 * c, i); v.y = snap_get(a, 4 * c + 1, i);
+            v.z = snap_get(a, 4 * c + 2, i); v.w = snap_get(a, 4 * c + 3, i);
+        }
+        tile[t * C + c] = v;
+    }
+    acp::fence_async_smem();
+    __syncthreads();
+    if (threadIdx.x == 0) {   // the whole tile leaves as one bulk store
+        acp::st_bulk(snap + k0 * R, s_tile, (uint32_t)(rows * R));
+        acp::st_bulk_commit();
+        acp::st_bulk_wait_all();
+    }
+}
+
+// row row[k] of snap (snap_rows rows) -> env dst[k], for k < m; NULL index arrays = k.  Entries with an out-of-range
+// row or env are skipped and raise a.bad.  Duplicate envs in dst: which row lands is undefined.
+__global__ void __launch_bounds__(kThreads) snapshot_load_kernel(const SnapArgs a, const unsigned char *snap,
+                                                                 int64_t snap_rows, const int64_t *row,
+                                                                 const int64_t *dst, int64_t m) {
+    extern __shared__ __align__(128) unsigned char s_tile[];
+    const int T = 1 << a.tile_log2, C = a.chunks, R = 16 * C;
+    int64_t *s_env = reinterpret_cast<int64_t *>(s_tile + (size_t)T * R);
+    int64_t *s_row = s_env + T;
+    uint64_t *bar = reinterpret_cast<uint64_t *>(s_row + T);
+    const int64_t k0 = (int64_t)blockIdx.x * T;
+    const int rows = (int)(m - k0 < T ? m - k0 : T);
+    for (int t = threadIdx.x; t < rows; t += kThreads) {
+        const int64_t r = row ? row[k0 + t] : k0 + t;
+        const int64_t d = dst ? dst[k0 + t] : k0 + t;
+        const bool ok = r >= 0 && r < snap_rows && d >= 0 && d < a.n;
+        if (!ok) snap_raise(a);
+        s_row[t] = ok ? r : -1;
+        s_env[t] = ok ? d : -1;
+    }
+    if (threadIdx.x == 0) {
+        acp::mbar_init(bar, 1);
+        acp::fence_mbar_init();
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {   // warp 0 gathers the tile's source rows: one bulk copy per row, all completing on `bar`
+        const int lane = threadIdx.x;
+        int valid = 0;
+        for (int t = lane; t < rows; t += 32) valid += s_row[t] >= 0;
+        valid = __reduce_add_sync(0xffffffffu, valid);
+        if (lane == 0) acp::mbar_arrive_expect_tx(bar, (uint32_t)(valid * R));
+        __syncwarp();
+        for (int t = lane; t < rows; t += 32)
+            if (s_row[t] >= 0) acp::ld_bulk(s_tile + (size_t)t * R, snap + s_row[t] * R, (uint32_t)R, bar);
+    }
+    acp::mbar_wait(bar, 0);
+    const uint4 *tile = reinterpret_cast<const uint4 *>(s_tile);
+    for (int e = threadIdx.x; e < T * C; e += kThreads) {
+        const int t = e & (T - 1), c = e >> a.tile_log2;
+        if (t >= rows) continue;
+        const int64_t i = s_env[t];
+        if (i < 0) continue;
+        const uint4 v = tile[t * C + c];
+        snap_put(a, 4 * c, i, v.x); snap_put(a, 4 * c + 1, i, v.y);
+        snap_put(a, 4 * c + 2, i, v.z); snap_put(a, 4 * c + 3, i, v.w);
+    }
 }
 
 // ---- LunarLander-v2 (lunar.cuh): one thread per env, the whole b2World::Step in registers/local ----
@@ -2007,6 +2162,8 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     if (h->side) cudaStreamDestroy(h->side);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join) cudaEventDestroy(h->ev_join);
+    if (h->snap_bad) cudaFreeHost(h->snap_bad);
+    cudaFree(h->snap_scratch);
     if (h->p2p.base) {
         for (int r = 0; r < h->p2p.world; r++)
             if (r != h->p2p.rank && h->p2p.peer[r]) cudaIpcCloseMemHandle(h->p2p.peer[r]);
@@ -2621,4 +2778,107 @@ extern "C" int b200gym_set_state(b200gym_t *h, const double *state_dev, const in
         CK(h, cudaMemcpyAsync(h->elapsed, elapsed_dev, sizeof(int32_t) * (size_t)h->n, cudaMemcpyDeviceToDevice, st));
     if (rng_dev) CK(h, cudaMemcpyAsync(h->rng, rng_dev, 32 * (size_t)h->n, cudaMemcpyDeviceToDevice, st));
     return 0;
+}
+
+// ---- env snapshots ----------------------------------------------------------
+static int snap_prepare(b200gym *h, const char *who) {
+    if (!h->snap_bad) {
+        if (cudaHostAlloc((void **)&h->snap_bad, sizeof(unsigned long long), cudaHostAllocMapped) != cudaSuccess ||
+            cudaHostGetDevicePointer((void **)&h->snap_bad_dev, h->snap_bad, 0) != cudaSuccess) {
+            if (h->snap_bad) cudaFreeHost(h->snap_bad);
+            h->snap_bad = nullptr;
+            return fail(h, "%s: cannot allocate the mapped index-error flag: %s", who, cudaGetErrorString(cudaGetLastError()));
+        }
+        *h->snap_bad = 0ULL;
+        CK(h, cudaFuncSetAttribute(snapshot_save_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   kSnapMaxTileBytes + kThreads * 8));
+        CK(h, cudaFuncSetAttribute(snapshot_load_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   kSnapMaxTileBytes + 2 * kThreads * 8 + 8));
+    }
+    return 0;
+}
+
+static SnapArgs snap_args(b200gym *h, int *tile, int *row_bytes) {
+    const int kind = h->cfg.kind;
+    *row_bytes = snap_row_bytes(kind);
+    *tile = snap_tile(*row_bytes);
+    SnapArgs a;
+    a.rng = reinterpret_cast<uint32_t *>(h->rng);
+    a.state = reinterpret_cast<uint32_t *>(h->state);
+    a.rec = h->lunar_rec;
+    a.elapsed = h->elapsed;
+    a.flags = h->flags;
+    a.n = h->n;
+    a.S2 = 2 * h->S;
+    a.W = snap_record_words(kind);
+    a.chunks = *row_bytes / 16;
+    a.tile_log2 = 0;
+    while ((1 << a.tile_log2) < *tile) a.tile_log2++;
+    a.bad = h->snap_bad_dev;
+    return a;
+}
+
+static int snap_save(b200gym *h, const int64_t *idx, int64_t m, void *snap, cudaStream_t st) {
+    int T, R;
+    const SnapArgs a = snap_args(h, &T, &R);
+    const unsigned grid = (unsigned)((m + T - 1) / T);
+    snapshot_save_kernel<<<grid, kThreads, (size_t)T * R + T * 8, st>>>(a, idx, m, (unsigned char *)snap);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+static int snap_load(b200gym *h, const void *snap, int64_t snap_rows, const int64_t *row, const int64_t *dst, int64_t m,
+                     cudaStream_t st) {
+    int T, R;
+    const SnapArgs a = snap_args(h, &T, &R);
+    const unsigned grid = (unsigned)((m + T - 1) / T);
+    snapshot_load_kernel<<<grid, kThreads, (size_t)T * R + 2 * T * 8 + 8, st>>>(a, (const unsigned char *)snap, snap_rows,
+                                                                              row, dst, m);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+static int snap_check_ptr(b200gym *h, const void *snap, const char *who) {
+    if (!snap) return fail(h, "%s: null snapshot pointer", who);
+    if ((uintptr_t)snap % 128 != 0) return fail(h, "%s: the snapshot base must be 128-byte aligned", who);
+    return 0;
+}
+
+extern "C" int b200gym_snapshot_save(b200gym_t *h, const int64_t *idx_dev, int64_t m, void *snap_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_snapshot_save: null handle");
+    if (m < 0 || (!idx_dev && m > h->n)) return fail(h, "b200gym_snapshot_save: bad row count %lld", (long long)m);
+    if (m == 0) return 0;
+    if (snap_check_ptr(h, snap_dev, "b200gym_snapshot_save")) return 1;
+    DeviceGuard guard(h->device);
+    if (snap_prepare(h, "b200gym_snapshot_save")) return 1;
+    return snap_save(h, idx_dev, m, snap_dev, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_snapshot_load(b200gym_t *h, const void *snap_dev, const int64_t *row_dev, const int64_t *dst_dev,
+                                     int64_t m, void *stream) {
+    if (!h) return fail(h, "b200gym_snapshot_load: null handle");
+    if (m < 0 || (!dst_dev && m > h->n)) return fail(h, "b200gym_snapshot_load: bad row count %lld", (long long)m);
+    if (m == 0) return 0;
+    if (snap_check_ptr(h, snap_dev, "b200gym_snapshot_load")) return 1;
+    DeviceGuard guard(h->device);
+    if (snap_prepare(h, "b200gym_snapshot_load")) return 1;
+    // the snapshot holds m rows (row_dev indexes into them)
+    return snap_load(h, snap_dev, m, row_dev, dst_dev, m, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_clone(b200gym_t *h, const int64_t *src_dev, void *stream) {
+    if (!h || !src_dev) return fail(h, "b200gym_clone: null argument");
+    DeviceGuard guard(h->device);
+    if (snap_prepare(h, "b200gym_clone")) return 1;
+    if (!h->snap_scratch) CK(h, cudaMalloc((void **)&h->snap_scratch, (size_t)h->n * snap_row_bytes(h->cfg.kind)));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (snap_save(h, nullptr, h->n, h->snap_scratch, st)) return 1;
+    return snap_load(h, h->snap_scratch, h->n, src_dev, nullptr, h->n, st);
+}
+
+extern "C" int b200gym_snapshot_index_error(b200gym_t *h) {
+    if (!h) return -1;
+    if (!h->snap_bad || *(volatile unsigned long long *)h->snap_bad == 0ULL) return 0;
+    *(volatile unsigned long long *)h->snap_bad = 0ULL;
+    return 1;
 }

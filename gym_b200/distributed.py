@@ -183,5 +183,19 @@ class ShardedVectorEnv:
         g = self._finish()
         return g["obs"], g["reward"], g["terminated"], g["truncated"], infos
 
+    def _no_snapshots(self, what):
+        from gym_b200 import error
+        raise error.Error(f"ShardedVectorEnv does not support {what}(): its gathered global results would be stale "
+                          "after a restore or clone")
+
+    def snapshot(self, indices=None):
+        self._no_snapshots("snapshot")
+
+    def restore(self, snap, indices=None):
+        self._no_snapshots("restore")
+
+    def clone(self, src):
+        self._no_snapshots("clone")
+
     def close(self):
         self.env.close()

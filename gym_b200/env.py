@@ -12,7 +12,7 @@ single-env agents run unchanged; the throughput path is ``B200VectorEnv``.
 import numpy as np
 
 from gym_b200 import _lib, error
-from gym_b200.vector_env import B200VectorEnv
+from gym_b200.vector_env import B200VectorEnv, _unpickle
 
 
 class B200Env:
@@ -58,6 +58,37 @@ class B200Env:
     @property
     def unwrapped(self):
         return self
+
+    @property
+    def device(self):
+        return self._vec.device
+
+    # pickle / deepcopy carry the whole env state (B200VectorEnv.snapshot): the copy continues bit-identically
+    _pickle_factory = None
+
+    def _rebuild_args(self):
+        v = self._vec
+        kw = v._rebuild_env_kwargs()
+        kw.update(max_episode_steps=v.max_episode_steps or 0, autoreset=self._autoreset, device=v.device.index)
+        return (v.spec,), kw   # self.spec may be gym's own EnvSpec (gym.make replaces it)
+
+    def _load_snapshot_payload(self, snap, seeded, has_reset):
+        self._vec._load_snapshot_payload(snap, seeded, has_reset)
+
+    def __reduce__(self):
+        v = self._vec
+        v._assert_open("pickle")
+        args, kwargs = self._rebuild_args()
+        payload = (v.snapshot().state_dict(), v._seeded, v._has_reset)
+        return _unpickle, (type(self)._pickle_factory or type(self), args, kwargs, payload)
+
+    def __deepcopy__(self, memo):
+        v = self._vec
+        v._assert_open("deepcopy")
+        args, kwargs = self._rebuild_args()
+        new = (type(self)._pickle_factory or type(self))(*args, **kwargs)
+        new._load_snapshot_payload(v.snapshot(), v._seeded, v._has_reset)
+        return new
 
     @property
     def _max_episode_steps(self):

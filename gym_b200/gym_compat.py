@@ -16,6 +16,8 @@ DEVICE, so it shows exactly where the env's own stream is.
 
 The classes are created on first use (``import gym`` happens here, not at ``import gym_b200``).
 """
+import sys
+
 import numpy as np
 
 _cache = {}
@@ -86,6 +88,10 @@ def classes():
             # (re)seeded by reset(seed=...) itself
             pass
 
+    # pickle finds the classes through these module-level constructors (the classes themselves are built here)
+    module = sys.modules[__name__]
+    GymEnv._pickle_factory = staticmethod(module.GymEnv)
+    GymVectorEnv._pickle_factory = staticmethod(module.GymVectorEnv)
     _cache["classes"] = (GymEnv, GymVectorEnv)
     return _cache["classes"]
 

@@ -30,6 +30,7 @@ import numpy as np
 
 from gym_b200 import _lib, envs as _envs, error
 from gym_b200.registration import spec as _spec
+from gym_b200.snapshot import FORMAT_VERSION, EnvSnapshot, check_compatible, env_config, host_indices
 from gym_b200.spaces import batch_space
 
 _STATE_DEFAULT, _STATE_WAITING_RESET, _STATE_WAITING_STEP = "default", "reset", "step"
@@ -48,6 +49,14 @@ def seed_words(seed):
     if seed >= 1 << 128:
         raise error.Error("gym_b200 supports seeds below 2**128")
     return (ctypes.c_uint32 * 4)(*[(seed >> (32 * k)) & 0xFFFFFFFF for k in range(4)])
+
+
+def _unpickle(factory, args, kwargs, payload):
+    """Rebuild an env pickled by ``B200VectorEnv.__reduce__`` / ``B200Env.__reduce__`` and load its snapshot."""
+    env = factory(*args, **kwargs)
+    state, seeded, has_reset = payload
+    env._load_snapshot_payload(EnvSnapshot.from_state_dict(state, env.device), seeded, has_reset)
+    return env
 
 
 class FinalInfos(dict):
@@ -161,6 +170,8 @@ class B200VectorEnv:
         self._lib = lib
         self._handle = handle
         self.autoreset = bool(autoreset)
+        self._params, self._cfg_flags = list(params), cfg_flags
+        self._obs_dev = None
         if cfg_flags & _lib.LUNAR_ENABLE_WIND:
             # LunarLander.__init__ draws wind_idx, then torque_idx, from numpy's GLOBAL generator, once per env
             # object (lunar_lander.py:234-235); SyncVectorEnv builds the objects in index order.  `wind_idx=` /
@@ -353,6 +364,7 @@ class B200VectorEnv:
             # at the next call (no synchronisation unless the flag is up)
             if self.discrete and self._lib.b200gym_invalid_seen(self._handle) == 1:
                 self.check_actions()
+            self._raise_snapshot_index_error()
             act, code = self._device_actions(actions)
             self._flip ^= 1
             out = self._out[self._flip]
@@ -520,6 +532,184 @@ class B200VectorEnv:
             self._seeded = True
         if state is not None:
             self._has_reset = True
+
+    # ------------------------------------------------------------------ snapshots
+    # What pickle / deepcopy carry for a reference env (env.state, np_random, TimeLimit._elapsed_steps), taken for
+    # any subset of the batch, on the device (include/b200gym.h: b200gym_snapshot_*, b200gym_clone).
+    @property
+    def snapshot_row_bytes(self):
+        return int(self._lib.b200gym_snapshot_row_bytes(self.kind))
+
+    def _snapshot_header(self):
+        return {"version": FORMAT_VERSION, "kind": self.kind, "row_bytes": self.snapshot_row_bytes,
+                "config": env_config(self.max_episode_steps, self.autoreset, self._params, self._cfg_flags)}
+
+    def _raise_snapshot_index_error(self):
+        if self._lib.b200gym_snapshot_index_error(self._handle) == 1:
+            raise error.Error("an earlier snapshot(), restore() or clone() was given an out-of-range index; "
+                              "those entries were skipped")
+
+    def _index_tensor(self, indices, what):
+        """None -> None; a CUDA tensor -> int64 on this device (range-checked by the kernels, reported by the next
+        call); anything else -> checked on the host, then copied to the device."""
+        if indices is None:
+            return None
+        torch = _torch()
+        if isinstance(indices, torch.Tensor) and indices.is_cuda:
+            if indices.dim() != 1 or indices.dtype.is_floating_point or indices.dtype == torch.bool:
+                raise error.Error(f"{what} must be a 1-D integer tensor, got {indices.dtype} of shape "
+                                  f"{tuple(indices.shape)}")
+            return indices.to(device=self.device, dtype=torch.int64).contiguous()
+        if isinstance(indices, torch.Tensor):
+            indices = indices.numpy()
+        return torch.from_numpy(host_indices(indices, self.num_envs, what)).to(self.device)
+
+    def _in_range(self, idx, fallback):
+        """idx with every out-of-range entry replaced by `fallback`'s: torch indexing must never see one."""
+        torch = _torch()
+        return torch.where((idx >= 0) & (idx < self.num_envs), idx, fallback)
+
+    def _last_obs(self):
+        """Device tensor (N, D) of the observations last returned (numpy backend: a view of the mapped staging
+        buffer, written by the device without a host copy)."""
+        if self.backend == "torch":
+            return self._out[self._flip]["obs"]
+        if self._obs_dev is None:
+            from gym_b200.distributed import _DeviceMemory
+            h = self._hio["obs"]   # page-locked and mapped: under unified addressing its host address is its device one
+            self._obs_dev = _torch().as_tensor(_DeviceMemory(h.ctypes.data, h.shape, "<f4"), device=self.device)
+        return self._obs_dev
+
+    def _next_obs(self):
+        """Where restored / cloned observations go: the next set of the double buffer (the step-(t+2) rule holds),
+        or the staging buffer on the numpy backend."""
+        if self.backend == "torch":
+            self._flip ^= 1
+            return self._out[self._flip]["obs"]
+        return self._last_obs()
+
+    def _obs_result(self, obs):
+        if self.backend == "torch":
+            return obs.clone() if self.copy else obs
+        _torch().cuda.current_stream(self.device).synchronize()
+        self._raise_snapshot_index_error()
+        obs = self._hio["obs"]
+        return obs.copy() if self.copy else obs
+
+    def _check_idle(self, what):
+        self._assert_open(what)
+        if self._state != _STATE_DEFAULT:
+            raise error.AlreadyPendingCallError(f"Calling `{what}` while waiting for a pending call to `{self._state}` "
+                                                "to complete", self._state)
+        self._raise_snapshot_index_error()
+
+    def snapshot(self, indices=None):
+        """-> ``EnvSnapshot`` of envs ``indices`` (default: all, in order): their engine state as device rows, the
+        observations last returned for them and a header (format version, kind, row bytes, construction config)."""
+        self._check_idle("snapshot")
+        torch = _torch()
+        idx = self._index_tensor(indices, "snapshot indices")
+        m = self.num_envs if idx is None else int(idx.shape[0])
+        rows = torch.empty((m, self.snapshot_row_bytes), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            if m:
+                _lib.check(self._lib.b200gym_snapshot_save(
+                    self._handle, None if idx is None else ctypes.c_void_p(idx.data_ptr()), m,
+                    ctypes.c_void_p(rows.data_ptr()), self._stream()), self._handle)
+            obs = self._last_obs()
+            obs = obs.clone() if idx is None else obs.index_select(0, self._in_range(idx, 0))
+        if self.backend == "numpy":
+            torch.cuda.current_stream(self.device).synchronize()
+            self._raise_snapshot_index_error()
+        return EnvSnapshot(self._snapshot_header(), rows, obs)
+
+    def restore(self, snap, indices=None):
+        """Load ``snap`` (row k into env ``indices[k]``; default: all envs, in order) -> ``(obs, {})`` like ``reset``,
+        with the observations the snapshot was taken with.  The other envs are left as they are.  A snapshot of
+        another kind or construction config raises ``error.Error``."""
+        self._check_idle("restore")
+        check_compatible(snap.header, self.kind, self.snapshot_row_bytes,
+                         env_config(self.max_episode_steps, self.autoreset, self._params, self._cfg_flags))
+        torch = _torch()
+        m, n = len(snap), self.num_envs
+        idx = self._index_tensor(indices, "restore indices")
+        if idx is None and m != n:
+            raise error.Error(f"a snapshot of {m} envs restores into {n} envs only with indices=")
+        if idx is not None and int(idx.shape[0]) != m:
+            raise error.Error(f"{int(idx.shape[0])} indices given for a snapshot of {m} envs")
+        rows, sobs = snap.rows.to(self.device), snap.obs.to(self.device)
+        with torch.cuda.device(self.device):
+            if m:
+                _lib.check(self._lib.b200gym_snapshot_load(
+                    self._handle, ctypes.c_void_p(rows.data_ptr()), None,
+                    None if idx is None else ctypes.c_void_p(idx.data_ptr()), m, self._stream()), self._handle)
+            prev = self._last_obs()
+            target = self._next_obs()
+            if idx is None:
+                target.copy_(sobs)
+            else:   # row n of the scratch takes the observations of skipped (out-of-range) entries
+                tmp = torch.empty((n + 1, self.obs_dim), dtype=torch.float32, device=self.device)
+                tmp[:n].copy_(prev)
+                tmp.index_copy_(0, self._in_range(idx, n), sobs)
+                target.copy_(tmp[:n])
+        if idx is None:
+            self._has_reset = self._seeded = True
+        return self._obs_result(target), {}
+
+    def clone(self, src):
+        """Env i becomes a copy of env ``src[i]`` for every i (duplicates allowed), on the device -> the new
+        observations, gathered from the last ones."""
+        self._check_idle("clone")
+        torch = _torch()
+        src = self._index_tensor(src, "clone sources")
+        if src is None or int(src.shape[0]) != self.num_envs:
+            raise error.Error(f"clone needs one source per env ({self.num_envs})")
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.b200gym_clone(self._handle, ctypes.c_void_p(src.data_ptr()), self._stream()),
+                       self._handle)
+            g = self._in_range(src, torch.arange(self.num_envs, device=self.device))   # a skipped env keeps its obs
+            prev = self._last_obs()
+            target = self._next_obs()
+            if target is prev:
+                target.copy_(prev.index_select(0, g))
+            else:
+                torch.index_select(prev, 0, g, out=target)
+        return self._obs_result(target)
+
+    # ------------------------------------------------------------------ pickle / deepcopy
+    _pickle_factory = None   # module-level callable that rebuilds this class (gym_compat's classes are built at run time)
+
+    def _rebuild_env_kwargs(self):
+        kw = dict(self.env_kwargs)
+        if self._cfg_flags & _lib.LUNAR_ENABLE_WIND:
+            kw.update(wind_idx=0, torque_idx=0)   # the counters come back with the rows: no draw from numpy's generator
+        return kw
+
+    def _rebuild_args(self):
+        kw = self._rebuild_env_kwargs()
+        kw.update(device=self.device.index, max_episode_steps=self.max_episode_steps or 0, backend=self.backend,
+                  copy=self.copy, first_index=self.first_index, autoreset=self.autoreset, dense_infos=self.dense_infos)
+        return (self.spec, self.num_envs), kw
+
+    def _load_snapshot_payload(self, snap, seeded, has_reset):
+        self.restore(snap)
+        self._seeded, self._has_reset = seeded, has_reset
+
+    def __reduce__(self):
+        """pickle: the constructor arguments + a host copy of the whole snapshot; unpickling rebuilds the handle on
+        the same device index and loads the rows, so the copy continues bit-identically."""
+        self._assert_open("pickle")
+        args, kwargs = self._rebuild_args()
+        payload = (self.snapshot().state_dict(), self._seeded, self._has_reset)
+        return _unpickle, (type(self)._pickle_factory or type(self), args, kwargs, payload)
+
+    def __deepcopy__(self, memo):
+        """A new handle on the same device loaded from a snapshot, device to device."""
+        self._assert_open("deepcopy")
+        args, kwargs = self._rebuild_args()
+        new = (type(self)._pickle_factory or type(self))(*args, **kwargs)
+        new._load_snapshot_payload(self.snapshot(), self._seeded, self._has_reset)
+        return new
 
     # ------------------------------------------------------------------ call / attrs
     def call_async(self, name, *args, **kwargs):

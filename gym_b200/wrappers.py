@@ -44,9 +44,83 @@ class VectorWrapper:
     def close(self, **kwargs):
         return self.env.close(**kwargs)
 
+    # B200VectorEnv.snapshot / restore / clone; a wrapper with per-env or running state extends them through the
+    # hooks below, keeping its part of a snapshot in snap.extras under its own layer key
+    def snapshot(self, indices=None):
+        snap = self.env.snapshot(indices)
+        extra = self._snapshot_extra(self.unwrapped._index_tensor(indices, "snapshot indices"))
+        if extra is not None:
+            snap.extras[self._layer_key()] = extra
+        return snap
+
+    def restore(self, snap, indices=None):
+        obs, info = self.env.restore(snap, indices)
+        key = self._layer_key()
+        if self._has_snapshot_state():
+            if key not in snap.extras:
+                from gym_b200 import error
+                raise error.Error(f"the snapshot carries no state for wrapper layer {key}")
+            self._restore_extra(snap.extras[key], self.unwrapped._index_tensor(indices, "restore indices"))
+        return self._restored_obs(obs), info
+
+    def clone(self, src):
+        import torch
+        obs = self.env.clone(src)
+        u = self.unwrapped
+        src = u._index_tensor(src, "clone sources")
+        self._clone_extra(u._in_range(src, torch.arange(u.num_envs, device=u.device)))
+        return self._restored_obs(obs)
+
+    def _layer_key(self):
+        depth, e = 0, self.env
+        while isinstance(e, VectorWrapper):
+            depth, e = depth + 1, e.env
+        return f"{depth}:{type(self).__name__}"
+
+    def _has_snapshot_state(self):
+        return False
+
+    def _snapshot_extra(self, idx):
+        return None
+
+    def _restore_extra(self, extra, idx):
+        pass
+
+    def _clone_extra(self, src):
+        pass
+
+    def _restored_obs(self, obs):
+        return obs
+
     @property
     def unwrapped(self):
         return self.env.unwrapped
+
+
+def _pick(u, t, idx):
+    """Rows `idx` of a per-env tensor (all rows: idx None); out-of-range entries read row 0."""
+    return t.clone() if idx is None else t.index_select(0, u._in_range(idx, 0))
+
+
+def _scatter(u, t, idx, values):
+    """t[idx] = values for a per-env tensor (all rows: idx None); out-of-range entries land in a scratch row."""
+    import torch
+    if idx is None:
+        t.copy_(values)
+        return
+    tmp = torch.cat([t, t[:1]])
+    tmp.index_copy_(0, u._in_range(idx, u.num_envs), values.to(t.device))
+    t.copy_(tmp[:u.num_envs])
+
+
+def _rms_state(r):
+    return {"stats": r.stats.clone(), "scratch": r.scratch.clone(), "cur": int(r.cur)}
+
+
+def _set_rms_state(r, e):
+    r.stats.copy_(e["stats"])
+    r.scratch.copy_(e["scratch"])
+    r.cur = int(e["cur"])
 
 
 class RecordEpisodeStatistics(VectorWrapper):
@@ -115,6 +189,26 @@ class RecordEpisodeStatistics(VectorWrapper):
         infos["episode"] = {"r": self._ep_r[k], "l": self._ep_l[k], "t": round(time.perf_counter() - self.t0, 6)}
         infos["_episode"] = mask
         return obs, rew, term, trunc, infos
+
+    # snapshots: the per-env accumulators follow the envs, the ring and the counter are saved and restored whole
+    def _has_snapshot_state(self):
+        return True
+
+    def _snapshot_extra(self, idx):
+        u = self.unwrapped
+        return {"episode_returns": _pick(u, self.episode_returns, idx), "episode_lengths": _pick(u, self.episode_lengths, idx),
+                "ring": self._ring.clone(), "counter": self._counter.clone()}
+
+    def _restore_extra(self, e, idx):
+        u = self.unwrapped
+        _scatter(u, self.episode_returns, idx, e["episode_returns"])
+        _scatter(u, self.episode_lengths, idx, e["episode_lengths"])
+        self._ring.copy_(e["ring"])
+        self._counter.copy_(e["counter"])
+
+    def _clone_extra(self, src):
+        self.episode_returns.copy_(self.episode_returns.index_select(0, src))
+        self.episode_lengths.copy_(self.episode_lengths.index_select(0, src))
 
     @property
     def episode_count(self):
@@ -206,7 +300,7 @@ class NormalizeObservation(VectorWrapper):
         self._flip = 0
         self._group, self._world = _shard_group(env, group)
 
-    def _normalize(self, obs):
+    def _normalize(self, obs, update=True):
         torch = self._torch
         self._flip ^= 1
         if self._out[self._flip] is None or self._out[self._flip].shape != obs.shape:
@@ -217,15 +311,31 @@ class NormalizeObservation(VectorWrapper):
         n, d = obs.shape
         st, sc = r.stats[r.cur], r.scratch[r.cur]
         with torch.cuda.device(obs.device):
-            _lib.check(lib.b200gym_rms_moments(_p(obs), 0, n, d, _p(st), _p(sc), env._stream()))
-            if self._group is not None:
-                import torch.distributed as dist
-                dist.all_reduce(sc, group=self._group)
+            if update:
+                _lib.check(lib.b200gym_rms_moments(_p(obs), 0, n, d, _p(st), _p(sc), env._stream()))
+                if self._group is not None:
+                    import torch.distributed as dist
+                    dist.all_reduce(sc, group=self._group)
             _lib.check(lib.b200gym_rms_apply_obs(_p(obs), _p(out), n, d, _p(st), _p(r.stats[r.cur ^ 1]), _p(sc),
-                                                 _p(r.scratch[r.cur ^ 1]), float(n * self._world), self.epsilon, 1,
-                                                 env._stream()))
-        r.cur ^= 1
+                                                 _p(r.scratch[r.cur ^ 1]), float(n * self._world), self.epsilon,
+                                                 1 if update else 0, env._stream()))
+        if update:
+            r.cur ^= 1
         return out
+
+    # snapshots: the statistics are saved and restored whole and left alone by clone; restored / cloned
+    # observations are normalised without updating them
+    def _has_snapshot_state(self):
+        return True
+
+    def _snapshot_extra(self, idx):
+        return _rms_state(self.obs_rms)
+
+    def _restore_extra(self, e, idx):
+        _set_rms_state(self.obs_rms, e)
+
+    def _restored_obs(self, obs):
+        return self._normalize(obs, update=False)
 
     def reset(self, **kwargs):
         obs, info = self.env.reset(**kwargs)
@@ -275,6 +385,27 @@ class NormalizeReward(VectorWrapper):
                                                     float(n * self._world), self.epsilon, env._stream()))
         r.cur ^= 1
         return obs, out, term, trunc, infos
+
+    # snapshots: the per-env discounted returns follow the envs; the statistics are saved and restored whole and
+    # left alone by clone
+    def _has_snapshot_state(self):
+        return True
+
+    def _returns(self):
+        u = self.unwrapped
+        if self.returns is None:
+            self.returns = self._torch.zeros(u.num_envs, dtype=self._torch.float64, device=u.device)
+        return self.returns
+
+    def _snapshot_extra(self, idx):
+        return dict(_rms_state(self.return_rms), returns=_pick(self.unwrapped, self._returns(), idx))
+
+    def _restore_extra(self, e, idx):
+        _set_rms_state(self.return_rms, e)
+        _scatter(self.unwrapped, self._returns(), idx, e["returns"])
+
+    def _clone_extra(self, src):
+        self.returns = self._returns().index_select(0, src)
 
 
 class VectorListInfo(VectorWrapper):

@@ -214,6 +214,36 @@ int b200gym_set_state(b200gym_t *h, const double *state_dev, const int32_t *elap
                       const uint64_t *rng_dev, void *stream);
 
 /*
+ * Env snapshots: save, restore and clone everything the engine owns for an env, on the device.
+ *
+ * Replaces: what pickle and copy.deepcopy carry for a reference env -- `env.state` (e.g. cartpole.py:133,204),
+ * `np_random` (core.py:75-84) and `TimeLimit._elapsed_steps` (time_limit.py:51,67) -- and, for the Box2D kinds,
+ * the whole b2World the reference's EzPickle rebuilds from constructor arguments instead (ezpickle.py).
+ *
+ * A snapshot is an array of rows, one per env, of b200gym_snapshot_row_bytes(kind) bytes (a multiple of 32):
+ * the PCG64 record, float64 state[state_dim], for the Box2D kinds the solver record (bodies, joint impulses,
+ * warm-start slots, terrain, obstacle boxes, wind counters, buffered 32-bit draw), the TimeLimit counter and the
+ * plain-Env "already terminated" flag.  Rows are only meaningful to a handle of the same kind and configuration.
+ * `snap_dev` must be 128-byte aligned.  The calls are asynchronous on `stream` and never synchronise.  An
+ * out-of-range index is skipped (the entry moves nothing; a save writes a zero row) and raises a sticky flag read by
+ * b200gym_snapshot_index_error().
+ */
+int64_t b200gym_snapshot_row_bytes(int kind);   /* host only, like b200gym_obs_dim; -1 for an unknown kind */
+/* env idx_dev[k] (idx_dev NULL: env k) -> row k, for k < m */
+int b200gym_snapshot_save(b200gym_t *h, const int64_t *idx_dev, int64_t m, void *snap_dev, void *stream);
+/* row row_dev[k] -> env dst_dev[k], for k < m; snap_dev holds m rows; either index array may be NULL (= k).
+ * Duplicate envs in dst_dev: which row lands is undefined. */
+int b200gym_snapshot_load(b200gym_t *h, const void *snap_dev, const int64_t *row_dev, const int64_t *dst_dev,
+                          int64_t m, void *stream);
+/* env i <- env src_dev[i] for every i (src_dev: [n] int64), through a handle-owned scratch snapshot of n rows:
+ * save every env, then load rows src_dev[i] into env i -- two coalesced passes instead of one scattered gather. */
+int b200gym_clone(b200gym_t *h, const int64_t *src_dev, void *stream);
+/* 1 when a snapshot kernel of this handle has met an out-of-range index since the last call (and clears the flag),
+ * 0 otherwise, -1 on a null handle.  Never synchronises: the kernels raise the flag in page-locked host memory, so
+ * it shows once they have run. */
+int b200gym_snapshot_index_error(b200gym_t *h);
+
+/*
  * LunarLander only (state_dim is 0 for it; get/set_state handle the TimeLimit counters and RNG):
  * the three rigid bodies {lander, leg(-1), leg(+1)} of every env as float32 [n][18] =
  * 3 x {c.x, c.y, angle, v.x, v.y, omega} and int32 [n][6] = {game_over, leg0 contact, leg1 contact,
