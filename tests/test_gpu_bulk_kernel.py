@@ -18,15 +18,26 @@ def _actions(env_id, rng, T, N):
     return rng.uniform(-lim, lim, size=(T, N, 1)).astype(np.float32)
 
 
-@pytest.mark.parametrize("env_id", ENV_IDS)
-def test_bulk_kernel_equals_simple_kernel(env_id, monkeypatch):
-    """N gives every resident CTA several tiles plus a ragged last tile (kernel A takes it); max_episode_steps=40
-    makes the whole batch truncate in the same step twice -- the dense inline resets, which go through the stage, and
-    the overflow of the deferred-reset list -- and the terminations in between go through the deferred list, whose
-    direct stores must land after the tile's bulk stores.  The action dtype cycles through int64 / int32 / uint8."""
+# (env_id, tiles per SM): 9 gives each resident CTA at most 3 tiles, so no stage of the ring is ever refilled;
+# 49 gives every CTA at least 7 tiles whatever the occupancy (288 threads: at most 7 CTAs per SM), so every one of
+# the kBulkStages stages is refilled and its mbarriers complete a second phase
+CASES = ([pytest.param(e, 9, id=e) for e in ENV_IDS] +
+         [pytest.param(e, 49, id=f"{e}-multi_round") for e in ENV_IDS])
+
+
+@pytest.mark.parametrize("env_id,tiles_per_sm", CASES)
+def test_bulk_kernel_equals_simple_kernel(env_id, tiles_per_sm, monkeypatch):
+    """A ragged last tile (kernel A takes it); max_episode_steps=40 makes the whole batch truncate in the same step
+    twice -- every warp is dense then and resets inline, through the stage -- and the terminations in between go
+    through the deferred list, whose direct stores must land after the tile's bulk stores.  The list never overflows
+    here (test_gpu_launch_shapes.py forces that).  The action dtype cycles through int64 / int32 / uint8.  N stays a
+    multiple of 16 at 49 tiles per SM: otherwise the float32 action rows of odd steps are not 16-byte aligned and
+    kernel P runs instead of B."""
     import torch
     import gym_b200
-    N, T = 132 * 256 * 9 + 178, 90
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    N = 132 * 256 * 9 + 178 if tiles_per_sm == 9 else tiles_per_sm * sms * 256 + 176
+    T = 90
     envs = {}
     for k in ("a", "b"):
         monkeypatch.setenv("B200GYM_KERNEL", k)

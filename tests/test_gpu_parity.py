@@ -309,17 +309,26 @@ def test_state_roundtrip_and_teacher_forcing(oracle_mod):
         orc.close()
 
 
-@pytest.mark.parametrize("env_id", ENV_IDS)
-def test_persistent_kernel_equals_simple_kernel(env_id, monkeypatch):
+# (env_id, tiles per SM): 9 gives each resident CTA two or three tiles; 96 gives every CTA at least 12 whatever the
+# occupancy (256 threads: at most 8 CTAs per SM), so the prefetch slots are refilled many times over
+PERSISTENT_CASES = ([pytest.param(e, 9, id=e) for e in ENV_IDS] +
+                    [pytest.param(e, 96, id=f"{e}-multi_round") for e in ENV_IDS])
+
+
+@pytest.mark.parametrize("env_id,tiles_per_sm", PERSISTENT_CASES)
+def test_persistent_kernel_equals_simple_kernel(env_id, tiles_per_sm, monkeypatch):
     """Kernel P (resident grid, per-thread cp.async prefetch, CTA-deferred resets; the default for large batches)
     against kernel A (one tile per CTA, plain loads): same arithmetic, so every output and the persistent state
     must be bit-identical.  N gives the resident grid several tiles per CTA plus a ragged last tile;
-    max_episode_steps=40 makes the whole batch truncate in the same step twice (the dense inline-reset path and
-    the overflow of the deferred-reset list), the terminations in between go through the deferred list; the
-    action dtype cycles through int64 / int32 / uint8 (uint8 takes the register-prefetch path)."""
+    max_episode_steps=40 makes the whole batch truncate in the same step twice (every warp is dense then and resets
+    inline), the terminations in between go through the deferred list, which never overflows here
+    (test_gpu_launch_shapes.py forces that); the action dtype cycles through int64 / int32 / uint8 (uint8 takes the
+    register-prefetch path)."""
     import gym_b200
     torch = _torch()
-    N, T = 132 * 256 * 9 + 178, 90
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    N = 132 * 256 * 9 + 178 if tiles_per_sm == 9 else tiles_per_sm * sms * 256 + 176
+    T = 90
     envs = {}
     for k in ("a", "p", "l"):   # "l": the lean instantiation of kernel P (32-bit indices, no peer / episode code)
         monkeypatch.setenv("B200GYM_KERNEL", k)
