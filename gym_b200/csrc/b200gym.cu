@@ -61,40 +61,23 @@ struct b200gym {
         unsigned long long *ring = nullptr, *counter = nullptr; int ring_size = 0;
     } ep;
     int sm_count = 132;
-    int occ[B200GYM_NUM_KINDS][3][4] = {};  // cached CTAs/SM of step_kernel_persistent per (kind, action width, lean + 2 * deep)
+    int occ[B200GYM_NUM_KINDS][3][2] = {};  // cached CTAs/SM of step_kernel_persistent per (kind, action width, lean)
     int occ_bulk[B200GYM_NUM_KINDS][3] = {};  // ... of step_kernel_persistent_bulk per (kind, action width)
-    int p_depth = 1;                        // kernel P/L: tiles in flight per thread (B200GYM_P_DEPTH=1|2)
-    int p_ctas = -1;                        // kernel P/L: resident CTAs per SM; -1 = occupancy limit, 0 = balance the tile
-                                            // rounds (see launch_step_typed), k > 0 = exactly k (B200GYM_P_CTAS, tuning runs)
     int kernel_choice = -1;                 // -1: kernel B (bulk copies) where bulk_by_default picks it, else P's lean
                                             // instantiation; 0: kernel A (one tile per CTA), 1: kernel P (resident grid,
                                             // asynchronous prefetch, deferred resets), 2: P's lean instantiation where it
                                             // applies (else P), 3: kernel B where it applies (else lean P);
                                             // B200GYM_KERNEL=a|p|l|b overrides
-    int gather_bulk = 1;                    // multi-GPU step: 1 = kernel G (staged tile + bulk pushes), 0 = per-thread
-                                            // peer stores from kernel A; B200GYM_GATHER=bulk|direct overrides
-    int block_a = 256;                      // CTA size of kernel A (B200GYM_BLOCK_A=64|128|256, tuning runs)
-    int box2d_block = 128;                  // LunarLander step kernel: CTA size (B200GYM_BOX2D_BLOCK=128|256, tuning runs)
     int box2d_defer = 1;                    // Box2D tasks: 1 = the autoresets of a step run in a last, compacted kernel
                                             // (B200GYM_BOX2D_DEFER=0: inline).  With the TOI kernel it takes reset() +
                                             // its embedded world step off the critical path of the envs that crash in a
                                             // TOI sub-step (H100 80GB HBM3 at 400 W, 2^16 envs, cold-L2 median:
                                             // LunarLander 1.82 -> 1.77 ms, BipedalWalker 9.16 -> 8.24 ms per step)
-    int box2d_split = 0;                    // Box2D tasks: 1 = the step kernel's resets overlap the TOI kernel on a side stream
-                                            // (B200GYM_BOX2D_SPLIT=1).  Measured neutral on the same H100 (LunarLander
-                                            // 1.78 vs 1.77 ms, BipedalWalker 8.26 vs 8.24): the envs that end an
-                                            // episode are mostly the parked ones, whose resets can only follow the TOI kernel -- so the plain sequence is
-                                            // the default
-    int toi_grid = 12;                      // TOI kernel: one-warp CTAs per SM (B200GYM_TOI_GRID, tuning runs)
     int box2d_toi_defer = 1;                // Box2D tasks: 1 = envs with a possible TOI event finish in the compacted TOI kernel
                                             // (B200GYM_BOX2D_TOI_DEFER=0: SolveTOI inline in the step kernel)
     int32_t *toi_list = nullptr;            // [n] env offsets parked for the TOI kernel, per launch range
     int32_t *toi_count = nullptr;           // [kResetSlots]
     uint32_t *toi_mid = nullptr;            // [kToiMidWords][n] SoA side buffer of the parked envs
-    int32_t *reset_list2 = nullptr;         // [n] / [kResetSlots]: the resets of the TOI kernel (its own list, so that the
-    int32_t *reset_count2 = nullptr;        // step kernel's resets can run on the side stream while the TOI kernel runs)
-    cudaStream_t side = nullptr;            // Box2D tasks: side stream of the step-kernel resets (fork / join by events)
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     int32_t *reset_list = nullptr;          // [n] env offsets to reset, filled per launch range
     int32_t *reset_count = nullptr;         // [kResetSlots] one counter per concurrently running launch range
     // fused all-gather over peer memory (b200gym_p2p_*)
@@ -524,7 +507,6 @@ __device__ __forceinline__ void ld_async(void *smem_dst, const void *gmem_src) {
 }
 __device__ __forceinline__ void ld_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void ld_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void ld_wait_all_but_one() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 
 // bulk (TMA, SASS UBLKCP) shared -> global store of a contiguous block; works on peer-mapped addresses
 __device__ __forceinline__ void st_bulk(void *gmem_dst, const void *smem_src, uint32_t bytes) {
@@ -607,16 +589,14 @@ struct PrefetchLayout {
 // LEAN (the single-GPU step without the fused RecordEpisodeStatistics, fewer than 2^31 envs): 32-bit env indices
 // (one IMAD.WIDE per address instead of a 64-bit add chain), no per-peer store loops, no episode accounting --
 // same arithmetic, same stores, fewer issue slots.
-template <int KIND, typename ActT, bool LEAN, int DEPTH>
+template <int KIND, typename ActT, bool LEAN>
 __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_persistent(const StepArgs a, const int num_tiles) {
     using E = Env<KIND>;
     using L = PrefetchLayout<KIND, ActT>;
     using Idx = typename std::conditional<LEAN, uint32_t, int64_t>::type;
-    static_assert(DEPTH == 1 || DEPTH == 2, "one or two tiles in flight per thread");
-    // DEPTH stages of per-thread input slots: the tile being advanced + DEPTH tiles in flight behind it would need
-    // DEPTH + 1 stages if a slot were still in use while its refill is issued; it is not -- a thread moves its slot
-    // into registers before it refills it -- so DEPTH stages hold DEPTH tiles in flight
-    __shared__ __align__(16) unsigned char in_mem[DEPTH * L::kBytes];
+    // one stage of per-thread input slots holds the next tile in flight: a thread moves its slot into registers
+    // before it refills it
+    __shared__ __align__(16) unsigned char in_mem[L::kBytes];
     __shared__ int reset_list[kResetCap];
     __shared__ int reset_count;
     const int tid = threadIdx.x;
@@ -627,10 +607,9 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
     const DirectSinkT<!LEAN> sink{a};
     const Idx first = (Idx)a.first, count = (Idx)a.count;
 
-    auto prefetch = [&](int tile, int stage) {
-        unsigned char *base = in_mem + stage * L::kBytes;
-        double *s_state = reinterpret_cast<double *>(base + L::kStateOff);
-        int32_t *s_elapsed = reinterpret_cast<int32_t *>(base + L::kElapsedOff);
+    auto prefetch = [&](int tile) {
+        double *s_state = reinterpret_cast<double *>(in_mem + L::kStateOff);
+        int32_t *s_elapsed = reinterpret_cast<int32_t *>(in_mem + L::kElapsedOff);
         const Idx j = (Idx)tile * kThreads + tid;
         if (tile < num_tiles && j < count) {
             const Idx i = first + j;
@@ -638,32 +617,28 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
             for (int k = 0; k < E::S; k++) acp::ld_async<8>(s_state + k * kThreads + tid, a.state + k * a.n + i);
             acp::ld_async<4>(s_elapsed + tid, a.elapsed + i);
             if constexpr (L::kActAsync)
-                acp::ld_async<L::kActBytes>(base + L::kActOff + tid * L::kActBytes, actions + (size_t)i * L::kActPerEnv);
+                acp::ld_async<L::kActBytes>(in_mem + L::kActOff + tid * L::kActBytes, actions + (size_t)i * L::kActPerEnv);
         }
-        acp::ld_commit();   // always one group per call: the wait below counts groups
+        acp::ld_commit();
     };
 
     int tile = blockIdx.x;
-    prefetch(tile, 0);
-    if constexpr (DEPTH == 2) prefetch(tile + (int)gridDim.x, 1);
-    int stage = 0;
+    prefetch(tile);
     for (; tile < num_tiles; tile += gridDim.x) {
         const Idx j = (Idx)tile * kThreads + tid;
         const bool in_range = j < count;
         const Idx i = first + j;
         ActT av{};
         if constexpr (!L::kActAsync) { if (in_range) av = __ldg(actions + (size_t)i * L::kActPerEnv); }
-        if constexpr (DEPTH == 2) acp::ld_wait_all_but_one(); else acp::ld_wait_all();
-        unsigned char *base = in_mem + stage * L::kBytes;
-        const double *s_state = reinterpret_cast<const double *>(base + L::kStateOff);
+        acp::ld_wait_all();
+        const double *s_state = reinterpret_cast<const double *>(in_mem + L::kStateOff);
         double s[E::S];
 #pragma unroll
         for (int k = 0; k < E::S; k++) s[k] = s_state[k * kThreads + tid];
-        const int32_t elapsed = reinterpret_cast<const int32_t *>(base + L::kElapsedOff)[tid];
-        if constexpr (L::kActAsync) av = *reinterpret_cast<const ActT *>(base + L::kActOff + tid * L::kActBytes);
-        // this thread's slots are in registers now: refill them with its env DEPTH tiles ahead
-        prefetch(tile + DEPTH * (int)gridDim.x, stage);
-        if constexpr (DEPTH == 2) stage ^= 1;
+        const int32_t elapsed = reinterpret_cast<const int32_t *>(in_mem + L::kElapsedOff)[tid];
+        if constexpr (L::kActAsync) av = *reinterpret_cast<const ActT *>(in_mem + L::kActOff + tid * L::kActBytes);
+        // this thread's slots are in registers now: refill them with its env of the next round
+        prefetch(tile + (int)gridDim.x);
         long long action_int = 0;
         float a0 = 0.0f;
         if constexpr (E::A == 0) action_int = (long long)av;
@@ -1124,7 +1099,15 @@ __global__ void __launch_bounds__(kThreads) snapshot_load_kernel(const SnapArgs 
 constexpr int kLunarThreads = 128;
 constexpr int kResetSlots = 64;   // launch ranges of one handle that may be in flight at once (host path: <= 64 chunks)
 
-constexpr int kLunarMaxThreads = 256;
+// lunar_step_kernel runs 128-thread CTAs, but its launch bounds name 256 threads x 2 CTAs: that caps it at 128
+// registers, the budget every LunarLander number in DESIGN §4.4 was measured under
+constexpr int kLunarRegCapThreads = 256;
+
+// TOI kernels: one warp per CTA, 12 CTAs per SM (what is resident with the 156-register kernel); the kernel strides over
+// the list.  Larger grids (fewer envs per warp) are slower (H100 80GB HBM3 at 400 W, 2^16 envs, cold-L2 median):
+// LunarLander 1.77 / 1.86 / 1.90 ms at 12 / 64 / 256 CTAs per SM, BipedalWalker (nearly every env parked)
+// 8.24 / 11.5 / 16.0 ms
+constexpr int kToiCtasPerSm = 12;
 
 // The TOI kernels run one warp per CTA and give each warp as FEW parked envs as the resident grid allows: the lanes
 // of a warp diverge completely in this code (different contact lists, GJK / root-finder trip counts, event counts),
@@ -1164,6 +1147,22 @@ __device__ __forceinline__ void lunar_load_mid(const StepArgs &a, int64_t i, lun
     mid.awake = true;   // only awake islands are parked
 }
 
+// reset() of env i in place: record, RNG and TimeLimit counter; the new observation goes to obs.  The arrays and n
+// are taken by reference, so that lunar_reset_list_kernel reads them from its parameter block where they are used;
+// taken by value they are loaded up front, and the compiler allocates and schedules that kernel differently.
+__device__ __forceinline__ void lunar_reset_env(uint32_t *const &rec, int32_t *const &elapsed, uint64_t *const &rng,
+                                                const int64_t &n, int64_t i, const lunar::Opts &O, float (&obs)[8]) {
+    lunar::World W;
+    W.flags = rec[(int64_t)lunar::W_FLAGS * n + i] & b2l::kFlagsKept;  // the b2World object survives reset()
+    W.wind_idx = O.wind ? (int32_t)rec[(int64_t)lunar::W_WIND * n + i] : 0;          // so do wind_idx / torque_idx
+    W.torque_idx = O.wind ? (int32_t)rec[(int64_t)(lunar::W_WIND + 1) * n + i] : 0;
+    Pcg64 g = pcg64_load(rng + 4 * i);
+    lunar::env_reset(W, g, O, obs);
+    lunar::store_world(W, rec, n, i, O.wind != 0);
+    pcg64_store(rng + 4 * i, g);
+    elapsed[i] = 0;
+}
+
 // everything after world.Step of LunarLander.step, then TimeLimit, outputs and the same-step autoreset
 __device__ __noinline__ void lunar_finish(const StepArgs &a, int64_t i, int64_t j, lunar::World &W, Pcg64 &g, int32_t elapsed,
                                           const lunar::Mid &mid) {
@@ -1194,7 +1193,7 @@ __device__ __noinline__ void lunar_finish(const StepArgs &a, int64_t i, int64_t 
 }
 
 template <typename ActT, bool CONT>
-__global__ void __launch_bounds__(kLunarMaxThreads, 2) lunar_step_kernel(const StepArgs a) {
+__global__ void __launch_bounds__(kLunarRegCapThreads, 2) lunar_step_kernel(const StepArgs a) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool in_range = j < a.count;
     const int64_t i = a.first + j;
@@ -1269,19 +1268,10 @@ __global__ void __launch_bounds__(32) lunar_toi_kernel(const StepArgs a) {
 // stream as the inline path.
 __global__ void __launch_bounds__(kLunarThreads) lunar_reset_list_kernel(const StepArgs a) {
     const int cnt = *a.reset_count;
-    const lunar::Opts &O = a.lunar_opts;
     for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < cnt; idx += gridDim.x * blockDim.x) {
         const int64_t i = a.first + a.reset_list[a.first + idx];
-        lunar::World W;
-        W.flags = a.lunar_rec[(int64_t)lunar::W_FLAGS * a.n + i] & b2l::kFlagsKept;
-        W.wind_idx = O.wind ? (int32_t)a.lunar_rec[(int64_t)lunar::W_WIND * a.n + i] : 0;
-        W.torque_idx = O.wind ? (int32_t)a.lunar_rec[(int64_t)(lunar::W_WIND + 1) * a.n + i] : 0;
-        Pcg64 g = pcg64_load(a.rng + 4 * i);
         float obs[8];
-        lunar::env_reset(W, g, O, obs);
-        lunar::store_world(W, a.lunar_rec, a.n, i, O.wind != 0);
-        pcg64_store(a.rng + 4 * i, g);
-        a.elapsed[i] = 0;
+        lunar_reset_env(a.lunar_rec, a.elapsed, a.rng, a.n, i, a.lunar_opts, obs);
         store_obs_all<8>(a, i, obs);
     }
 }
@@ -1292,16 +1282,8 @@ __global__ void __launch_bounds__(kLunarThreads) lunar_reset_kernel(uint32_t *re
     const int64_t i = (int64_t)blockIdx.x * kLunarThreads + threadIdx.x;
     if (i >= n) return;
     if (mask && !mask[i]) return;
-    lunar::World W;
-    W.flags = rec[(int64_t)lunar::W_FLAGS * n + i] & b2l::kFlagsKept;  // the b2World object survives reset()
-    W.wind_idx = O.wind ? (int32_t)rec[(int64_t)lunar::W_WIND * n + i] : 0;          // so do wind_idx / torque_idx
-    W.torque_idx = O.wind ? (int32_t)rec[(int64_t)(lunar::W_WIND + 1) * n + i] : 0;
-    Pcg64 g = pcg64_load(rng + 4 * i);
     float o[8];
-    lunar::env_reset(W, g, O, o);
-    lunar::store_world(W, rec, n, i, O.wind != 0);
-    pcg64_store(rng + 4 * i, g);
-    elapsed[i] = 0;
+    lunar_reset_env(rec, elapsed, rng, n, i, O, o);
     if (obs) store_row<8>(obs, i, o);
 }
 
@@ -1340,6 +1322,44 @@ static int lunar_upload_consts(b200gym *h) {
 }
 
 // ---- BipedalWalker-v3 (walker.cuh): one thread per env --------------------------------------------
+// side buffer of a parked env: the sweep starts of the bodies
+__device__ __forceinline__ void walker_store_mid(const StepArgs &a, int64_t i, const walker::World &W) {
+    uint32_t *m = a.toi_mid + i;
+    for (int b = 0; b < walker::NB; b++) {
+        m[(int64_t)(3 * b + 0) * a.n] = __float_as_uint(W.b[b].c0.x);
+        m[(int64_t)(3 * b + 1) * a.n] = __float_as_uint(W.b[b].c0.y);
+        m[(int64_t)(3 * b + 2) * a.n] = __float_as_uint(W.b[b].a0);
+    }
+}
+
+__device__ __forceinline__ void walker_load_mid(const StepArgs &a, int64_t i, walker::World &W) {
+    const uint32_t *m = a.toi_mid + i;
+    for (int b = 0; b < walker::NB; b++) {
+        W.b[b].c0.x = __uint_as_float(m[(int64_t)(3 * b + 0) * a.n]);
+        W.b[b].c0.y = __uint_as_float(m[(int64_t)(3 * b + 1) * a.n]);
+        W.b[b].a0 = __uint_as_float(m[(int64_t)(3 * b + 2) * a.n]);
+    }
+}
+
+// reset() of env i in place: record (with the buffered 32-bit draw), RNG and TimeLimit counter; the new observation
+// goes to obs.  References as in lunar_reset_env.
+template <bool HC>
+__device__ __forceinline__ void walker_reset_env(uint32_t *const &rec, int32_t *const &elapsed, uint64_t *const &rng,
+                                                 const int64_t &n, int64_t i, float (&obs)[24]) {
+    walker::World W;
+    walker::Rng r;
+    walker::bind_world(W, rec, n, i);
+    W.flags = rec[(int64_t)walker::W_FLAGS * n + i] & b2l::kFlagsKept;  // the b2World object survives reset()
+    r.has32 = rec[(int64_t)walker::W_RNG32 * n + i];
+    r.val32 = rec[(int64_t)(walker::W_RNG32 + 1) * n + i];
+    r.g = pcg64_load(rng + 4 * i);
+    W.np = 0; W.p_lo = 0; W.p_hi = -1;
+    walker::env_reset<HC>(W, r, obs);
+    walker::store_world(W, rec, n, i, r, HC);
+    pcg64_store(rng + 4 * i, r.g);
+    elapsed[i] = 0;
+}
+
 // everything after world.Step of BipedalWalker.step, then TimeLimit, outputs and the same-step autoreset
 template <bool HC>
 __device__ __noinline__ void walker_finish(const StepArgs &a, int64_t i, int64_t j, walker::World &W, walker::Rng &rng,
@@ -1386,12 +1406,7 @@ __global__ void __launch_bounds__(kLunarThreads, 4) walker_step_kernel(const Ste
     if (awake && b2l::toi_needed<walker::SceneT<HC>>(W)) {
         if (a.toi_list) {   // park the env for walker_toi_kernel: the record after the discrete solve + the sweep starts
             walker::store_world(W, a.lunar_rec, a.n, i, rng, HC);
-            uint32_t *m = a.toi_mid + i;
-            for (int b = 0; b < walker::NB; b++) {
-                m[(int64_t)(3 * b + 0) * a.n] = __float_as_uint(W.b[b].c0.x);
-                m[(int64_t)(3 * b + 1) * a.n] = __float_as_uint(W.b[b].c0.y);
-                m[(int64_t)(3 * b + 2) * a.n] = __float_as_uint(W.b[b].a0);
-            }
+            walker_store_mid(a, i, W);
             a.toi_list[a.first + atomicAdd(a.toi_count, 1)] = (int32_t)j;
             return;
         }
@@ -1417,12 +1432,7 @@ __global__ void __launch_bounds__(32) walker_toi_kernel(const StepArgs a) {
             walker::World W;
             walker::Rng rng;
             walker::load_world(W, a.lunar_rec, a.n, i, rng, HC);
-            const uint32_t *m = a.toi_mid + i;
-            for (int b = 0; b < walker::NB; b++) {
-                W.b[b].c0.x = __uint_as_float(m[(int64_t)(3 * b + 0) * a.n]);
-                W.b[b].c0.y = __uint_as_float(m[(int64_t)(3 * b + 1) * a.n]);
-                W.b[b].a0 = __uint_as_float(m[(int64_t)(3 * b + 2) * a.n]);
-            }
+            walker_load_mid(a, i, W);
             // the window of obstacle boxes env_pre computed around the hull's position before the step
             if constexpr (HC) walker::poly_window(W, W.b[0].c0.x - 4.0f, W.b[0].c0.x + 4.0f, W.p_lo, W.p_hi);
             const int32_t elapsed = a.elapsed[i];
@@ -1437,19 +1447,8 @@ __global__ void __launch_bounds__(kLunarThreads, 4) walker_reset_list_kernel(con
     const int cnt = *a.reset_count;
     for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < cnt; idx += gridDim.x * blockDim.x) {
         const int64_t i = a.first + a.reset_list[a.first + idx];
-        walker::World W;
-        walker::Rng r;
-        walker::bind_world(W, a.lunar_rec, a.n, i);
-        W.flags = a.lunar_rec[(int64_t)walker::W_FLAGS * a.n + i] & b2l::kFlagsKept;
-        r.has32 = a.lunar_rec[(int64_t)walker::W_RNG32 * a.n + i];
-        r.val32 = a.lunar_rec[(int64_t)(walker::W_RNG32 + 1) * a.n + i];
-        r.g = pcg64_load(a.rng + 4 * i);
-        W.np = 0; W.p_lo = 0; W.p_hi = -1;
         float obs[24];
-        walker::env_reset<HC>(W, r, obs);
-        walker::store_world(W, a.lunar_rec, a.n, i, r, HC);
-        pcg64_store(a.rng + 4 * i, r.g);
-        a.elapsed[i] = 0;
+        walker_reset_env<HC>(a.lunar_rec, a.elapsed, a.rng, a.n, i, obs);
         store_obs_all<24>(a, i, obs);
     }
 }
@@ -1460,19 +1459,8 @@ __global__ void __launch_bounds__(kLunarThreads) walker_reset_kernel(uint32_t *r
     const int64_t i = (int64_t)blockIdx.x * kLunarThreads + threadIdx.x;
     if (i >= n) return;
     if (mask && !mask[i]) return;
-    walker::World W;
-    walker::Rng r;
-    walker::bind_world(W, rec, n, i);
-    W.flags = rec[(int64_t)walker::W_FLAGS * n + i] & b2l::kFlagsKept;  // the b2World object survives reset()
-    r.has32 = rec[(int64_t)walker::W_RNG32 * n + i];
-    r.val32 = rec[(int64_t)(walker::W_RNG32 + 1) * n + i];
-    r.g = pcg64_load(rng + 4 * i);
     float o[24];
-    W.np = 0; W.p_lo = 0; W.p_hi = -1;
-    walker::env_reset<HC>(W, r, o);
-    walker::store_world(W, rec, n, i, r, HC);
-    pcg64_store(rng + 4 * i, r.g);
-    elapsed[i] = 0;
+    walker_reset_env<HC>(rec, elapsed, rng, n, i, o);
     if (obs) store_row<24>(obs, i, o);
 }
 
@@ -1720,7 +1708,7 @@ template <int KIND, typename ActT>
 static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
     int64_t done = 0;
     const int64_t tiles = a.count / kThreads;
-    if ((a.npeer > 0 || a.bulk_sink) && h->gather_bulk && tiles > 0) {
+    if ((a.npeer > 0 || a.bulk_sink) && tiles > 0) {
         // kernel G (bulk pushes): every destination row block must be 16-byte aligned
         auto ok = [&](const float *o, const double *r, const uint8_t *te, const uint8_t *tr) {
             return (uintptr_t)(o + a.first * Env<KIND>::D) % 16 == 0 && (uintptr_t)(r + a.first) % 16 == 0 &&
@@ -1774,37 +1762,16 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
         if (aligned) {
             // the lean instantiation: no fused episode statistics, every index fits 32 bits
             const bool lean = h->kernel_choice != 1 && !a.ep_acc && h->n < (int64_t)1 << 30;
-            const bool deep = h->p_depth == 2;
-            int &occ = h->occ[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2][(lean ? 1 : 0) + (deep ? 2 : 0)];
+            const auto kernel = lean ? step_kernel_persistent<KIND, ActT, true> : step_kernel_persistent<KIND, ActT, false>;
+            int &occ = h->occ[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2][lean ? 1 : 0];
             if (occ == 0) {
-                if (lean && deep) CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent<KIND, ActT, true, 2>, kThreads, 0));
-                else if (lean) CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent<KIND, ActT, true, 1>, kThreads, 0));
-                else if (deep) CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent<KIND, ActT, false, 2>, kThreads, 0));
-                else CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent<KIND, ActT, false, 1>, kThreads, 0));
+                CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 0));
                 if (occ < 1) occ = 1;
             }
             const int64_t all_tiles = (a.count + kThreads - 1) / kThreads;
-            // resident CTAs per SM: the occupancy limit, or -- when that leaves the last round of tiles mostly
-            // empty -- the smaller count that makes every CTA walk (nearly) the same number of tiles
-            int per_sm = occ;
-            if (h->p_ctas > 0 && h->p_ctas < occ) per_sm = h->p_ctas;
-            else if (h->p_ctas == 0) {
-                double best = 0.0;
-                for (int c = occ; c >= (occ > 2 ? occ - 2 : 1); c--) {
-                    const int64_t g = (int64_t)h->sm_count * c;
-                    const int64_t rounds = (all_tiles + g - 1) / g;
-                    // throughput model: tiles per round-time; a round's time grows with the resident warps only
-                    // weakly (latency-bound), so weigh occupancy by its square root
-                    const double score = (double)all_tiles / (double)(rounds * g) * sqrt((double)c / occ);
-                    if (score > best + 1e-9) { best = score; per_sm = c; }
-                }
-            }
-            int64_t grid = (int64_t)h->sm_count * per_sm;
+            int64_t grid = (int64_t)h->sm_count * occ;
             if (grid > all_tiles) grid = all_tiles;
-            if (lean && deep) step_kernel_persistent<KIND, ActT, true, 2><<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
-            else if (lean) step_kernel_persistent<KIND, ActT, true, 1><<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
-            else if (deep) step_kernel_persistent<KIND, ActT, false, 2><<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
-            else step_kernel_persistent<KIND, ActT, false, 1><<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
+            kernel<<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
             CK(h, cudaGetLastError());
             done = a.count;
         }
@@ -1813,8 +1780,7 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
         StepArgs t = a;
         t.first = a.first + done;
         t.count = a.count - done;
-        const int bs = h->block_a;
-        step_kernel<KIND, ActT><<<(unsigned)((t.count + bs - 1) / bs), bs, 0, st>>>(t);
+        step_kernel<KIND, ActT><<<blocks_for(t.count), kThreads, 0, st>>>(t);
         CK(h, cudaGetLastError());
     }
     return 0;
@@ -1837,6 +1803,66 @@ static int launch_step_kind(b200gym *h, const StepArgs &a, int action_dtype, cud
     }
 }
 
+// A Box2D step: step kernel -> TOI kernel over the parked envs -> compacted reset-list kernel; the last two only when
+// their path is deferred (else the step kernel solves TOI / resets inline)
+static int launch_step_box2d(b200gym *h, const StepArgs &a, int action_dtype, cudaStream_t st) {
+    using Kernel = void (*)(const StepArgs);
+    Kernel step, toi, reset_list;
+    if (h->is_lunar) {
+        if (h->cfg.kind == B200GYM_LUNARLANDER_CONT) {
+            if (action_dtype != B200GYM_ACT_F32) return fail(h, "Box env needs float32 actions (got dtype code %d)", action_dtype);
+            if ((uintptr_t)a.actions % 8 != 0) return fail(h, "LunarLanderContinuous actions must be 8-byte aligned");
+            step = lunar_step_kernel<float, true>;
+        } else {
+            switch (action_dtype) {
+            case B200GYM_ACT_I64: step = lunar_step_kernel<long long, false>; break;
+            case B200GYM_ACT_I32: step = lunar_step_kernel<int, false>; break;
+            case B200GYM_ACT_U8: step = lunar_step_kernel<unsigned char, false>; break;
+            default: return fail(h, "Discrete env needs an integer action dtype (got code %d)", action_dtype);
+            }
+        }
+        toi = lunar_toi_kernel;
+        reset_list = lunar_reset_list_kernel;
+    } else {
+        if (action_dtype != B200GYM_ACT_F32) return fail(h, "Box env needs float32 actions (got dtype code %d)", action_dtype);
+        if ((uintptr_t)a.actions % 16 != 0) return fail(h, "BipedalWalker actions must be 16-byte aligned");
+        const bool hc = h->cfg.kind == B200GYM_BIPEDALWALKER_HARDCORE;
+        step = hc ? walker_step_kernel<true> : walker_step_kernel<false>;
+        toi = hc ? walker_toi_kernel<true> : walker_toi_kernel<false>;
+        reset_list = hc ? walker_reset_list_kernel<true> : walker_reset_list_kernel<false>;
+    }
+    StepArgs b = a;
+    const bool defer = h->cfg.autoreset && h->box2d_defer && h->reset_list;
+    if (defer) {   // the caller may have picked a counter slot (one per concurrently running range)
+        b.reset_list = h->reset_list;
+        if (!b.reset_count) b.reset_count = h->reset_count;
+        CK(h, cudaMemsetAsync(b.reset_count, 0, sizeof(int32_t), st));
+    } else {
+        b.reset_list = nullptr; b.reset_count = nullptr;
+    }
+    // continuous collision of the parked envs in its own launch (see lunar_toi_kernel)
+    const bool toi_defer = h->box2d_toi_defer && h->toi_list;
+    if (toi_defer) {
+        b.toi_list = h->toi_list;
+        b.toi_mid = h->toi_mid;
+        if (!b.toi_count) b.toi_count = h->toi_count;
+        CK(h, cudaMemsetAsync(b.toi_count, 0, sizeof(int32_t), st));
+    } else {
+        b.toi_list = nullptr; b.toi_count = nullptr; b.toi_mid = nullptr;
+    }
+    const int64_t blocks = (b.count + kLunarThreads - 1) / kLunarThreads;
+    step<<<(unsigned)blocks, kLunarThreads, 0, st>>>(b);
+    CK(h, cudaGetLastError());
+    if (toi_defer) {
+        toi<<<(unsigned)std::min<int64_t>(b.count, (int64_t)kToiCtasPerSm * h->sm_count), 32, 0, st>>>(b);
+        CK(h, cudaGetLastError());
+    }
+    // at most 2 CTAs per SM of the compacted reset kernel (it strides over the list)
+    if (defer) reset_list<<<(unsigned)std::min<int64_t>(blocks, 2 * h->sm_count), kLunarThreads, 0, st>>>(b);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
 static int launch_step(b200gym *h, const StepArgs &a, int action_dtype, cudaStream_t st) {
     switch (h->cfg.kind) {
     case B200GYM_CARTPOLE: return launch_step_kind<B200GYM_CARTPOLE>(h, a, action_dtype, st);
@@ -1847,102 +1873,7 @@ static int launch_step(b200gym *h, const StepArgs &a, int action_dtype, cudaStre
     case B200GYM_LUNARLANDER:
     case B200GYM_LUNARLANDER_CONT:
     case B200GYM_BIPEDALWALKER:
-    case B200GYM_BIPEDALWALKER_HARDCORE: {
-        StepArgs b = a;
-        const bool defer = h->cfg.autoreset && h->box2d_defer && h->reset_list;
-        if (defer) {   // the caller may have picked a counter slot (one per concurrently running range)
-            b.reset_list = h->reset_list;
-            if (!b.reset_count) b.reset_count = h->reset_count;
-            CK(h, cudaMemsetAsync(b.reset_count, 0, sizeof(int32_t), st));
-        } else {
-            b.reset_list = nullptr; b.reset_count = nullptr;
-        }
-        // continuous collision of the parked envs in its own launch (see lunar_toi_kernel)
-        const bool toi_defer = h->box2d_toi_defer && h->toi_list;
-        if (toi_defer) {
-            b.toi_list = h->toi_list;
-            b.toi_mid = h->toi_mid;
-            if (!b.toi_count) b.toi_count = h->toi_count;
-            CK(h, cudaMemsetAsync(b.toi_count, 0, sizeof(int32_t), st));
-        } else {
-            b.toi_list = nullptr; b.toi_count = nullptr; b.toi_mid = nullptr;
-        }
-        // one warp per CTA, 12 CTAs per SM (what is resident with the 156-register kernel); the kernel strides over
-        // the list.  Larger grids (fewer envs per warp) are slower (H100 80GB HBM3 at 400 W, 2^16 envs, cold-L2 median):
-        // LunarLander 1.77 / 1.86 / 1.90 ms at 12 / 64 / 256 CTAs per SM, BipedalWalker (nearly every env parked)
-        // 8.24 / 11.5 / 16.0 ms
-        const unsigned tgrid = (unsigned)std::min<int64_t>(b.count, (int64_t)h->toi_grid * h->sm_count);
-        // With both on, the resets come from two kernels: those of the step kernel go onto list 1 and restart on the
-        // side stream WHILE the TOI kernel runs (a reset is a long serial chain -- terrain draw + an embedded world
-        // step -- but touches only its own env); those of the TOI kernel
-        // go onto list 2 and restart after it.  b2 = the arguments of the TOI kernel and of the second reset launch.
-        const bool split = defer && toi_defer && h->side && h->box2d_split;
-        StepArgs b2 = b;
-        if (split) {
-            const ptrdiff_t slot = b.reset_count - h->reset_count;   // the caller's counter slot
-            b2.reset_list = h->reset_list2;
-            b2.reset_count = h->reset_count2 + ((slot >= 0 && slot < kResetSlots) ? slot : 0);
-            CK(h, cudaMemsetAsync(b2.reset_count, 0, sizeof(int32_t), st));
-        }
-        // at most this many CTAs of the compacted reset kernel (it strides over the list)
-        const unsigned rgrid = (unsigned)std::min<int64_t>((b.count + kLunarThreads - 1) / kLunarThreads, 2 * h->sm_count);
-        if (h->is_lunar) {
-            const int bs = h->box2d_block;
-            const unsigned grid = (unsigned)((b.count + bs - 1) / bs);
-            if (h->cfg.kind == B200GYM_LUNARLANDER_CONT) {
-                if (action_dtype != B200GYM_ACT_F32) return fail(h, "Box env needs float32 actions (got dtype code %d)", action_dtype);
-                if ((uintptr_t)b.actions % 8 != 0) return fail(h, "LunarLanderContinuous actions must be 8-byte aligned");
-                lunar_step_kernel<float, true><<<grid, bs, 0, st>>>(b);
-            } else {
-                switch (action_dtype) {
-                case B200GYM_ACT_I64: lunar_step_kernel<long long, false><<<grid, bs, 0, st>>>(b); break;
-                case B200GYM_ACT_I32: lunar_step_kernel<int, false><<<grid, bs, 0, st>>>(b); break;
-                case B200GYM_ACT_U8: lunar_step_kernel<unsigned char, false><<<grid, bs, 0, st>>>(b); break;
-                default: return fail(h, "Discrete env needs an integer action dtype (got code %d)", action_dtype);
-                }
-            }
-            CK(h, cudaGetLastError());
-            if (split) {   // the step kernel's resets on the side stream, under the TOI kernel
-                CK(h, cudaEventRecord(h->ev_fork, st));
-                CK(h, cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-                lunar_reset_list_kernel<<<rgrid, kLunarThreads, 0, h->side>>>(b);
-                CK(h, cudaEventRecord(h->ev_join, h->side));
-            }
-            if (toi_defer) {
-                lunar_toi_kernel<<<tgrid, 32, 0, st>>>(b2);
-                CK(h, cudaGetLastError());
-            }
-            if (defer) lunar_reset_list_kernel<<<rgrid, kLunarThreads, 0, st>>>(b2);
-            if (split) CK(h, cudaStreamWaitEvent(st, h->ev_join, 0));
-        } else {
-            if (action_dtype != B200GYM_ACT_F32) return fail(h, "Box env needs float32 actions (got dtype code %d)", action_dtype);
-            if ((uintptr_t)b.actions % 16 != 0) return fail(h, "BipedalWalker actions must be 16-byte aligned");
-            const unsigned grid = (unsigned)((b.count + kLunarThreads - 1) / kLunarThreads);
-            const bool hc = h->cfg.kind == B200GYM_BIPEDALWALKER_HARDCORE;
-            if (hc) walker_step_kernel<true><<<grid, kLunarThreads, 0, st>>>(b);
-            else walker_step_kernel<false><<<grid, kLunarThreads, 0, st>>>(b);
-            CK(h, cudaGetLastError());
-            if (split) {   // the step kernel's resets on the side stream, under the TOI kernel
-                CK(h, cudaEventRecord(h->ev_fork, st));
-                CK(h, cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-                if (hc) walker_reset_list_kernel<true><<<rgrid, kLunarThreads, 0, h->side>>>(b);
-                else walker_reset_list_kernel<false><<<rgrid, kLunarThreads, 0, h->side>>>(b);
-                CK(h, cudaEventRecord(h->ev_join, h->side));
-            }
-            if (toi_defer) {
-                if (hc) walker_toi_kernel<true><<<tgrid, 32, 0, st>>>(b2);
-                else walker_toi_kernel<false><<<tgrid, 32, 0, st>>>(b2);
-                CK(h, cudaGetLastError());
-            }
-            if (defer) {
-                if (hc) walker_reset_list_kernel<true><<<rgrid, kLunarThreads, 0, st>>>(b2);
-                else walker_reset_list_kernel<false><<<rgrid, kLunarThreads, 0, st>>>(b2);
-            }
-            if (split) CK(h, cudaStreamWaitEvent(st, h->ev_join, 0));
-        }
-        CK(h, cudaGetLastError());
-        return 0;
-    }
+    case B200GYM_BIPEDALWALKER_HARDCORE: return launch_step_box2d(h, a, action_dtype, st);
     }
     return fail(h, "bad kind %d", h->cfg.kind);
 }
@@ -2037,30 +1968,15 @@ extern "C" int b200gym_create(const b200gym_config *cfg, int64_t num_envs, int d
     h->NACT = k_nact[cfg->kind];
     h->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
     {
-        const char *fs = getenv("B200GYM_SIMPLE_KERNEL");
         const char *kc = getenv("B200GYM_KERNEL");
         if (kc && (kc[0] == 'a' || kc[0] == 'p' || kc[0] == 'l' || kc[0] == 'b'))
             h->kernel_choice = kc[0] == 'a' ? 0 : kc[0] == 'p' ? 1 : kc[0] == 'l' ? 2 : 3;
-        const char *pd = getenv("B200GYM_P_DEPTH");
-        if (pd && (pd[0] == '1' || pd[0] == '2')) h->p_depth = pd[0] - '0';
-        const char *pc = getenv("B200GYM_P_CTAS");
-        if (pc && atoi(pc) >= -1 && atoi(pc) <= 8) h->p_ctas = atoi(pc);
-        if (fs && fs[0] == '1') h->kernel_choice = 0;
         const char *pfb = getenv("B200GYM_P2P_FUSE_BARRIER");
         if (pfb && (pfb[0] == '0' || pfb[0] == '1')) h->p2p_fuse = pfb[0] - '0';
-        const char *gb = getenv("B200GYM_GATHER");
-        if (gb && (gb[0] == 'b' || gb[0] == 'd')) h->gather_bulk = gb[0] == 'b';
-        const char *bb = getenv("B200GYM_BOX2D_BLOCK");
-        if (bb && (atoi(bb) == 128 || atoi(bb) == 256)) h->box2d_block = atoi(bb);
-        const char *bsp = getenv("B200GYM_BOX2D_SPLIT");
-        if (bsp && (bsp[0] == '0' || bsp[0] == '1')) h->box2d_split = bsp[0] - '0';
-        if (const char *tge = getenv("B200GYM_TOI_GRID")) { const int v = atoi(tge); if (v >= 1 && v <= 1024) h->toi_grid = v; }
         const char *btd = getenv("B200GYM_BOX2D_TOI_DEFER");
         if (btd && (btd[0] == '0' || btd[0] == '1')) h->box2d_toi_defer = btd[0] - '0';
         const char *bdf = getenv("B200GYM_BOX2D_DEFER");
         if (bdf && (bdf[0] == '0' || bdf[0] == '1')) h->box2d_defer = bdf[0] - '0';
-        const char *ba = getenv("B200GYM_BLOCK_A");
-        if (ba && (atoi(ba) == 64 || atoi(ba) == 128 || atoi(ba) == 256)) h->block_a = atoi(ba);
     }
     DeviceGuard guard(device);
     const size_t n = (size_t)num_envs;
@@ -2096,12 +2012,6 @@ extern "C" int b200gym_create(const b200gym_config *cfg, int64_t num_envs, int d
         if (cudaMalloc(&h->lunar_rec, sizeof(uint32_t) * words * n) != cudaSuccess ||
             cudaMemset(h->lunar_rec, 0, sizeof(uint32_t) * words * n) != cudaSuccess ||
             cudaMalloc((void **)&h->reset_list, sizeof(int32_t) * n) != cudaSuccess ||
-            cudaMalloc((void **)&h->reset_list2, sizeof(int32_t) * n) != cudaSuccess ||
-            cudaMalloc((void **)&h->reset_count2, sizeof(int32_t) * kResetSlots) != cudaSuccess ||
-            cudaMemset(h->reset_count2, 0, sizeof(int32_t) * kResetSlots) != cudaSuccess ||
-            cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming) != cudaSuccess ||
             cudaMalloc((void **)&h->toi_list, sizeof(int32_t) * n) != cudaSuccess ||
             cudaMalloc((void **)&h->toi_count, sizeof(int32_t) * kResetSlots) != cudaSuccess ||
             cudaMemset(h->toi_count, 0, sizeof(int32_t) * kResetSlots) != cudaSuccess ||
@@ -2157,11 +2067,6 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     cudaFree(h->toi_list);
     cudaFree(h->toi_count);
     cudaFree(h->toi_mid);
-    cudaFree(h->reset_list2);
-    cudaFree(h->reset_count2);
-    if (h->side) cudaStreamDestroy(h->side);
-    if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-    if (h->ev_join) cudaEventDestroy(h->ev_join);
     if (h->snap_bad) cudaFreeHost(h->snap_bad);
     cudaFree(h->snap_scratch);
     if (h->p2p.base) {

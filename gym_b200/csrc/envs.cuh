@@ -74,12 +74,8 @@ __constant__ double kCosCoef[6] = {4.16666666666666019037e-02, -1.38888888888741
 // the library path of sincos_small, out of line: it only runs in plain-Env mode after termination, and inlined it
 // costs the 32-register hot loop of the step kernels spill slots
 __device__ __noinline__ void sincos_library(double x, double *sn, double *cs) {
-#ifdef B200_DIAG_CUDA_SINCOS   // diagnosis builds only (scripts/r2b_variants.sh): CUDA's own sincos on the cold path
-    sincos(x, sn, cs);
-#else
     *sn = gt::sin(x);
     *cs = gt::cos(x);
-#endif
 }
 
 __device__ __forceinline__ void sincos_small(double x, double &sn, double &cs) {

@@ -5,5 +5,4 @@ F="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false -X
 mkdir -p _variants
 nvcc $F -DB200_MIN_CTAS=6 -o _variants/lib_c6.so gym_b200/csrc/b200gym.cu &
 nvcc $F -DB200_MIN_CTAS=5 -o _variants/lib_c5.so gym_b200/csrc/b200gym.cu &
-nvcc $F -DB200_DIAG_CUDA_SINCOS -o _variants/lib_cudasincos.so gym_b200/csrc/b200gym.cu &
 wait

@@ -29,14 +29,12 @@ NTHREADS = os.cpu_count() or 1
 # at 49 every B CTA walks >= 7 tiles; at 96 every B CTA walks >= 13 and every P CTA >= 12.
 SHAPES = {"bulk_shape": 49, "persistent_shape": 96}
 
-# engine variants: kernel A (the reference for the others), B, P, and P's lean instantiation with one and two
-# tiles in flight per thread
+# engine variants: kernel A (the reference for the others), B, P, and P's lean instantiation
 VARIANTS = {
-    "a": dict(B200GYM_KERNEL="a", B200GYM_P_DEPTH="1"),
-    "b": dict(B200GYM_KERNEL="b", B200GYM_P_DEPTH="1"),
-    "p": dict(B200GYM_KERNEL="p", B200GYM_P_DEPTH="1"),
-    "l1": dict(B200GYM_KERNEL="l", B200GYM_P_DEPTH="1"),
-    "l2": dict(B200GYM_KERNEL="l", B200GYM_P_DEPTH="2"),
+    "a": dict(B200GYM_KERNEL="a"),
+    "b": dict(B200GYM_KERNEL="b"),
+    "p": dict(B200GYM_KERNEL="p"),
+    "l": dict(B200GYM_KERNEL="l"),
 }
 
 
@@ -53,8 +51,7 @@ def _shape_n(shape):
 def _make(env_id, n, env_vars=None, **kwargs):
     import gym_b200
     with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("B200GYM_P_CTAS", "-1")
-        for k in ("B200GYM_KERNEL", "B200GYM_P_DEPTH", "B200GYM_HOST_CHUNKS"):
+        for k in ("B200GYM_KERNEL", "B200GYM_HOST_CHUNKS"):
             mp.delenv(k, raising=False)
         for k, v in (env_vars or {}).items():
             mp.setenv(k, v)
