@@ -1,19 +1,22 @@
-// hostsim.cpp -- the device solver source of the Box2D tasks, compiled for the CPU.
+// hostsim.cpp -- the device source of the step and reset kernels, compiled for the CPU.
 //
-// TEST INFRASTRUCTURE (never shipped, never imported by gym_b200/): includes gym_b200/csrc/{rng,envs,b2lite,lunar,
-// walker}.cuh and box2d_consts.h through tests/hostsim/cuda_shim.h and drives them with plain loops that mirror the
-// bodies of lunar_step_kernel / walker_step_kernel / *_reset_kernel in gym_b200/csrc/b200gym.cu (same record layout,
-// same load -> env_step -> TimeLimit -> autoreset -> store sequence).  tests/test_hostsim_cpu.py compares it bit for
-// bit with the C oracle, so the `-m "not gpu"` suite exercises the code the kernels run: solver, scenes, record
-// packing, host-computed constants, numpy-compatible RNG.
+// TEST INFRASTRUCTURE (never shipped, never imported by gym_b200/): includes gym_b200/csrc/{rng,envs,lunar,walker,
+// per_env}.cuh and box2d_consts.h through tests/hostsim/cuda_shim.h and calls the kernels' own per-env drivers
+// (per_env.cuh) with plain loops, in the order the kernels are launched.  tests/test_hostsim_cpu.py compares it bit for
+// bit with the C oracle, so the `-m "not gpu"` suite runs the code the kernels run: the drivers (action decode,
+// TimeLimit, autoreset, final observations, the parked-env and reset lists of the Box2D tasks), solver, scenes, record
+// packing, host-computed constants, numpy-compatible RNG.  What it does not run: the kernels' thread and warp logic
+// (indexing, shared-memory tiles and lists, the warp-synchronous TOI rounds) and launch code.
 #include "cuda_shim.h"
 
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #include "../../gym_b200/csrc/rng.cuh"
 #include "../../gym_b200/csrc/envs.cuh"
 #include "../../gym_b200/csrc/box2d_consts.h"
+#include "../../gym_b200/csrc/per_env.cuh"
 
 using bgym::Pcg64;
 
@@ -23,10 +26,18 @@ struct Sim {
     int kind = 0;            // enum b200gym_kind: 5 lunar, 7 lunar continuous, 6 walker, 8 walker hardcore
     int64_t n = 0;
     int max_steps = 0;
+    bool defer = true;       // the product default: parked-env TOI pass and reset pass (false: both inline, as
+                             // B200GYM_BOX2D_TOI_DEFER=0 / B200GYM_BOX2D_DEFER=0 select on the device)
+    int ranges = 1;          // launch ranges a step is split into, the last one ragged (the host path's chunks)
     lunar::Opts opts{};
     std::vector<uint32_t> rec;       // [words][n]
     std::vector<uint64_t> rng;       // [n][4]
     std::vector<int32_t> elapsed;
+    std::vector<int32_t> toi_list, reset_list;   // [n]
+    std::vector<uint32_t> toi_mid;               // [kToiMidWords][n]
+    int32_t toi_count = 0, reset_count = 0;
+    int64_t toi_total = 0, reset_total = 0;      // entries the TOI and reset passes have taken, over all steps
+    unsigned long long invalid = 0, invalid_seen = 0;
     bool lunar() const { return kind == 5 || kind == 7; }
     bool hardcore() const { return kind == 8; }
 };
@@ -39,80 +50,38 @@ void ensure_consts() {
     g_consts_ready = true;
 }
 
-void lunar_reset_env(Sim &S, int64_t i, float *obs) {     // lunar_reset_kernel
-    lunar::World W;
-    W.flags = S.rec[(int64_t)lunar::W_FLAGS * S.n + i] & b2l::kFlagsKept;
-    W.wind_idx = S.opts.wind ? (int32_t)S.rec[(int64_t)lunar::W_WIND * S.n + i] : 0;
-    W.torque_idx = S.opts.wind ? (int32_t)S.rec[(int64_t)(lunar::W_WIND + 1) * S.n + i] : 0;
-    Pcg64 g = bgym::pcg64_load(&S.rng[4 * i]);
-    float o[8];
-    lunar::env_reset(W, g, S.opts, o);
-    lunar::store_world(W, S.rec.data(), S.n, i, S.opts.wind != 0);
-    bgym::pcg64_store(&S.rng[4 * i], g);
-    S.elapsed[i] = 0;
-    if (obs) std::memcpy(obs + 8 * i, o, sizeof o);
-}
-
-template <bool HC>
-void walker_reset_env(Sim &S, int64_t i, float *obs) {    // walker_reset_kernel<HC>
-    walker::World W;
-    walker::Rng r;
-    walker::bind_world(W, S.rec.data(), S.n, i);
-    W.flags = S.rec[(int64_t)walker::W_FLAGS * S.n + i] & b2l::kFlagsKept;
-    r.has32 = S.rec[(int64_t)walker::W_RNG32 * S.n + i];
-    r.val32 = S.rec[(int64_t)(walker::W_RNG32 + 1) * S.n + i];
-    r.g = bgym::pcg64_load(&S.rng[4 * i]);
-    W.np = 0; W.p_lo = 0; W.p_hi = -1;
-    float o[24];
-    walker::env_reset<HC>(W, r, o);
-    walker::store_world(W, S.rec.data(), S.n, i, r, HC);
-    bgym::pcg64_store(&S.rng[4 * i], r.g);
-    S.elapsed[i] = 0;
-    if (obs) std::memcpy(obs + 24 * i, o, sizeof o);
-}
-
-template <bool HC>
-void walker_step_env(Sim &S, int64_t i, const float *act, float *obs_out, double *reward, uint8_t *term, uint8_t *trunc,
-                     float *final_obs) {                  // walker_step_kernel<HC>
-    const float action[4] = {act[4 * i], act[4 * i + 1], act[4 * i + 2], act[4 * i + 3]};
-    walker::World W;
-    walker::Rng rng;
-    walker::load_world(W, S.rec.data(), S.n, i, rng, HC);
-    int32_t elapsed = S.elapsed[i];
-    float obs[24];
-    double r;
-    bool terminated;
-    walker::env_step<HC>(W, action, false, walker::V(0.0f, 0.0f), obs, r, terminated);
-    elapsed += 1;
-    const bool truncated = (S.max_steps > 0) && (elapsed >= S.max_steps);
-    reward[i] = r; term[i] = terminated ? 1 : 0; trunc[i] = truncated ? 1 : 0;
-    if (terminated || truncated) {
-        if (final_obs) std::memcpy(final_obs + 24 * i, obs, sizeof obs);
-        rng.g = bgym::pcg64_load(&S.rng[4 * i]);
-        walker::env_reset<HC>(W, rng, obs);
-        bgym::pcg64_store(&S.rng[4 * i], rng.g);
-        elapsed = 0;
-    }
-    walker::store_world(W, S.rec.data(), S.n, i, rng, HC);
-    S.elapsed[i] = elapsed;
-    std::memcpy(obs_out + 24 * i, obs, sizeof obs);
+// one launch range through the passes launch_step_box2d issues: step pass over the range, TOI pass over the parked
+// list, reset pass over the reset list (one lane per "warp": live = 1)
+template <typename StepF, typename ToiF, typename ResetF>
+void box2d_range(const StepArgs &a, StepF step, ToiF toi, ResetF reset) {
+    if (a.toi_list) *a.toi_count = 0;
+    if (a.reset_list) *a.reset_count = 0;
+    for (int64_t j = 0; j < a.count; j++) step(a, j);
+    if (a.toi_list)
+        for (int idx = 0; idx < *a.toi_count; idx++) toi(a, idx, 1u);
+    if (a.reset_list)
+        for (int idx = 0; idx < *a.reset_count; idx++) reset(a, idx);
 }
 
 }  // namespace
 
 extern "C" {
 
-void *hs_create(int kind, int64_t n, int max_steps, int wind, double gravity, double wind_power, double turbulence_power) {
-    if (n <= 0 || kind < 5 || kind > 8) return nullptr;
+void *hs_create(int kind, int64_t n, int max_steps, int wind, double gravity, double wind_power, double turbulence_power,
+                int defer, int ranges) {
+    if (n <= 0 || kind < 5 || kind > 8 || ranges < 1) return nullptr;
     ensure_consts();
     Sim *S = new Sim();
-    S->kind = kind; S->n = n; S->max_steps = max_steps;
+    S->kind = kind; S->n = n; S->max_steps = max_steps; S->defer = defer != 0; S->ranges = ranges;
     S->opts.continuous = kind == 7; S->opts.wind = wind != 0; S->opts.gravity = (float)gravity;
     S->opts.wind_power = wind_power; S->opts.turbulence_power = turbulence_power;
     const size_t words = S->lunar() ? lunar::kWords : (S->hardcore() ? walker::kWordsHC : walker::kWords);
     S->rec.assign(words * (size_t)n, 0u);
     S->rng.assign(4 * (size_t)n, 0ull);
     S->elapsed.assign((size_t)n, 0);
+    S->toi_list.assign((size_t)n, 0);
+    S->reset_list.assign((size_t)n, 0);
+    S->toi_mid.assign((size_t)kToiMidWords * (size_t)n, 0u);
     return S;
 }
 void hs_destroy(void *h) { delete (Sim *)h; }
@@ -146,55 +115,64 @@ void hs_get_wind_idx(void *h, int32_t *wind, int32_t *torque) {
     }
 }
 
-void hs_reset(void *h, float *obs) {
+void hs_reset(void *h, float *obs) {   // lunar_reset_kernel / walker_reset_kernel<HC>
     Sim &S = *(Sim *)h;
+    uint32_t *rec = S.rec.data();
+    int32_t *elapsed = S.elapsed.data();
+    uint64_t *rng = S.rng.data();
     for (int64_t i = 0; i < S.n; i++) {
-        if (S.lunar()) lunar_reset_env(S, i, obs);
-        else if (S.hardcore()) walker_reset_env<true>(S, i, obs);
-        else walker_reset_env<false>(S, i, obs);
+        if (S.lunar()) {
+            float o[8];
+            lunar_reset_env(rec, elapsed, rng, S.n, i, S.opts, o);
+            if (obs) store_row<8>(obs, i, o);
+        } else {
+            float o[24];
+            if (S.hardcore()) walker_reset_env<true>(rec, elapsed, rng, S.n, i, o);
+            else walker_reset_env<false>(rec, elapsed, rng, S.n, i, o);
+            if (obs) store_row<24>(obs, i, o);
+        }
     }
 }
 
 // actions: int64 [n] (kind 5) or float32 [n][2] (kind 7) or float32 [n][4] (kinds 6, 8); returns #invalid actions
 int64_t hs_step(void *h, const void *actions, float *obs_out, double *reward, uint8_t *term, uint8_t *trunc, float *final_obs) {
     Sim &S = *(Sim *)h;
-    int64_t invalid = 0;
-    for (int64_t i = 0; i < S.n; i++) {
-        if (!S.lunar()) {
-            if (S.hardcore()) walker_step_env<true>(S, i, (const float *)actions, obs_out, reward, term, trunc, final_obs);
-            else walker_step_env<false>(S, i, (const float *)actions, obs_out, reward, term, trunc, final_obs);
-            continue;
-        }
-        // lunar_step_kernel<ActT, CONT>
-        long long act = 0;
-        float ca0 = 0.0f, ca1 = 0.0f;
-        if (S.kind == 7) { ca0 = ((const float *)actions)[2 * i]; ca1 = ((const float *)actions)[2 * i + 1]; }
-        else {
-            act = ((const int64_t *)actions)[i];
-            if (act < 0 || act > 3) { invalid++; continue; }
-        }
-        lunar::World W;
-        lunar::load_world(W, S.rec.data(), S.n, i, S.opts.wind != 0);
-        Pcg64 g = bgym::pcg64_load(&S.rng[4 * i]);
-        int32_t elapsed = S.elapsed[i];
-        float obs[8];
-        double r;
-        bool terminated;
-        lunar::env_step(W, g, S.opts, (int)act, ca0, ca1, lunar::V(0.0f, 0.0f), obs, r, terminated);
-        elapsed += 1;
-        const bool truncated = (S.max_steps > 0) && (elapsed >= S.max_steps);
-        reward[i] = r; term[i] = terminated ? 1 : 0; trunc[i] = truncated ? 1 : 0;
-        if (terminated || truncated) {
-            if (final_obs) std::memcpy(final_obs + 8 * i, obs, sizeof obs);
-            lunar::env_reset(W, g, S.opts, obs);
-            elapsed = 0;
-        }
-        lunar::store_world(W, S.rec.data(), S.n, i, S.opts.wind != 0);
-        bgym::pcg64_store(&S.rng[4 * i], g);
-        S.elapsed[i] = elapsed;
-        std::memcpy(obs_out + 8 * i, obs, sizeof obs);
+    StepArgs a{};
+    a.rng = S.rng.data();
+    a.elapsed = S.elapsed.data();
+    a.invalid = &S.invalid;
+    a.invalid_seen = &S.invalid_seen;
+    a.lunar_rec = S.rec.data();
+    a.actions = actions;
+    a.obs = obs_out; a.reward = reward; a.terminated = term; a.truncated = trunc; a.final_obs = final_obs;
+    a.n = S.n;
+    a.max_steps = S.max_steps;
+    a.autoreset = 1;
+    a.lunar_opts = S.opts;
+    if (S.defer) {
+        a.toi_list = S.toi_list.data(); a.toi_count = &S.toi_count; a.toi_mid = S.toi_mid.data();
+        a.reset_list = S.reset_list.data(); a.reset_count = &S.reset_count;
     }
-    return invalid;
+    S.invalid = 0;
+    const int64_t per = (S.n + S.ranges - 1) / S.ranges;
+    for (a.first = 0; a.first < S.n; a.first += per) {
+        a.count = a.first + per < S.n ? per : S.n - a.first;
+        switch (S.kind) {
+        case 5: box2d_range(a, lunar_step_env<long long, false>, lunar_toi_env, lunar_reset_list_env); break;
+        case 7: box2d_range(a, lunar_step_env<float, true>, lunar_toi_env, lunar_reset_list_env); break;
+        case 6: box2d_range(a, walker_step_env<false>, walker_toi_env<false>, walker_reset_list_env<false>); break;
+        default: box2d_range(a, walker_step_env<true>, walker_toi_env<true>, walker_reset_list_env<true>); break;
+        }
+        if (S.defer) { S.toi_total += S.toi_count; S.reset_total += S.reset_count; }
+    }
+    return (int64_t)S.invalid;
+}
+
+// how many envs the TOI pass and the reset pass have taken since hs_create (0 and 0 for the inline configuration)
+void hs_list_totals(void *h, int64_t *toi, int64_t *reset) {
+    Sim &S = *(Sim *)h;
+    *toi = S.toi_total;
+    *reset = S.reset_total;
 }
 
 // the 200 terrain heights and the hardcore boxes of env i (walker kinds); returns the number of boxes
@@ -219,7 +197,7 @@ int64_t hs_overflows(void *h) {
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------------------
-// classic control: Env<KIND>::step / reset of gym_b200/csrc/envs.cuh driven like advance_env / reset_env of b200gym.cu
+// classic control: the per-env drivers of reset_kernel and kernel A (step_kernel) over Env<KIND> of envs.cuh
 // (autoreset mode: TimeLimit counter, same-step reset with the env's own PCG64 stream, final_obs rows)
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
@@ -232,65 +210,48 @@ struct Classic {
     std::vector<double> state;     // [S][n]
     std::vector<uint64_t> rng;     // [n][4]
     std::vector<int32_t> elapsed;
+    std::vector<uint8_t> flags;
+    unsigned long long invalid = 0, invalid_seen = 0;
 };
 
 template <int KIND>
-void classic_reset(Classic &C, const double *bounds, float *obs) {
-    using E = bgym::Env<KIND>;
+void classic_reset(Classic &C, const double *bounds, float *obs) {   // launch_reset_kind + reset_kernel
     double lo, hi;
-    E::default_bounds(lo, hi);
+    bgym::Env<KIND>::default_bounds(lo, hi);
     if (bounds) { lo = bounds[0]; hi = bounds[1]; }
-    for (int64_t i = 0; i < C.n; i++) {
-        double s[E::S];
-        float o[E::D];
-        Pcg64 g = bgym::pcg64_load(&C.rng[4 * i]);
-        E::reset(s, g, lo, hi, o);
-        bgym::pcg64_store(&C.rng[4 * i], g);
-        for (int k = 0; k < E::S; k++) C.state[(int64_t)k * C.n + i] = s[k];
-        C.elapsed[i] = 0;
-        std::memcpy(obs + (int64_t)E::D * i, o, sizeof o);
-    }
+    double *state = C.state.data();
+    int32_t *elapsed = C.elapsed.data();
+    uint8_t *flags = C.flags.data();
+    uint64_t *rng = C.rng.data();
+    for (int64_t i = 0; i < C.n; i++) reset_env_bounded<KIND>(state, elapsed, flags, rng, obs, C.n, i, lo, hi);
 }
 
+// kernel A over the whole batch: advance_env for every env, then reset_env for those whose episode ended
 template <int KIND>
 int64_t classic_step(Classic &C, const void *actions, float *obs_out, double *reward, uint8_t *term, uint8_t *trunc,
                      float *final_obs) {
     using E = bgym::Env<KIND>;
-    int64_t invalid = 0;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    StepArgs a{};
+    a.state = C.state.data(); a.elapsed = C.elapsed.data(); a.flags = C.flags.data(); a.rng = C.rng.data();
+    a.invalid = &C.invalid; a.invalid_seen = &C.invalid_seen;
+    a.actions = actions;
+    a.obs = obs_out; a.reward = reward; a.terminated = term; a.truncated = trunc; a.final_obs = final_obs;
+    a.n = C.n; a.first = 0; a.count = C.n;
+    a.max_steps = C.max_steps; a.autoreset = 1; a.param0 = C.param0;
+    const DirectSinkT<false> sink{a};
+    C.invalid = 0;
+    std::vector<int64_t> resets;
     for (int64_t i = 0; i < C.n; i++) {
         double s[E::S];
-        for (int k = 0; k < E::S; k++) s[k] = C.state[(int64_t)k * C.n + i];
-        int32_t elapsed = C.elapsed[i];
-        int act = 0;
+        for (int k = 0; k < E::S; k++) s[k] = a.state[k * a.n + i];
+        long long action_int = 0;
         float a0 = 0.0f;
-        if (E::A == 0) {
-            const long long v = ((const int64_t *)actions)[i];
-            if (v < 0 || v >= E::NACT) { invalid++; continue; }
-            act = (int)v;
-        } else {
-            a0 = ((const float *)actions)[i];
-        }
-        float obs[E::D];
-        double r;
-        bool terminated;
-        E::step(s, elapsed == 0, act, a0, C.param0, obs, r, terminated);
-        elapsed += 1;
-        const bool truncated = (C.max_steps > 0) && (elapsed >= C.max_steps);
-        reward[i] = r; term[i] = terminated ? 1 : 0; trunc[i] = truncated ? 1 : 0;
-        if (terminated || truncated) {
-            if (final_obs) std::memcpy(final_obs + (int64_t)E::D * i, obs, sizeof obs);
-            Pcg64 g = bgym::pcg64_load(&C.rng[4 * i]);
-            double lo, hi;
-            E::default_bounds(lo, hi);
-            E::reset(s, g, lo, hi, obs);
-            bgym::pcg64_store(&C.rng[4 * i], g);
-            elapsed = 0;
-        }
-        for (int k = 0; k < E::S; k++) C.state[(int64_t)k * C.n + i] = s[k];
-        C.elapsed[i] = elapsed;
-        std::memcpy(obs_out + (int64_t)E::D * i, obs, sizeof obs);
+        decode_action<KIND>(__ldg(reinterpret_cast<const ActT *>(a.actions) + i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, a.elapsed[i], action_int, a0)) resets.push_back(i);
     }
-    return invalid;
+    for (const int64_t i : resets) reset_env<KIND>(a, sink, i);
+    return (int64_t)C.invalid;
 }
 
 }  // namespace
@@ -304,6 +265,7 @@ void *hs_classic_create(int kind, int64_t n, int max_steps, double param0) {
     C->state.assign(4 * (size_t)n, 0.0);
     C->rng.assign(4 * (size_t)n, 0ull);
     C->elapsed.assign((size_t)n, 0);
+    C->flags.assign((size_t)n, 0);
     return C;
 }
 void hs_classic_destroy(void *h) { delete (Classic *)h; }

@@ -1,4 +1,4 @@
-"""ctypes wrapper of tests/hostsim/hostsim.cpp: the device source of the Box2D tasks running on the CPU.
+"""ctypes wrapper of tests/hostsim/hostsim.cpp: the device source of the step and reset kernels running on the CPU.
 
 Built on demand with g++ into tests/hostsim/_build/ (git-ignored), with the flags that make float32 arithmetic
 round like the device build does (`-ffp-contract=off`, matching nvcc's `-fmad=false`).
@@ -19,7 +19,7 @@ _LIB_SMALLCAP = os.path.join(_BUILD, "libhostsim_smallcap.so")
 SMALLCAP = {"lunar": 1, "walker": 2}
 _SRCS = [os.path.join(_HERE, "hostsim.cpp"), os.path.join(_HERE, "cuda_shim.h")] + [
     os.path.join(_ROOT, "gym_b200", "csrc", f) for f in ("rng.cuh", "envs.cuh", "glibc_trig.cuh", "b2lite.cuh", "b2lite_toi.cuh", "lunar.cuh",
-                                                         "walker.cuh", "box2d_consts.h")]
+                                                         "walker.cuh", "per_env.cuh", "box2d_consts.h")]
 
 KIND = {"LunarLander": 5, "BipedalWalker": 6, "LunarLanderContinuous": 7, "BipedalWalkerHardcore": 8}
 _lib = None
@@ -40,7 +40,7 @@ def lib(smallcap=False):
         L = ctypes.CDLL(path)
         vp, i64, i32, dbl = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_double
         L.hs_create.restype = vp
-        L.hs_create.argtypes = [i32, i64, i32, i32, dbl, dbl, dbl]
+        L.hs_create.argtypes = [i32, i64, i32, i32, dbl, dbl, dbl, i32, i32]
         L.hs_destroy.argtypes = [vp]
         L.hs_seed_range.argtypes = [vp, vp, i64]
         L.hs_set_wind_idx.argtypes = [vp, vp, vp]
@@ -48,6 +48,7 @@ def lib(smallcap=False):
         L.hs_reset.argtypes = [vp, vp]
         L.hs_step.restype = i64
         L.hs_step.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+        L.hs_list_totals.argtypes = [vp, vp, vp]
         L.hs_walker_terrain.restype = i32
         L.hs_walker_terrain.argtypes = [vp, i64, vp, vp]
         L.hs_classic_create.restype = vp
@@ -82,22 +83,33 @@ def _seed_words(seed):
 
 
 class HostSim:
-    """One batch of envs stepped by the device source on the CPU; same call shape as oracle.OracleLunar/OracleWalker."""
+    """One batch of envs stepped by the device source on the CPU; same call shape as oracle.OracleLunar/OracleWalker.
+
+    defer=True runs a step as the device does by default: a step pass, a TOI pass over the envs the step pass parked
+    and a reset pass over the envs whose episode ended; defer=False solves both inline in the step pass
+    (B200GYM_BOX2D_TOI_DEFER=0 / B200GYM_BOX2D_DEFER=0).  ranges > 1 splits every step into that many launch ranges,
+    the last one ragged, as the host path splits a batch into chunks."""
 
     def __init__(self, name, num_envs, max_episode_steps, gravity=-10.0, enable_wind=False, wind_power=15.0,
-                 turbulence_power=1.5, wind_idx=None, torque_idx=None, smallcap=False):
+                 turbulence_power=1.5, wind_idx=None, torque_idx=None, smallcap=False, defer=True, ranges=1):
         self._L = lib(smallcap)
         self.kind = KIND[name]
         self.n = int(num_envs)
         self.lunar = self.kind in (5, 7)
         self.obs_dim = 8 if self.lunar else 24
         self._h = self._L.hs_create(self.kind, self.n, int(max_episode_steps or 0), int(bool(enable_wind)), float(gravity),
-                                  float(wind_power), float(turbulence_power))
+                                  float(wind_power), float(turbulence_power), int(bool(defer)), int(ranges))
         assert self._h
         if wind_idx is not None:
             wi = np.ascontiguousarray(np.broadcast_to(wind_idx, (self.n,)), dtype=np.int32)
             ti = np.ascontiguousarray(np.broadcast_to(torque_idx, (self.n,)), dtype=np.int32)
             self._L.hs_set_wind_idx(self._h, wi.ctypes.data, ti.ctypes.data)
+
+    def list_totals(self):
+        """(envs taken by the TOI pass, envs taken by the reset pass) since construction."""
+        t = np.zeros(2, dtype=np.int64)
+        self._L.hs_list_totals(self._h, t[0:].ctypes.data, t[1:].ctypes.data)
+        return int(t[0]), int(t[1])
 
     def overflows(self):
         """Number of envs whose manifold table ever overflowed."""
@@ -146,7 +158,8 @@ class HostSim:
 
 
 class HostSimClassic:
-    """Env<KIND>::step / reset of gym_b200/csrc/envs.cuh on the CPU (autoreset mode); call shape of oracle.OracleVec."""
+    """The per-env drivers of reset_kernel and kernel A over Env<KIND> of gym_b200/csrc/envs.cuh on the CPU (autoreset
+    mode); call shape of oracle.OracleVec."""
 
     # kind -> (obs_dim, act_dim, state_dim); enum b200gym_kind
     DIMS = {0: (4, 0, 4), 1: (2, 0, 2), 2: (2, 1, 2), 3: (3, 1, 2), 4: (6, 0, 4)}

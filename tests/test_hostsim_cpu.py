@@ -1,11 +1,14 @@
-"""The DEVICE source of the Box2D tasks, compiled for the CPU, against the C oracle.  Runs without a GPU.
+"""The DEVICE source of the step and reset kernels, compiled for the CPU, against the C oracle.  Runs without a GPU.
 
-tests/hostsim/hostsim.cpp includes gym_b200/csrc/{rng,b2lite,lunar,walker}.cuh and box2d_consts.h through a small
-CUDA shim and mirrors the kernel bodies with plain loops.  What this pins on every CPU run: the register-resident
+tests/hostsim/hostsim.cpp includes gym_b200/csrc/{rng,envs,b2lite,lunar,walker,per_env}.cuh and box2d_consts.h
+through a small CUDA shim and calls the kernels' own per-env drivers (per_env.cuh) with plain loops, in the order the
+kernels are launched.  What this pins on every CPU run: the drivers (action decode, TimeLimit, autoreset, final
+observations, the Box2D step / TOI / reset passes with their parked-env and reset lists), the register-resident
 solver (compile-time island topology), the scenes, the record packing (load_world / store_world), the host-computed
 shape / mass / joint constants and the numpy-compatible RNG of the device code are bit-identical to the independent
 C implementation in oracle/ -- the same statement tests/test_gpu_lunar.py / test_gpu_walker.py make on the GPU for
-the nvcc build of this source.  (Not covered here: the kernels' own indexing / launch code and nvcc's code
+the nvcc build of this source.  (Not covered here: the kernels' thread and warp logic -- indexing, the
+warp-synchronous TOI rounds, the shared-memory tiles of kernels P, B and G --, launch code and nvcc's code
 generation -- that is what the `-m gpu` tests are for.)
 """
 import numpy as np
@@ -100,6 +103,31 @@ def test_walker_device_source_on_cpu_equals_oracle(name, hardcore, policy):
                 else:
                     a[i] = gaits[i](want[0][i])
     assert n_done > (N // 2 if policy == "random" or hardcore else 0)
+
+
+@pytest.mark.parametrize("defer", [True, False], ids=["deferred", "inline"])
+@pytest.mark.parametrize("name", ["LunarLander", "BipedalWalkerHardcore"])
+def test_box2d_step_configurations_on_cpu_equal_oracle(name, defer):
+    """The Box2D step as the device can run it: with the TOI and reset passes deferred (the default) or inline in the
+    step pass, and with the batch split into three launch ranges, the last one ragged, as the host path splits it
+    into chunks.  Every configuration must give the oracle's trajectories bit for bit, and the deferred one must
+    really have parked envs for the TOI pass and reset envs from the reset list."""
+    lunar = name == "LunarLander"
+    N, T, steps = (40, 160, 1000) if lunar else (20, 120, 2000)
+    sim = HostSim(name, N, steps, defer=defer, ranges=3)
+    ref = orc.OracleLunar(N, max_episode_steps=steps) if lunar else orc.OracleWalker(N, hardcore=True, max_episode_steps=steps)
+    assert np.array_equal(sim.reset(seed=12), ref.reset(seed=12))
+    rng = np.random.default_rng(6)
+    n_done = 0
+    for t in range(T):
+        a = rng.integers(0, 4, size=N) if lunar else rng.uniform(-1.3, 1.3, size=(N, 4)).astype(np.float32)
+        n_done += int(_compare(t, sim.step(a), ref.step(a)).sum())
+    assert n_done > N // 2
+    toi, reset = sim.list_totals()
+    if defer:
+        assert toi > 0 and reset == n_done, (toi, reset, n_done)
+    else:
+        assert toi == reset == 0
 
 
 def test_manifold_table_overflow_is_handled_identically():
