@@ -113,6 +113,7 @@ SIGNATURES = {
     "b200gym_rms_apply_reward": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
                                         _vp]),
     "b200gym_box2d_overflows": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
+    "b200gym_box2d_list_counts": (_i32, [_vp, _vp, _i32, _vp, _vp]),
     "b200gym_selftest_trig": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "b200gym_selftest": (_i32, [_i32, _i64, ctypes.c_uint64, ctypes.POINTER(_i64)]),
 }

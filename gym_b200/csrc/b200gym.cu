@@ -1738,6 +1738,21 @@ extern "C" int b200gym_box2d_overflows(b200gym_t *h, void *stream, int64_t *coun
     return 0;
 }
 
+extern "C" int b200gym_box2d_list_counts(b200gym_t *h, void *stream, int slots, int32_t *parked_out, int32_t *resets_out) {
+    if (!h || !parked_out || !resets_out) return fail(h, "b200gym_box2d_list_counts: null argument");
+    if (!h->is_lunar && !h->is_walker) return fail(h, "b200gym_box2d_list_counts: not a Box2D-task handle");
+    if (slots < 1 || slots > kResetSlots)
+        return fail(h, "b200gym_box2d_list_counts: slots must be in [1, %d], got %d", kResetSlots, slots);
+    DeviceGuard guard(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t bytes = sizeof(int32_t) * (size_t)slots;
+    cudaError_t e = cudaMemcpyAsync(parked_out, h->toi_count, bytes, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(resets_out, h->reset_count, bytes, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(h, "b200gym_box2d_list_counts: %s", cudaGetErrorString(e));
+    return 0;
+}
+
 extern "C" int b200gym_selftest(int device, int64_t samples, uint64_t seed, int64_t *mismatches_out) {
     if (!mismatches_out || samples <= 0) return fail(nullptr, "b200gym_selftest: bad argument");
     DeviceGuard guard(device);

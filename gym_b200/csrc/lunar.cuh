@@ -241,7 +241,12 @@ LD void env_reset(World &W, Pcg64 &rng, const Opts &O, float (&obs)[8]) {
     }
     W.flags = stepped;
     W.prev_shaping = 0.0;
-    for (int s = 0; s < kSlots; s++) W.slot_key[s] = 0u;
+    // the warm-start store starts empty, its unused rows zeroed as well: the reset-list kernel resets a World it never
+    // loaded, so rows left as they were would put uninitialised memory into the record and its snapshots
+    for (int s = 0; s < kSlots; s++) {
+        W.slot_key[s] = 0u;
+        for (int p = 0; p < 2; p++) { W.slot_id[s][p] = 0u; W.slot_nI[s][p] = 0.0f; W.slot_tI[s][p] = 0.0f; }
+    }
     const double fx = bgym::pcg64_uniform(rng, -1000.0, 1000.0);                 // :371-377
     const double fy = bgym::pcg64_uniform(rng, -1000.0, 1000.0);
     double r;

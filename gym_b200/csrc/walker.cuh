@@ -363,7 +363,11 @@ __device__ __noinline__ void env_reset(World &W, Rng &rng, float (&obs)[24]) {
     }
     W.flags = stepped;
     W.prev_shaping = 0.0;
-    for (int s = 0; s < kSlots; s++) W.slot_key[s] = 0u;
+    // the warm-start store starts empty, its unused rows zeroed as well (see lunar::env_reset)
+    for (int s = 0; s < kSlots; s++) {
+        W.slot_key[s] = 0u;
+        for (int p = 0; p < 2; p++) { W.slot_id[s][p] = 0u; W.slot_nI[s][p] = 0.0f; W.slot_tI[s][p] = 0.0f; }
+    }
     const double fx = bgym::pcg64_uniform(rng.g, -5, 5);                         // :450-452 INITIAL_RANDOM
     const float zero[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     double r;

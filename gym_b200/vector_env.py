@@ -491,6 +491,18 @@ class B200VectorEnv:
         _lib.check(self._lib.b200gym_box2d_overflows(self._handle, self._stream(), ctypes.byref(count)), self._handle)
         return int(count.value)
 
+    def box2d_list_counts(self, slots=1):
+        """Box2D tasks, a diagnostic: (parked, resets) int32 arrays of `slots` entries -- how many envs the last step
+        parked for the TOI kernel and queued for the compacted reset kernel, per launch range (the torch backend
+        runs one range, counted in slot 0; the numpy backend counts chunk c in slot c).  A pass that runs inline
+        leaves its counter at 0 (include/b200gym.h: b200gym_box2d_list_counts).  Synchronises."""
+        self._assert_open("box2d_list_counts")
+        parked = np.zeros(slots, dtype=np.int32)
+        resets = np.zeros(slots, dtype=np.int32)
+        _lib.check(self._lib.b200gym_box2d_list_counts(self._handle, self._stream(), int(slots), parked.ctypes.data,
+                                                       resets.ctypes.data), self._handle)
+        return parked, resets
+
     def lunar_wind_idx(self):
         """LunarLander(enable_wind=True) only: the per-env (wind_idx, torque_idx) int32 arrays
         (lunar_lander.py:234-235,461,472), read back from the device."""

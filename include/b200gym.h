@@ -370,6 +370,16 @@ int b200gym_rms_apply_reward(const double *reward_dev, double *out_dev, double *
 int b200gym_box2d_overflows(b200gym_t *h, void *stream, int64_t *count_out);
 
 /*
+ * Box2D tasks, a diagnostic: how many envs the last step parked for the TOI kernel (parked_out) and queued for the
+ * compacted reset kernel (resets_out), per launch range.  Copies counter slots [0, slots) of each, 1 <= slots <= 64:
+ * b200gym_step counts in slot 0, chunk c of b200gym_step_host in slot c.  A pass that runs inline
+ * (B200GYM_BOX2D_TOI_DEFER=0 / B200GYM_BOX2D_DEFER=0) never writes its counters, so they read 0.  Synchronises
+ * `stream`.
+ */
+int b200gym_box2d_list_counts(b200gym_t *h, void *stream, int slots, int32_t *parked_out,
+                              int32_t *resets_out);
+
+/*
  * Device self-test of the kernels' constant-divisor division (csrc/envs.cuh:div_by_const)
  * against IEEE `/`: `samples` pseudo-random doubles (both signs, 64 binades) x 4 divisors.
  * Synchronous; *mismatches_out must come back 0.

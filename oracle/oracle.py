@@ -319,9 +319,10 @@ class OracleLunar:
 
     __del__ = close
 
-    def reset(self, seed=None):
+    def reset(self, seed=None, first=0):
+        """env k is seeded seed + first + k: the oracle stands in for envs [first, first + n) of a larger batch"""
         if seed is not None:
-            lib().orc_lunar_seed_range(self._h, seed_words(seed).ctypes.data, 0)
+            lib().orc_lunar_seed_range(self._h, seed_words(seed).ctypes.data, int(first))
         obs = np.zeros((self.n, 8), dtype=np.float32)
         lib().orc_lunar_reset(self._h, obs.ctypes.data)
         return obs
@@ -387,9 +388,10 @@ class OracleWalker:
 
     __del__ = close
 
-    def reset(self, seed=None):
+    def reset(self, seed=None, first=0):
+        """env k is seeded seed + first + k (see OracleLunar.reset)"""
         if seed is not None:
-            lib().orc_walker_seed_range(self._h, seed_words(seed).ctypes.data, 0)
+            lib().orc_walker_seed_range(self._h, seed_words(seed).ctypes.data, int(first))
         obs = np.zeros((self.n, 24), dtype=np.float32)
         lib().orc_walker_reset(self._h, obs.ctypes.data)
         return obs

@@ -230,6 +230,22 @@ def test_lunar_oracle_is_deterministic_and_seed_fanout_is_seed_plus_index():
         assert np.array_equal(oa[2], ob[0])
 
 
+@pytest.mark.parametrize("kind", ["lunar", "walker"])
+def test_oracle_window_stands_in_for_a_slice_of_the_batch(kind):
+    """reset(seed, first=lo) of an m-env oracle seeds env k with seed + lo + k: it then steps exactly as envs
+    [lo, lo + m) of a larger batch (how the GPU tests check windows of batches too large for the oracle)."""
+    make = orc.OracleLunar if kind == "lunar" else orc.OracleWalker
+    big, win = make(24), make(8)
+    assert np.array_equal(big.reset(seed=7)[16:], win.reset(seed=7, first=16))
+    rng = np.random.default_rng(1)
+    for _ in range(40):
+        act = rng.integers(0, 4, size=24) if kind == "lunar" else rng.uniform(-1, 1, size=(24, 4)).astype(np.float32)
+        for x, y in zip(big.step(act), win.step(act[16:])):
+            assert np.array_equal(x[16:], y)
+    big.close()
+    win.close()
+
+
 def test_walker_oracle_invariants():
     """bipedal_walker.py:517-606: obs shape/dtype, lidar fractions in [0, 1], leg contact flags binary, reward
     -100 exactly on termination, truncation only from the TimeLimit."""
