@@ -112,6 +112,7 @@ SIGNATURES = {
     "b200gym_rms_apply_obs": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i32, _vp]),
     "b200gym_rms_apply_reward": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
                                         _vp]),
+    "b200gym_sample_space": (_i32, [_vp, _i64, _i32, _i64, _vp, _vp, _vp, _vp]),
     "b200gym_box2d_overflows": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_box2d_list_counts": (_i32, [_vp, _vp, _i32, _vp, _vp]),
     "b200gym_selftest_trig": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp]),

@@ -36,6 +36,7 @@
 #include "box2d_consts.h"
 #include "per_env.cuh"
 #include "rng.cuh"
+#include "space_sample.cuh"
 
 using namespace bgym;
 
@@ -1444,6 +1445,21 @@ static int launch_reset(b200gym *h, const uint8_t *mask, const double *bounds, f
 }
 
 // ---------------------------------------------------------------------------
+// space_sample_kernel: `envs.action_space.sample()` of the batched action space (space_sample.cuh: one 16-byte
+// vector per thread and round, grid-strided; a table jump to the first vector, one multiply-add to each next one)
+// ---------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads) space_sample_kernel(const SampleArgs a, T *__restrict__ out) {
+    __shared__ LcgJumpTable table;   // rows [0, jump_digits) of kLcgJump, 512 B each
+    const uint4 *src = reinterpret_cast<const uint4 *>(&kLcgJump);
+    uint4 *dst = reinterpret_cast<uint4 *>(&table);
+    for (int i = threadIdx.x; i < a.jump_digits * 32; i += kSampleThreads) dst[i] = src[i];
+    __syncthreads();
+    sample_thread<T>(a, out, (int64_t)blockIdx.x * kSampleThreads + threadIdx.x, (int64_t)gridDim.x * kSampleThreads,
+                     table);
+}
+
+// ---------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------
 struct DeviceGuard {
@@ -2001,6 +2017,45 @@ extern "C" int b200gym_rms_apply_reward(const double *reward_dev, double *out_de
     rms_apply_kernel<true><<<norm_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(
         nullptr, nullptr, reward_dev, out_dev, returns_dev, terminated_dev, truncated_dev, n, 1, stats_dev, stats_next_dev,
         scratch_dev, scratch_next_dev, batch_count, epsilon, 1);
+    CK(nullptr, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int cols, int64_t n_choices,
+                                    const double *low_host, const double *high_host, void *out_dev, void *stream) {
+    if (!pcg64 || !out_dev || rows <= 0 || cols <= 0 || cols > kSampleMaxCols || n_choices < 0 ||
+        (n_choices > 0 && cols != 1) || (n_choices == 0 && (!low_host || !high_host)) ||
+        rows > INT64_MAX / kSampleMaxCols)
+        return fail(nullptr, "b200gym_sample_space: bad argument (MultiDiscrete needs cols = 1, a Box 1 <= cols <= %d "
+                             "and its bounds)", kSampleMaxCols);
+    if ((uintptr_t)out_dev % 16)
+        return fail(nullptr, "b200gym_sample_space: out is not 16-byte aligned");
+    SampleArgs a{};
+    a.start.state = make_u128(pcg64[0], pcg64[1]);
+    a.start.inc = make_u128(pcg64[2], pcg64[3]);
+    a.total = rows * cols;
+    a.cols = cols;
+    a.n_choices = (double)n_choices;
+    if (n_choices == 0) {
+        for (int c = 0; c < cols; c++) {
+            a.low[c] = low_host[c];
+            a.high[c] = high_host[c];
+            if (!std::isfinite(a.low[c]) || !std::isfinite(a.high[c]) || !std::isfinite(a.high[c] - a.low[c]))
+                return fail(nullptr, "b200gym_sample_space: column %d is not a bounded Box (low %g, high %g)", c,
+                            a.low[c], a.high[c]);
+        }
+    }
+    const int dev = device_of(out_dev);
+    if (dev < 0) return fail(nullptr, "b200gym_sample_space: out is not a device pointer");
+    DeviceGuard guard(dev);
+    const int vec = n_choices > 0 ? 2 : 4;
+    const int64_t blocks = sample_blocks(a.total, vec);
+    sample_setup(a, blocks * kSampleThreads, vec);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_choices > 0)
+        space_sample_kernel<long long><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, (long long *)out_dev);
+    else
+        space_sample_kernel<float><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, (float *)out_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
 }

@@ -63,6 +63,81 @@ __host__ __device__ __forceinline__ double pcg64_uniform(Pcg64 &g, double low, d
     return low + range * pcg64_next_double(g);
 }
 
+// ---- jump-ahead: the state `delta` draws later, in O(log delta) ----
+// `delta` steps of the LCG are the affine map state -> mult * state + geo * inc, where mult = A^delta and
+// geo = A^(delta-1) + ... + A + 1 (mod 2^128) do not depend on inc.
+struct LcgMap {
+    u128 mult;
+    u128 geo;
+};
+
+// `first`, then `second`
+__host__ __device__ constexpr LcgMap lcg_compose(LcgMap first, LcgMap second) {
+    return {second.mult * first.mult, second.mult * first.geo + second.geo};
+}
+
+// pcg_advance_lcg_128 (PCG's square-and-multiply over the bits of delta) with inc = 1
+__host__ __device__ constexpr LcgMap lcg_jump_map(u128 delta) {
+    u128 cur_mult = ((u128)0x2360ED051FC65DA4ULL << 64) | (u128)0x4385DF649FCCF645ULL, cur_plus = 1;
+    u128 acc_mult = 1, acc_plus = 0;
+    while (delta > 0) {
+        if (delta & 1) {
+            acc_mult *= cur_mult;
+            acc_plus = acc_plus * cur_mult + cur_plus;
+        }
+        cur_plus = (cur_mult + 1) * cur_plus;
+        cur_mult *= cur_mult;
+        delta >>= 1;
+    }
+    return {acc_mult, acc_plus};
+}
+
+__host__ __device__ __forceinline__ void pcg64_apply(Pcg64 &g, const LcgMap &m) {
+    g.state = m.mult * g.state + m.geo * g.inc;
+}
+
+// numpy's PCG64.advance(delta) on the state words (the buffered 32-bit draw is not numpy's to clear here)
+__host__ __device__ inline void pcg64_jump(Pcg64 &g, u128 delta) { pcg64_apply(g, lcg_jump_map(delta)); }
+
+// The jump a sampling thread makes to the start of its elements, one table entry per non-zero hex digit of delta:
+// m[k][d] is the map of d * 16^k steps.  8 KB, built by the compiler, read-only in global memory.
+struct LcgJumpTable {
+    LcgMap m[16][16];
+};
+
+__host__ __device__ constexpr LcgJumpTable make_lcg_jump_table() {
+    LcgJumpTable t{};
+    for (int k = 0; k < 16; k++) {
+        const LcgMap unit = k == 0 ? lcg_jump_map(1) : lcg_compose(t.m[k - 1][15], t.m[k - 1][1]);
+        t.m[k][0] = LcgMap{1, 0};
+        t.m[k][1] = unit;
+        for (int d = 2; d < 16; d++) t.m[k][d] = lcg_compose(t.m[k][d - 1], unit);
+    }
+    return t;
+}
+
+static __device__ const LcgJumpTable kLcgJump = make_lcg_jump_table();
+
+// pcg64_jump for a 64-bit delta through a copy of kLcgJump (the kernels stage the rows they use in shared memory):
+// 2 multiplies per non-zero hex digit instead of ~3 per bit
+__host__ __device__ __forceinline__ void pcg64_jump_table(Pcg64 &g, uint64_t delta, const LcgJumpTable &table) {
+    for (int k = 0; delta != 0; k++, delta >>= 4)
+        if (delta & 15) pcg64_apply(g, table.m[k][delta & 15]);
+}
+
+// ---- one element of a batched action space's sample(): one 64-bit draw each, in C order ----
+// MultiDiscrete.sample: (random(shape) * nvec).astype(int64) (gym/spaces/multi_discrete.py:123); the cast rounds
+// toward zero
+__host__ __device__ __forceinline__ long long sample_multidiscrete(Pcg64 &g, double n) {
+    return (long long)(pcg64_next_double(g) * n);
+}
+
+// Box.sample of a bounded float Box: uniform(low, high).astype(float32) (gym/spaces/box.py:171-222); low and high
+// are the float32 bounds widened to float64, the cast rounds to nearest
+__host__ __device__ __forceinline__ float sample_box(Pcg64 &g, double low, double high) {
+    return (float)pcg64_uniform(g, low, high);
+}
+
 // SeedSequence(seed).generate_state(4, uint64) for a seed given as four
 // little-endian uint32 entropy words (seed < 2^128; shorter seeds are
 // zero-padded, which hashes identically to numpy's own padding).

@@ -225,6 +225,44 @@ class MultiDiscrete(Space):
         return isinstance(other, MultiDiscrete) and np.all(self.nvec == other.nvec)
 
 
+PCG64_MULT = 0x2360ED051FC65DA44385DF649FCCF645
+_MASK128 = (1 << 128) - 1
+
+
+def pcg64_jump(state, inc, delta):
+    """The PCG64 LCG state ``delta`` draws after ``state`` (PCG's pcg_advance_lcg_128: square-and-multiply over the
+    bits of ``delta``, taken mod 2**128 like ``PCG64.advance``)."""
+    cur_mult, cur_plus, acc_mult, acc_plus = PCG64_MULT, inc & _MASK128, 1, 0
+    delta &= _MASK128
+    while delta:
+        if delta & 1:
+            acc_mult = acc_mult * cur_mult & _MASK128
+            acc_plus = (acc_plus * cur_mult + cur_plus) & _MASK128
+        cur_plus = (cur_mult + 1) * cur_plus & _MASK128
+        cur_mult = cur_mult * cur_mult & _MASK128
+        delta >>= 1
+    return (acc_mult * state + acc_plus) & _MASK128
+
+
+def pcg64_state(bit_generator):
+    """``bit_generator.state`` of a PCG64 bit generator; ``error.Error`` for any other kind (Philox, PCG64DXSM, ...),
+    whose streams the device does not reproduce."""
+    state = bit_generator.state
+    if state.get("bit_generator") != "PCG64":
+        raise error.Error(f"device sampling reproduces numpy's PCG64 stream only; this space's generator is "
+                          f"{state.get('bit_generator')}")
+    return state
+
+
+def pcg64_skip(bit_generator, state, count):
+    """Move a PCG64 bit generator from ``state`` (as ``pcg64_state`` returned it) to where ``count`` 64-bit draws
+    leave it.  The buffered 32-bit draw (``has_uint32`` / ``uinteger``) stays as it was, as the draws of ``random`` /
+    ``uniform`` leave it -- ``PCG64.advance`` would clear it."""
+    words = state["state"]
+    state["state"] = dict(words, state=pcg64_jump(words["state"], words["inc"], count))
+    bit_generator.state = state
+
+
 def batch_space(space, n=1):
     """gym/vector/utils/spaces.py:46-68: Box tiles its bounds, Discrete -> MultiDiscrete([n]*N)."""
     if isinstance(space, Box):

@@ -31,7 +31,7 @@ import numpy as np
 from gym_b200 import _lib, envs as _envs, error
 from gym_b200.registration import spec as _spec
 from gym_b200.snapshot import FORMAT_VERSION, EnvSnapshot, check_compatible, env_config, host_indices
-from gym_b200.spaces import batch_space
+from gym_b200.spaces import batch_space, pcg64_skip, pcg64_state
 
 _STATE_DEFAULT, _STATE_WAITING_RESET, _STATE_WAITING_STEP = "default", "reset", "step"
 
@@ -144,6 +144,7 @@ class B200VectorEnv:
         self.obs_dim = self.single_observation_space.shape[0]
         self.discrete = hasattr(self.single_action_space, "n")
         self.act_dim = 0 if self.discrete else self.single_action_space.shape[0]
+        self._sample_cache = None   # (single action space, its sample_actions plan)
 
         lib = _lib.load()
         torch = _torch()
@@ -456,6 +457,52 @@ class B200VectorEnv:
         if count.value:
             raise error.InvalidAction(f"{count.value} out-of-range Discrete action(s) were passed to step()")
         return 0
+
+    # ------------------------------------------------------------------ action sampling
+    def _sample_plan(self):
+        """(n_choices, cols, low, high) of the single action space, checked once per space object: Discrete(n) from 0
+        batches to MultiDiscrete (n_choices = n), a bounded float32 Box of shape (A,) to a Box of shape (N, A)."""
+        single = self.single_action_space
+        if self._sample_cache is not None and self._sample_cache[0] is single:
+            return self._sample_cache[1]
+        if hasattr(single, "n") and int(getattr(single, "start", 0)) == 0:
+            plan = (int(single.n), 1, None, None)
+        elif (hasattr(single, "low") and np.dtype(single.dtype) == np.float32 and len(single.shape) == 1
+              and 1 <= single.shape[0] <= 32 and np.all(np.isfinite(single.low)) and np.all(np.isfinite(single.high))):
+            plan = (0, int(single.shape[0]), np.ascontiguousarray(single.low, dtype=np.float64),
+                    np.ascontiguousarray(single.high, dtype=np.float64))
+        else:
+            raise error.Error(f"sample_actions supports Discrete(n) and bounded float32 Box action spaces, not {single!r}")
+        self._sample_cache = (single, plan)
+        return plan
+
+    def sample_actions(self):
+        """``self.action_space.sample()``, drawn on the device: the same values bit for bit (int64 (N,) for Discrete
+        kinds, float32 (N, A) for continuous ones) as a tensor on ``self.device``, enqueued on torch's current stream
+        with no synchronisation, ready for ``step()``.  The space's generator ends where ``sample()`` would leave it,
+        so host and device sampling interleave freely.  ``backend="numpy"`` returns ``self.action_space.sample()``."""
+        self._assert_open("sample_actions")
+        space = self.action_space
+        if self.backend == "numpy":
+            return space.sample()
+        n_choices, cols, low, high = self._sample_plan()
+        shape = (self.num_envs,) if n_choices else (self.num_envs, cols)
+        if (type(space).__name__ != ("MultiDiscrete" if n_choices else "Box") or tuple(space.shape) != shape
+                or np.dtype(space.dtype) != (np.int64 if n_choices else np.float32)):
+            raise error.Error(f"action_space {space!r} is no longer the batched space of {self.single_action_space!r}")
+        bit_generator = space.np_random.bit_generator
+        state = pcg64_state(bit_generator)
+        s, inc = state["state"]["state"], state["state"]["inc"]
+        mask = (1 << 64) - 1
+        words = (ctypes.c_uint64 * 4)(s >> 64, s & mask, inc >> 64, inc & mask)
+        torch = _torch()
+        out = torch.empty(shape, dtype=torch.int64 if n_choices else torch.float32, device=self.device)
+        _lib.check(self._lib.b200gym_sample_space(words, self.num_envs, cols, n_choices,
+                                                  None if low is None else low.ctypes.data,
+                                                  None if high is None else high.ctypes.data,
+                                                  ctypes.c_void_p(out.data_ptr()), self._stream()))
+        pcg64_skip(bit_generator, state, out.numel())
+        return out
 
     # ------------------------------------------------------------------ state access
     def get_state(self):

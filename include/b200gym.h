@@ -361,6 +361,22 @@ int b200gym_rms_apply_reward(const double *reward_dev, double *out_dev, double *
                              void *stream);
 
 /*
+ * `envs.action_space.sample()` of a batched action space, bit for bit, as ONE launch on `stream`: MultiDiscrete
+ * (gym/spaces/multi_discrete.py:123: `(random(shape) * nvec).astype(int64)`, every element with the same n) and a
+ * bounded float32 Box (gym/spaces/box.py:171-222: `uniform(low, high, size).astype(float32)`) -- the batches
+ * gym/vector/utils/spaces.py:46-68 makes of Discrete(n) and Box action spaces.  Both take one 64-bit draw of the
+ * space's numpy PCG64 stream per element, in C order.
+ *   pcg64        {state_hi, state_lo, inc_hi, inc_lo} of the space's bit generator before the call (passed by value:
+ *                the caller moves its generator rows * cols draws ahead itself)
+ *   n_choices    MultiDiscrete: n (cols must be 1), out is int64 [rows]; 0: Box, out is float32 [rows][cols]
+ *   low_host, high_host  Box only: the float32 bounds of each of the cols (<= 32) columns, widened to float64
+ *   out_dev      16-byte aligned device buffer; the launch runs on the device that owns it
+ * Stateless: errors through b200gym_last_error(NULL).  Asynchronous.
+ */
+int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int cols, int64_t n_choices, const double *low_host,
+                         const double *high_host, void *out_dev, void *stream);
+
+/*
  * Box2D tasks: number of envs in which a touching (body, ground fixture) pair was ever dropped because the scene's
  * manifold table was full (8 pairs for LunarLander*, 10 for BipedalWalker*; real Box2D has no such limit).  The
  * dropped pair is treated as not touching -- the CPU oracle applies the identical rule -- so this counts
