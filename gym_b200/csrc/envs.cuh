@@ -72,11 +72,13 @@ __constant__ double kCosCoef[6] = {4.16666666666666019037e-02, -1.38888888888741
                                    2.08757232129817482790e-09, -1.13596475577881948265e-11};
 
 // the library path of sincos_small, out of line: it only runs in plain-Env mode after termination, and inlined it
-// costs the 32-register hot loop of the step kernels spill slots
-__device__ __noinline__ void sincos_library(double x, double *sn, double *cs) {
-    *sn = gt::sin(x);
-    *cs = gt::cos(x);
-}
+// costs the 32-register hot loop of the step kernels spill slots.  It returns both values in registers: with pointer
+// out-parameters sn and cs would live in the caller's stack frame, and every step -- library path or not -- would
+// store them to local memory and load cos back on the dependence chain
+struct SinCos {
+    double sn, cs;
+};
+__device__ __noinline__ SinCos sincos_library(double x) { return SinCos{gt::sin(x), gt::cos(x)}; }
 
 __device__ __forceinline__ void sincos_small(double x, double &sn, double &cs) {
     if (fabs(x) < 0.7) {
@@ -100,7 +102,9 @@ __device__ __forceinline__ void sincos_small(double x, double &sn, double &cs) {
         const double hz = fma(0.5, z, -qx);
         cs = (1.0 - qx) - (hz - z * zr);
     } else {
-        sincos_library(x, &sn, &cs);
+        const SinCos r = sincos_library(x);
+        sn = r.sn;
+        cs = r.cs;
     }
 }
 

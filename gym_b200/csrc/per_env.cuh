@@ -140,7 +140,7 @@ __device__ __forceinline__ void episode_account(const StepArgs &a, I i, double r
 }
 
 // Where the results of env i go.  DirectSink: straight to the caller's arrays (and, when peers are mapped,
-// to theirs) with per-thread stores.  The kernels that stage their outputs in shared memory have sinks of their own
+// to theirs) with per-thread stores; final_obs rows (info["final_observation"]) are never peer-mapped.  The kernels that stage their outputs in shared memory have sinks of their own
 // (b200gym.cu: StagedSink, InPlaceSink).
 // PEERS = false: the caller knows there are no peer-mapped destinations (single-GPU step), so the per-destination
 // loops and their constant-bank traffic disappear from the hot loop.
@@ -164,6 +164,10 @@ struct DirectSinkT {
     }
     template <typename I>
     __device__ __forceinline__ void elapsed(I i, int32_t e) const { a.elapsed[i] = e; }
+    template <int D, typename I>
+    __device__ __forceinline__ void final_obs(I i, const float (&v)[D]) const {
+        if (a.final_obs) store_row<D>(a.final_obs, i, v);
+    }
 };
 using DirectSink = DirectSinkT<true>;
 
@@ -223,7 +227,7 @@ __device__ __forceinline__ bool advance_env(const StepArgs &a, const Sink &sink,
     sink.scalars(i, reward, terminated ? 1 : 0, truncated ? 1 : 0);
     if constexpr (EP) episode_account(a, i, reward, terminated || truncated);
     if (needs_reset) {
-        if (a.final_obs) store_row<E::D>(a.final_obs, i, obs);           // info["final_observation"]
+        sink.template final_obs<E::D>(i, obs);                            // info["final_observation"]
     } else {
         sink.template state<E::S>(i, s);
         sink.elapsed(i, elapsed);
