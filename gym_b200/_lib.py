@@ -55,6 +55,30 @@ class HostIO(ctypes.Structure):
     ]
 
 
+SUBENV_MAX_STAGES = 5
+# enum b200gym_subenv_op
+SUB_EPISODE, SUB_NORM_OBS, SUB_NORM_REWARD, SUB_CLIP_OBS, SUB_CLIP_REWARD = 0, 1, 2, 3, 4
+
+
+class Subenv(ctypes.Structure):
+    """struct b200gym_subenv"""
+    _fields_ = [
+        ("num_stages", ctypes.c_int32),
+        ("op", ctypes.c_int32 * SUBENV_MAX_STAGES),
+        ("raw_reward_type", ctypes.c_int32),
+        ("int_reward_on_fall", ctypes.c_int32),
+        ("p0", ctypes.c_double * SUBENV_MAX_STAGES),
+        ("p1", ctypes.c_double * SUBENV_MAX_STAGES),
+        ("obs_stats", ctypes.c_void_p),
+        ("rew_stats", ctypes.c_void_p),
+        ("ep_return", ctypes.c_void_p),
+        ("ep_length", ctypes.c_void_p),
+        ("clip_action", ctypes.c_int32),
+        ("act_low", ctypes.c_float * 4),
+        ("act_high", ctypes.c_float * 4),
+    ]
+
+
 class P2PLayout(ctypes.Structure):
     """struct b200gym_p2p_layout"""
     _fields_ = [
@@ -113,6 +137,11 @@ SIGNATURES = {
     "b200gym_rms_apply_reward": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
                                         _vp]),
     "b200gym_sample_space": (_i32, [_vp, _i64, _i32, _i64, _vp, _vp, _vp, _vp]),
+    "b200gym_subenv_set": (_i32, [_vp, ctypes.POINTER(Subenv)]),
+    "b200gym_subenv_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200gym_subenv_reset": (_i32, [_vp, _vp, _vp, _vp]),
+    "b200gym_clip_actions": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "b200gym_subenv_host_buffers": (_i32, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp)]),
     "b200gym_box2d_overflows": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_box2d_list_counts": (_i32, [_vp, _vp, _i32, _vp, _vp]),
     "b200gym_selftest_trig": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp]),

@@ -37,6 +37,7 @@
 #include "per_env.cuh"
 #include "rng.cuh"
 #include "space_sample.cuh"
+#include "subenv.cuh"
 
 using namespace bgym;
 
@@ -114,6 +115,24 @@ struct b200gym {
     unsigned long long *snap_bad = nullptr;       // page-locked, device-mapped word: an out-of-range snapshot index was met
     unsigned long long *snap_bad_dev = nullptr;   // device alias
     unsigned char *snap_scratch = nullptr;        // b200gym_clone: n rows
+    // per-env wrapper chain (b200gym_subenv_set); the host-buffer path runs it inside its calls
+    struct {
+        bool on = false, clip = false, norm_obs = false, episode = false;
+        SubenvArgs args{};
+        float act_low[4] = {}, act_high[4] = {};
+        double *final64 = nullptr;                // page-locked, mapped staging of the float64 final observations
+        float *ep_r = nullptr;                    // ... of infos["final_info"][i]["episode"]["r"] / ["l"]
+        int32_t *ep_l = nullptr;
+        double *final64_dev = nullptr;            // their device aliases
+        float *ep_r_dev = nullptr;
+        int32_t *ep_l_dev = nullptr;
+        // host-buffer path with a chain: the step and the chain run on these HBM copies of the outputs, which then go
+        // to the mapped staging buffers as bulk copies (the terminal rows and episode fields of the finishing envs
+        // are written there by the chain directly)
+        float *obs = nullptr, *fin = nullptr;
+        double *reward = nullptr;
+        uint8_t *term = nullptr, *trunc = nullptr;
+    } sub;
     mutable std::string err;
 };
 
@@ -1777,6 +1796,14 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     cudaFree(h->toi_mid);
     if (h->snap_bad) cudaFreeHost(h->snap_bad);
     cudaFree(h->snap_scratch);
+    if (h->sub.final64) cudaFreeHost(h->sub.final64);
+    if (h->sub.ep_r) cudaFreeHost(h->sub.ep_r);
+    if (h->sub.ep_l) cudaFreeHost(h->sub.ep_l);
+    cudaFree(h->sub.obs);
+    cudaFree(h->sub.fin);
+    cudaFree(h->sub.reward);
+    cudaFree(h->sub.term);
+    cudaFree(h->sub.trunc);
     if (h->p2p.base) {
         for (int r = 0; r < h->p2p.world; r++)
             if (r != h->p2p.rank && h->p2p.peer[r]) cudaIpcCloseMemHandle(h->p2p.peer[r]);
@@ -2222,6 +2249,165 @@ extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int c
     return 0;
 }
 
+// ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------
+struct ActBounds {
+    float lo[4], hi[4];
+};
+
+// envs [first, first + count)
+__global__ void __launch_bounds__(kThreads) subenv_step_kernel(const SubenvArgs a, int64_t first, int64_t count,
+                                                               float *obs, double *reward, const uint8_t *term,
+                                                               const uint8_t *trunc, const float *fin, float *fin_out,
+                                                               double *fin64, float *ep_r, int32_t *ep_l) {
+    const int64_t k = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (k < count) subenv_step_env(a, first + k, obs, reward, term, trunc, fin, fin_out, fin64, ep_r, ep_l);
+}
+
+__global__ void __launch_bounds__(kThreads) subenv_reset_kernel(const SubenvArgs a, const uint8_t *mask, float *obs) {
+    const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i < a.n && (!mask || mask[i])) subenv_reset_env(a, i, obs);
+}
+
+// ClipAction (clip_action.py:31-40): np.clip(action, low, high) in float32, before the env sees the action
+__global__ void __launch_bounds__(kThreads) clip_action_kernel(const float *in, float *out, int64_t total, int A,
+                                                               const ActBounds b) {
+    const int64_t e = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (e < total) {
+        const int k = (int)(e % A);
+        out[e] = np_clipf(in[e], b.lo[k], b.hi[k]);
+    }
+}
+
+static int launch_clip_actions(const b200gym *h, const float *in, float *out, int64_t rows, int A, const float *lo,
+                               const float *hi, cudaStream_t st) {
+    ActBounds b{};
+    for (int k = 0; k < A; k++) { b.lo[k] = lo[k]; b.hi[k] = hi[k]; }
+    const int64_t total = rows * A;
+    clip_action_kernel<<<blocks_for(total), kThreads, 0, st>>>(in, out, total, A, b);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+static int launch_subenv_step(b200gym *h, int64_t first, int64_t count, float *obs, double *reward,
+                              const uint8_t *term, const uint8_t *trunc, const float *fin, float *fin_out,
+                              double *fin64, float *ep_r, int32_t *ep_l, cudaStream_t st) {
+    subenv_step_kernel<<<blocks_for(count), kThreads, 0, st>>>(h->sub.args, first, count, obs, reward, term, trunc, fin,
+                                                               fin_out, fin64, ep_r, ep_l);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+static int launch_subenv_reset(b200gym *h, const uint8_t *mask, float *obs, cudaStream_t st) {
+    subenv_reset_kernel<<<blocks_for(h->n), kThreads, 0, st>>>(h->sub.args, mask, obs);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain) {
+    if (!h) return fail(h, "b200gym_subenv_set: null handle");
+    if (!chain) {
+        h->sub.on = h->sub.clip = h->sub.norm_obs = h->sub.episode = false;
+        return 0;
+    }
+    if (!h->cfg.autoreset) return fail(h, "b200gym_subenv_set: a wrapper chain needs autoreset");
+    if (chain->num_stages < 0 || chain->num_stages > B200GYM_SUBENV_MAX_STAGES)
+        return fail(h, "b200gym_subenv_set: %d stages (at most %d)", chain->num_stages, B200GYM_SUBENV_MAX_STAGES);
+    SubenvArgs a{};
+    a.num_stages = chain->num_stages;
+    a.D = h->D;
+    a.n = h->n;
+    a.obs_stats = chain->obs_stats_dev;
+    a.rew_stats = chain->rew_stats_dev;
+    a.ep_return = chain->ep_return_dev;
+    a.ep_length = chain->ep_length_dev;
+    if (chain->raw_reward_type < kRewardPy || chain->raw_reward_type > kRewardF32)
+        return fail(h, "b200gym_subenv_set: unknown raw reward type %d", chain->raw_reward_type);
+    a.raw_reward_type = chain->raw_reward_type;
+    a.int_reward_on_fall = chain->int_reward_on_fall != 0;
+    unsigned seen = 0;
+    for (int s = 0; s < a.num_stages; s++) {
+        const int op = chain->op[s];
+        if (op < B200GYM_SUB_EPISODE || op > B200GYM_SUB_CLIP_REWARD || (seen >> op & 1u))
+            return fail(h, "b200gym_subenv_set: stage %d has an unknown or repeated op %d", s, op);
+        seen |= 1u << op;
+        if ((op == B200GYM_SUB_NORM_OBS && !a.obs_stats) || (op == B200GYM_SUB_NORM_REWARD && !a.rew_stats) ||
+            (op == B200GYM_SUB_EPISODE && (!a.ep_return || !a.ep_length)))
+            return fail(h, "b200gym_subenv_set: stage %d needs its state buffers", s);
+        a.op[s] = op;
+        a.p0[s] = chain->p0[s];
+        a.p1[s] = chain->p1[s];
+    }
+    if (chain->clip_action && h->A == 0) return fail(h, "b200gym_subenv_set: ClipAction needs a Box action space");
+    h->sub.args = a;
+    h->sub.clip = chain->clip_action != 0;
+    for (int k = 0; k < h->A && k < 4; k++) {
+        h->sub.act_low[k] = chain->act_low[k];
+        h->sub.act_high[k] = chain->act_high[k];
+    }
+    h->sub.norm_obs = (seen >> B200GYM_SUB_NORM_OBS & 1u) != 0;
+    h->sub.episode = (seen >> B200GYM_SUB_EPISODE & 1u) != 0;
+    h->sub.on = true;
+    return 0;
+}
+
+extern "C" int b200gym_subenv_step(b200gym_t *h, float *obs_dev, double *reward_dev, const uint8_t *terminated_dev,
+                                   const uint8_t *truncated_dev, float *final_obs_dev, double *final_obs64_dev,
+                                   float *episode_r_dev, int32_t *episode_l_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_subenv_step: null handle");
+    if (!h->sub.on) return fail(h, "b200gym_subenv_step: no wrapper chain is set");
+    if (!obs_dev || !reward_dev || !terminated_dev || !truncated_dev || !final_obs_dev ||
+        (h->sub.norm_obs && !final_obs64_dev) || (h->sub.episode && (!episode_r_dev || !episode_l_dev)))
+        return fail(h, "b200gym_subenv_step: null buffer");
+    DeviceGuard guard(h->device);
+    return launch_subenv_step(h, 0, h->n, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev,
+                              final_obs_dev, final_obs64_dev, episode_r_dev, episode_l_dev, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_subenv_reset(b200gym_t *h, const uint8_t *mask_dev, float *obs_dev, void *stream) {
+    if (!h || !obs_dev) return fail(h, "b200gym_subenv_reset: null argument");
+    if (!h->sub.on) return fail(h, "b200gym_subenv_reset: no wrapper chain is set");
+    DeviceGuard guard(h->device);
+    return launch_subenv_reset(h, mask_dev, obs_dev, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_clip_actions(const float *in_dev, float *out_dev, int64_t n, int act_dim, const float *low_host,
+                                    const float *high_host, void *stream) {
+    if (!in_dev || !out_dev || !low_host || !high_host || n <= 0 || act_dim < 1 || act_dim > 4)
+        return fail(nullptr, "b200gym_clip_actions: bad argument (1 <= act_dim <= 4)");
+    const int dev = device_of(out_dev);
+    if (dev < 0) return fail(nullptr, "b200gym_clip_actions: out is not a device pointer");
+    DeviceGuard guard(dev);
+    return launch_clip_actions(nullptr, in_dev, out_dev, n, act_dim, low_host, high_host, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_out, float **episode_r_out,
+                                           int32_t **episode_l_out) {
+    if (!h || !final_obs64_out || !episode_r_out || !episode_l_out)
+        return fail(h, "b200gym_subenv_host_buffers: null argument");
+    DeviceGuard guard(h->device);
+    const size_t n = (size_t)h->n;
+    if (!h->sub.final64) {
+        CK(h, cudaHostAlloc((void **)&h->sub.final64, n * h->D * sizeof(double), cudaHostAllocMapped));
+        CK(h, cudaHostAlloc((void **)&h->sub.ep_r, n * sizeof(float), cudaHostAllocMapped));
+        CK(h, cudaHostAlloc((void **)&h->sub.ep_l, n * sizeof(int32_t), cudaHostAllocMapped));
+        memset(h->sub.final64, 0, n * h->D * sizeof(double));
+        memset(h->sub.ep_r, 0, n * sizeof(float));
+        memset(h->sub.ep_l, 0, n * sizeof(int32_t));
+        CK(h, cudaHostGetDevicePointer((void **)&h->sub.final64_dev, h->sub.final64, 0));
+        CK(h, cudaHostGetDevicePointer((void **)&h->sub.ep_r_dev, h->sub.ep_r, 0));
+        CK(h, cudaHostGetDevicePointer((void **)&h->sub.ep_l_dev, h->sub.ep_l, 0));
+        CK(h, cudaMalloc((void **)&h->sub.obs, n * h->D * sizeof(float)));
+        CK(h, cudaMalloc((void **)&h->sub.fin, n * h->D * sizeof(float)));
+        CK(h, cudaMalloc((void **)&h->sub.reward, n * sizeof(double)));
+        CK(h, cudaMalloc((void **)&h->sub.term, n));
+        CK(h, cudaMalloc((void **)&h->sub.trunc, n));
+    }
+    *final_obs64_out = h->sub.final64;
+    *episode_r_out = h->sub.ep_r;
+    *episode_l_out = h->sub.ep_l;
+    return 0;
+}
+
 // ---- host-buffer path -------------------------------------------------------
 // The staging buffers are page-locked AND mapped into the device's address space: the step kernel writes its
 // results straight into host memory (for the classic-control kinds as bulk shared->global copies of 256-env
@@ -2284,8 +2470,10 @@ static int step_host_enqueue(b200gym *h, const void *actions_host, int action_dt
         if (v >= 1 && v <= 64) chunks = v;
     }
     const int64_t per = ((n + chunks - 1) / chunks + kThreads - 1) / kThreads * kThreads;
-    StepArgs a = make_args(h, h->dio.actions, h->dio.obs, h->dio.reward, h->dio.terminated, h->dio.truncated,
-                           want_final ? h->dio.final_obs : nullptr);
+    const bool chain = h->sub.on;
+    StepArgs a = chain ? make_args(h, h->dio.actions, h->sub.obs, h->sub.reward, h->sub.term, h->sub.trunc, h->sub.fin)
+                       : make_args(h, h->dio.actions, h->dio.obs, h->dio.reward, h->dio.terminated, h->dio.truncated,
+                                   want_final ? h->dio.final_obs : nullptr);
     a.bulk_sink = 1;
     int c = 0;
     for (int64_t lo = 0; lo < n; lo += per, c++) {
@@ -2293,11 +2481,27 @@ static int step_host_enqueue(b200gym *h, const void *actions_host, int action_dt
         cudaStream_t st = h->hstream[c & 1];
         CK(h, cudaMemcpyAsync((char *)h->dio.actions + lo * asz, (const char *)actions_host + lo * asz, cnt * asz,
                               cudaMemcpyHostToDevice, st));
+        if (h->sub.on && h->sub.clip) {
+            float *act = (float *)h->dio.actions + lo * h->A;
+            if (launch_clip_actions(h, act, act, cnt, h->A, h->sub.act_low, h->sub.act_high, st)) return 1;
+        }
         a.first = lo;
         a.count = cnt;
         a.reset_count = h->reset_count ? h->reset_count + (c % kResetSlots) : nullptr;
         a.toi_count = h->toi_count ? h->toi_count + (c % kResetSlots) : nullptr;
         if (launch_step(h, a, action_dtype, st)) return 1;
+        if (chain) {   // the chain over this chunk in HBM, then its dense outputs to the staging buffers in bulk
+            const size_t D = (size_t)h->D;
+            if (launch_subenv_step(h, lo, cnt, h->sub.obs, h->sub.reward, h->sub.term, h->sub.trunc, h->sub.fin,
+                                   h->dio.final_obs, h->sub.final64_dev, h->sub.ep_r_dev, h->sub.ep_l_dev, st))
+                return 1;
+            CK(h, cudaMemcpyAsync(h->hio.obs + lo * D, h->sub.obs + lo * D, cnt * D * sizeof(float),
+                                  cudaMemcpyDeviceToHost, st));
+            CK(h, cudaMemcpyAsync(h->hio.reward + lo, h->sub.reward + lo, cnt * sizeof(double), cudaMemcpyDeviceToHost,
+                                  st));
+            CK(h, cudaMemcpyAsync(h->hio.terminated + lo, h->sub.term + lo, cnt, cudaMemcpyDeviceToHost, st));
+            CK(h, cudaMemcpyAsync(h->hio.truncated + lo, h->sub.trunc + lo, cnt, cudaMemcpyDeviceToHost, st));
+        }
     }
     if (c > 1) {  // stream 0 also waits for the chunks of stream 1
         CK(h, cudaEventRecord(h->hevent, h->hstream[1]));
@@ -2321,7 +2525,10 @@ extern "C" int b200gym_step_host(b200gym_t *h, const void *actions_host, int act
         actions_host = h->hio.actions;
         action_dtype = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
     }
-    const bool want_final = final_obs_host != nullptr && h->cfg.autoreset;
+    // a wrapper chain reads the terminal rows of the finishing envs, and writes the float64 ones to its own staging
+    if (h->sub.on && !h->sub.final64)
+        return fail(h, "b200gym_step_host: call b200gym_subenv_host_buffers before stepping with a wrapper chain");
+    const bool want_final = (final_obs_host != nullptr || h->sub.on) && h->cfg.autoreset;
     const int rc = step_host_enqueue(h, actions_host, action_dtype, want_final);
     // drain both streams whatever happened: nothing may still be writing into host memory when we return
     const cudaError_t e1 = cudaStreamSynchronize(h->hstream[1]), e0 = cudaStreamSynchronize(h->hstream[0]);
@@ -2354,7 +2561,8 @@ extern "C" int b200gym_reset_host(b200gym_t *h, const uint8_t *mask_host, const 
     // envs that are not reset keep their content
     if (obs_host && obs_host != h->hio.obs && mask_host) memcpy(h->hio.obs, obs_host, n * h->D * sizeof(float));
     if (mask_host) CK(h, cudaMemcpyAsync(h->d_mask, mask_host, n, cudaMemcpyHostToDevice, st));
-    const int rc = launch_reset(h, mask_host ? h->d_mask : nullptr, bounds_host, h->dio.obs, st);
+    int rc = launch_reset(h, mask_host ? h->d_mask : nullptr, bounds_host, h->dio.obs, st);
+    if (!rc && h->sub.on) rc = launch_subenv_reset(h, mask_host ? h->d_mask : nullptr, h->dio.obs, st);
     const cudaError_t e = cudaStreamSynchronize(st);
     if (rc) return 1;
     if (e != cudaSuccess) return fail(h, "b200gym_reset_host: %s", cudaGetErrorString(e));

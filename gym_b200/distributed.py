@@ -142,6 +142,8 @@ class ShardedVectorEnv:
             gather = "nccl"
         if gather not in ("p2p", "nccl", None, False):
             raise ValueError("gather must be 'p2p', 'nccl' or None")
+        if kwargs.get("wrappers"):
+            raise ValueError("ShardedVectorEnv does not take per-env wrappers")
         self.group = group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world_size = dist.get_world_size(group) if dist.is_initialized() else 1

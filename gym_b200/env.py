@@ -17,6 +17,8 @@ from gym_b200.vector_env import B200VectorEnv, _unpickle
 
 class B200Env:
     def __init__(self, env_id, max_episode_steps=None, autoreset=False, device=None, **kwargs):
+        if kwargs.get("wrappers"):
+            raise ValueError("B200Env does not take per-env wrappers (they belong to B200VectorEnv)")
         self._vec = B200VectorEnv(env_id, 1, device=device, max_episode_steps=max_episode_steps,
                                   backend="numpy", copy=True, autoreset=autoreset, **kwargs)
         self.spec = self._vec.spec

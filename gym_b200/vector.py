@@ -10,9 +10,8 @@ def make(id, num_envs=1, asynchronous=True, wrappers=None, disable_env_checker=N
     """``gym.vector.make`` (gym/vector/__init__.py:12-73).
 
     ``asynchronous`` is accepted for signature compatibility: the GPU is the
-    (only) asynchronous worker.  Per-env Python ``wrappers`` cannot be applied to
-    device-resident envs and are rejected.
+    (only) asynchronous worker.  ``wrappers`` are applied to every sub-env on the
+    device (``gym_b200.subenv`` lists the supported ones; anything else raises
+    ``ValueError``).
     """
-    if wrappers:
-        raise ValueError("gym_b200.vector.make does not take per-env Python wrappers")
-    return B200VectorEnv(id, num_envs, **kwargs)
+    return B200VectorEnv(id, num_envs, wrappers=wrappers, **kwargs)

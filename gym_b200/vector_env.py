@@ -25,10 +25,11 @@ Two output backends:
 """
 import ctypes
 import os
+import time
 
 import numpy as np
 
-from gym_b200 import _lib, envs as _envs, error
+from gym_b200 import _lib, envs as _envs, error, subenv as _subenv
 from gym_b200.registration import spec as _spec
 from gym_b200.snapshot import FORMAT_VERSION, EnvSnapshot, check_compatible, env_config, host_indices
 from gym_b200.spaces import batch_space, pcg64_skip, pcg64_state
@@ -60,34 +61,42 @@ def _unpickle(factory, args, kwargs, payload):
 
 
 class FinalInfos(dict):
-    """``infos`` of the torch backend: the done mask is materialised on first access."""
+    """``infos`` of the torch backend: the done masks (``_final_observation`` and, with per-env episode statistics,
+    ``_final_info``) are materialised on first access."""
 
-    def __init__(self, final_obs, terminated, truncated):
+    def __init__(self, final_obs, terminated, truncated, final_info=None):
         super().__init__(final_observation=final_obs)
         self._t, self._u = terminated, truncated
+        self._masks = ("_final_observation",)
+        if final_info is not None:
+            dict.__setitem__(self, "final_info", final_info)
+            self._masks = ("_final_observation", "_final_info")
 
-    def _mask(self):
-        if not dict.__contains__(self, "_final_observation"):
-            dict.__setitem__(self, "_final_observation", self._t | self._u)
-        return dict.__getitem__(self, "_final_observation")
+    def _mask(self, k):
+        if not dict.__contains__(self, k):
+            other = [m for m in self._masks if dict.__contains__(self, m)]
+            dict.__setitem__(self, k, dict.__getitem__(self, other[0]) if other else self._t | self._u)
+        return dict.__getitem__(self, k)
 
     def __getitem__(self, k):
-        if k == "_final_observation":
-            return self._mask()
+        if k in self._masks:
+            return self._mask(k)
         return dict.__getitem__(self, k)
 
     def __contains__(self, k):
-        return k == "_final_observation" or dict.__contains__(self, k)
+        return k in self._masks or dict.__contains__(self, k)
 
     def get(self, k, default=None):
         return self[k] if k in self else default
 
     def keys(self):
-        self._mask()
+        for m in self._masks:
+            self._mask(m)
         return dict.keys(self)
 
     def items(self):
-        self._mask()
+        for m in self._masks:
+            self._mask(m)
         return dict.items(self)
 
 
@@ -106,14 +115,19 @@ class B200VectorEnv:
             plus mask every step instead of the reference's object arrays (use for large N).
         first_index: global index of env 0 when a batch is sharded across GPUs; the
             int-seed fan-out becomes ``seed + first_index + i``.
+        wrappers: per-env wrappers, innermost first, as ``gym.vector.make(..., wrappers=[...])`` applies them to
+            every sub-env (``gym_b200.subenv``); they run on the device after each step.
         **kwargs: env constructor kwargs (``g`` for Pendulum, ``goal_velocity`` for MountainCar*).
     """
 
     is_vector_env = True
 
     def __init__(self, env_id, num_envs, device=None, max_episode_steps=None, backend="torch",
-                 copy=None, first_index=0, autoreset=True, dense_infos=False, **kwargs):
+                 copy=None, first_index=0, autoreset=True, dense_infos=False, wrappers=None, **kwargs):
         self.spec = _spec(env_id)
+        stages = _subenv.parse(wrappers)
+        if stages and not autoreset:
+            raise ValueError("per-env wrappers need autoreset=True (SyncVectorEnv resets through them)")
         if backend not in ("torch", "numpy"):
             raise ValueError("backend must be 'torch' or 'numpy'")
         self.backend = backend
@@ -145,6 +159,7 @@ class B200VectorEnv:
         self.discrete = hasattr(self.single_action_space, "n")
         self.act_dim = 0 if self.discrete else self.single_action_space.shape[0]
         self._sample_cache = None   # (single action space, its sample_actions plan)
+        self._chain = _subenv.Chain(stages, self.kind, self.obs_dim, self.single_action_space) if stages else None
 
         lib = _lib.load()
         torch = _torch()
@@ -191,6 +206,10 @@ class B200VectorEnv:
         self._flip = 0
         self._out = None
         self._hio = None
+        if self._chain is not None:
+            self._chain.allocate(torch, self.num_envs, self.device)
+            _lib.check(lib.b200gym_subenv_set(handle, ctypes.byref(self._chain.struct())), handle)
+            self._t0 = time.perf_counter()
         if backend == "torch":
             self._out = [self._alloc_outputs(), self._alloc_outputs()]
         else:
@@ -207,7 +226,19 @@ class B200VectorEnv:
             terminated=torch.zeros((n,), dtype=torch.bool, device=dev),
             truncated=torch.zeros((n,), dtype=torch.bool, device=dev),
             final_obs=torch.zeros((n, d), dtype=torch.float32, device=dev),
+            **self._chain_outputs(torch, lambda shape, dtype: torch.zeros(shape, dtype=dtype, device=dev)),
         )
+
+    def _chain_outputs(self, torch, alloc):
+        """The outputs a wrapper chain adds: float64 final observations when it normalises them, the episode fields
+        when it records episode statistics."""
+        c, n, d, out = self._chain, self.num_envs, self.obs_dim, {}
+        if c is not None and c.norm_obs:
+            out["final_obs64"] = alloc((n, d), torch.float64)
+        if c is not None and c.episode:
+            out["ep_r"] = alloc((n,), torch.float32)
+            out["ep_l"] = alloc((n,), torch.int32)
+        return out
 
     def _map_host_buffers(self):
         """numpy views of the library's page-locked staging buffers (b200gym_host_buffers)."""
@@ -232,6 +263,15 @@ class B200VectorEnv:
             truncated=view(hio.truncated, ctypes.c_uint8, (n,), np.uint8),
             final_obs=view(hio.final_obs, ctypes.c_float, (n, d), np.float32),
         )
+        if self._chain is not None:
+            f64, ep_r, ep_l = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+            _lib.check(self._lib.b200gym_subenv_host_buffers(self._handle, ctypes.byref(f64), ctypes.byref(ep_r),
+                                                             ctypes.byref(ep_l)), self._handle)
+            if self._chain.norm_obs:
+                self._hio["final_obs64"] = view(f64.value, ctypes.c_double, (n, d), np.float64)
+            if self._chain.episode:
+                self._hio.update(ep_r=view(ep_r.value, ctypes.c_float, (n,), np.float32),
+                                 ep_l=view(ep_l.value, ctypes.c_int32, (n,), np.int32))
 
     def _stream(self):
         return ctypes.c_void_p(_torch().cuda.current_stream(self.device).cuda_stream)
@@ -297,6 +337,9 @@ class B200VectorEnv:
             out = self._out[self._flip]
             _lib.check(self._lib.b200gym_reset(self._handle, None, bptr, ctypes.c_void_p(out["obs"].data_ptr()),
                                                self._stream()), self._handle)
+            if self._chain is not None:
+                _lib.check(self._lib.b200gym_subenv_reset(self._handle, None, ctypes.c_void_p(out["obs"].data_ptr()),
+                                                          self._stream()), self._handle)
             self._pending = out
         else:
             _torch().cuda.current_stream(self.device).synchronize()  # seeding ran on torch's stream
@@ -367,6 +410,14 @@ class B200VectorEnv:
                 self.check_actions()
             self._raise_snapshot_index_error()
             act, code = self._device_actions(actions)
+            c = self._chain
+            if c is not None and c.clip_action:
+                clipped = _torch().empty_like(act)
+                _lib.check(self._lib.b200gym_clip_actions(ctypes.c_void_p(act.data_ptr()),
+                                                          ctypes.c_void_p(clipped.data_ptr()), self.num_envs,
+                                                          self.act_dim, c.act_low.ctypes.data, c.act_high.ctypes.data,
+                                                          self._stream()))
+                act = clipped
             self._flip ^= 1
             out = self._out[self._flip]
             _lib.check(self._lib.b200gym_step(
@@ -374,6 +425,12 @@ class B200VectorEnv:
                 ctypes.c_void_p(out["obs"].data_ptr()), ctypes.c_void_p(out["reward"].data_ptr()),
                 ctypes.c_void_p(out["terminated"].data_ptr()), ctypes.c_void_p(out["truncated"].data_ptr()),
                 ctypes.c_void_p(out["final_obs"].data_ptr()), self._stream()), self._handle)
+            if c is not None:
+                def ptr(k):
+                    return ctypes.c_void_p(out[k].data_ptr()) if k in out else None
+                _lib.check(self._lib.b200gym_subenv_step(
+                    self._handle, ptr("obs"), ptr("reward"), ptr("terminated"), ptr("truncated"), ptr("final_obs"),
+                    ptr("final_obs64"), ptr("ep_r"), ptr("ep_l"), self._stream()), self._handle)
             self._pending = out
             self._last_actions = act  # keep alive until the kernel has consumed it
         else:
@@ -418,7 +475,8 @@ class B200VectorEnv:
             o = self._pending
             if self.copy:
                 o = {k: v.clone() for k, v in o.items()}
-            infos = FinalInfos(o["final_obs"], o["terminated"], o["truncated"])
+            episode = {"episode": {"r": o["ep_r"], "l": o["ep_l"], "t": self._episode_time()}} if "ep_r" in o else None
+            infos = FinalInfos(o.get("final_obs64", o["final_obs"]), o["terminated"], o["truncated"], episode)
             return o["obs"], o["reward"], o["terminated"], o["truncated"], infos
         h = self._hio
         term = h["terminated"].view(np.bool_)   # the kernel writes 0/1 bytes
@@ -429,20 +487,33 @@ class B200VectorEnv:
         infos = {}
         if self.autoreset and self.dense_infos:
             # dense form for large batches: (N, D) array + mask (materialised on first access), no Python loop
-            fo = h["final_obs"].copy() if self.copy else h["final_obs"]
-            infos = FinalInfos(fo, term, trunc)
+            fo = h.get("final_obs64", h["final_obs"])
+            episode = None
+            if "ep_r" in h:
+                ep_r, ep_l = (h["ep_r"].copy(), h["ep_l"].copy()) if self.copy else (h["ep_r"], h["ep_l"])
+                episode = {"episode": {"r": ep_r, "l": ep_l, "t": self._episode_time()}}
+            infos = FinalInfos(fo.copy() if self.copy else fo, term, trunc, episode)
         elif self.autoreset:
             done = term | trunc
             if done.any():
                 # vector_env.py:208-258: object arrays + `_key` masks, only when some env finished
                 fo = np.full(self.num_envs, None, dtype=object)
                 fi = np.full(self.num_envs, None, dtype=object)
+                final = h.get("final_obs64", h["final_obs"])
+                t = self._episode_time() if "ep_r" in h else None
                 for i in np.flatnonzero(done):
-                    fo[i] = h["final_obs"][i].copy()
-                    fi[i] = {}
+                    fo[i] = final[i].copy()
+                    # a per-env RecordEpisodeStatistics puts its episode into the step info, which SyncVectorEnv
+                    # moves to final_info[i] (record_episode_statistics.py:127-139, sync_vector_env.py:152-156)
+                    fi[i] = {} if t is None else {"episode": {"r": h["ep_r"][i].copy(), "l": h["ep_l"][i].copy(),
+                                                              "t": t}}
                 infos = {"final_observation": fo, "_final_observation": done.copy(),
                          "final_info": fi, "_final_info": done.copy()}
         return obs, reward, term, trunc, infos
+
+    def _episode_time(self):
+        """RecordEpisodeStatistics' "t": wall seconds since the wrappers were built."""
+        return round(time.perf_counter() - self._t0, 6)
 
     def step(self, actions):
         """One SyncVectorEnv.step: (obs, rewards, terminateds, truncateds, infos)."""
@@ -599,9 +670,15 @@ class B200VectorEnv:
     def snapshot_row_bytes(self):
         return int(self._lib.b200gym_snapshot_row_bytes(self.kind))
 
+    def _snapshot_config(self):
+        config = env_config(self.max_episode_steps, self.autoreset, self._params, self._cfg_flags)
+        if self._chain is not None:
+            config["wrappers"] = self._chain.describe()
+        return config
+
     def _snapshot_header(self):
         return {"version": FORMAT_VERSION, "kind": self.kind, "row_bytes": self.snapshot_row_bytes,
-                "config": env_config(self.max_episode_steps, self.autoreset, self._params, self._cfg_flags)}
+                "config": self._snapshot_config()}
 
     def _raise_snapshot_index_error(self):
         if self._lib.b200gym_snapshot_index_error(self._handle) == 1:
@@ -677,18 +754,21 @@ class B200VectorEnv:
                     ctypes.c_void_p(rows.data_ptr()), self._stream()), self._handle)
             obs = self._last_obs()
             obs = obs.clone() if idx is None else obs.index_select(0, self._in_range(idx, 0))
+            extras = {}
+            if self._chain is not None:
+                extras["subenv"] = self._chain.snapshot_extra(
+                    lambda t: t.clone() if idx is None else t.index_select(0, self._in_range(idx, 0)))
         if self.backend == "numpy":
             torch.cuda.current_stream(self.device).synchronize()
             self._raise_snapshot_index_error()
-        return EnvSnapshot(self._snapshot_header(), rows, obs)
+        return EnvSnapshot(self._snapshot_header(), rows, obs, extras)
 
     def restore(self, snap, indices=None):
         """Load ``snap`` (row k into env ``indices[k]``; default: all envs, in order) -> ``(obs, {})`` like ``reset``,
         with the observations the snapshot was taken with.  The other envs are left as they are.  A snapshot of
         another kind or construction config raises ``error.Error``."""
         self._check_idle("restore")
-        check_compatible(snap.header, self.kind, self.snapshot_row_bytes,
-                         env_config(self.max_episode_steps, self.autoreset, self._params, self._cfg_flags))
+        check_compatible(snap.header, self.kind, self.snapshot_row_bytes, self._snapshot_config())
         torch = _torch()
         m, n = len(snap), self.num_envs
         idx = self._index_tensor(indices, "restore indices")
@@ -696,12 +776,16 @@ class B200VectorEnv:
             raise error.Error(f"a snapshot of {m} envs restores into {n} envs only with indices=")
         if idx is not None and int(idx.shape[0]) != m:
             raise error.Error(f"{int(idx.shape[0])} indices given for a snapshot of {m} envs")
+        if self._chain is not None and "subenv" not in snap.extras:
+            raise error.Error("the snapshot carries no state for this env's per-env wrappers")
         rows, sobs = snap.rows.to(self.device), snap.obs.to(self.device)
         with torch.cuda.device(self.device):
             if m:
                 _lib.check(self._lib.b200gym_snapshot_load(
                     self._handle, ctypes.c_void_p(rows.data_ptr()), None,
                     None if idx is None else ctypes.c_void_p(idx.data_ptr()), m, self._stream()), self._handle)
+            if self._chain is not None:
+                self._chain.restore_extra(snap.extras["subenv"], lambda t, v: self._scatter_rows(t, idx, v))
             prev = self._last_obs()
             target = self._next_obs()
             if idx is None:
@@ -715,6 +799,17 @@ class B200VectorEnv:
             self._has_reset = self._seeded = True
         return self._obs_result(target), {}
 
+    def _scatter_rows(self, t, idx, values):
+        """t[idx] = values along dim 0 (all rows: idx None); out-of-range entries land in a scratch row."""
+        torch = _torch()
+        values = values.to(self.device)
+        if idx is None:
+            t.copy_(values)
+            return
+        tmp = torch.cat([t, t[:1]])
+        tmp.index_copy_(0, self._in_range(idx, self.num_envs), values)
+        t.copy_(tmp[:self.num_envs])
+
     def clone(self, src):
         """Env i becomes a copy of env ``src[i]`` for every i (duplicates allowed), on the device -> the new
         observations, gathered from the last ones."""
@@ -727,6 +822,8 @@ class B200VectorEnv:
             _lib.check(self._lib.b200gym_clone(self._handle, ctypes.c_void_p(src.data_ptr()), self._stream()),
                        self._handle)
             g = self._in_range(src, torch.arange(self.num_envs, device=self.device))   # a skipped env keeps its obs
+            if self._chain is not None:
+                self._chain.clone_extra(g)   # as deepcopy of the source sub-env would: its statistics come along
             prev = self._last_obs()
             target = self._next_obs()
             if target is prev:
@@ -748,6 +845,8 @@ class B200VectorEnv:
         kw = self._rebuild_env_kwargs()
         kw.update(device=self.device.index, max_episode_steps=self.max_episode_steps or 0, backend=self.backend,
                   copy=self.copy, first_index=self.first_index, autoreset=self.autoreset, dense_infos=self.dense_infos)
+        if self._chain is not None:
+            kw["wrappers"] = list(self._chain.stages)
         return (self.spec, self.num_envs), kw
 
     def _load_snapshot_payload(self, snap, seeded, has_reset):

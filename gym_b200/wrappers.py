@@ -159,10 +159,13 @@ class RecordEpisodeStatistics(VectorWrapper):
     def _fused_target(self):
         """The engine handle whose step kernel can do the bookkeeping itself: the wrapped env must be the
         B200VectorEnv proper (torch backend) -- not a sharded env returning gathered global tensors, not another
-        wrapper that changes rewards."""
+        wrapper that changes rewards, and without a per-env wrapper chain that changes them (gym_b200.subenv: the step
+        kernel would account the raw rewards, before the chain transforms them)."""
         from gym_b200.vector_env import B200VectorEnv
         e = self.env
-        return e if (isinstance(e, B200VectorEnv) and e.backend == "torch" and e.num_envs == self.num_envs) else None
+        if not (isinstance(e, B200VectorEnv) and e.backend == "torch" and e.num_envs == self.num_envs):
+            return None
+        return None if (e._chain is not None and e._chain.changes_rewards) else e
 
     def step(self, actions):
         self._flip ^= 1

@@ -361,6 +361,73 @@ int b200gym_rms_apply_reward(const double *reward_dev, double *out_dev, double *
                              void *stream);
 
 /*
+ * Per-env wrapper chains: what `gym.vector.make(id, n, wrappers=[...])` computes, where every sub-env carries its own
+ * wrapper stack (csrc/subenv.cuh).  One thread per env, no reduction across envs: bit-identical to the reference.
+ * The stages run in list order, innermost first, at most one of each op:
+ *   B200GYM_SUB_EPISODE      RecordEpisodeStatistics: float32 return / int32 length accumulators; a reward that is a
+ *                            Python number or np.float32 at this position is rounded to float32 before the add, an
+ *                            np.float64 is added in float64, then rounded
+ *   B200GYM_SUB_NORM_OBS     NormalizeObservation(epsilon = p0): one RunningMeanStd per env, updated with the terminal
+ *                            AND the reset observation of a finishing env
+ *   B200GYM_SUB_NORM_REWARD  NormalizeReward(gamma = p0, epsilon = p1)
+ *   B200GYM_SUB_CLIP_OBS / B200GYM_SUB_CLIP_REWARD  np.clip(x, p0, p1); the caller rounds ClipObservation's bounds to
+ *                            float32 where the observation is float32 at that position; ClipReward rounds its own
+ *                            where the reward is an np.float32
+ * The reward's Python type is tracked per env-step: raw_reward_type (0 a Python number, 1 np.float64, 2 np.float32),
+ * except that with int_reward_on_fall a terminated step with reward -100 is a Python int (BipedalWalker's fall);
+ * NormalizeReward makes it np.float64, ClipReward np.float64 unless it was np.float32.
+ * The per-env state is caller-owned device memory, SoA rows of n: obs_stats float64 [2*D + 1][n] (mean, var, count;
+ * initialise to 0, 1, 1e-4), rew_stats float64 [4][n] (mean, var, count, discounted return: 0, 1, 1e-4, 0),
+ * ep_return float32 [n], ep_length int32 [n].  clip_action: ClipAction on a Box action space, with the bounds given.
+ *
+ * b200gym_subenv_set      stores the chain in the handle (NULL removes it); needs autoreset
+ * b200gym_subenv_step     ONE launch after b200gym_step over its outputs: rewards and observations in place, the
+ *                         terminal rows of finishing envs read from final_obs (transformed in place, or written to
+ *                         final_obs64 [n][D] as float64 when the chain normalises observations), episode_r / _l of
+ *                         the finishing envs written
+ * b200gym_subenv_reset    after b200gym_reset: the observation stages on the (masked) reset rows, episode
+ *                         accumulators zeroed; the statistics are kept
+ * b200gym_clip_actions    stateless: out[n][act_dim] = np.clip(in, low, high) in float32, NaN propagating
+ * b200gym_subenv_host_buffers  page-locked staging of final_obs64 / episode_r / episode_l for the host-buffer path
+ *                         (and HBM copies of the step's outputs); with a chain set, b200gym_step_host clips the
+ *                         actions, steps into HBM, runs the chain there and copies the results to the staging buffers
+ *                         in bulk, chunk by chunk, inside the same call (it needs this call first), and
+ *                         b200gym_reset_host runs the chain reset
+ */
+#define B200GYM_SUBENV_MAX_STAGES 5
+enum b200gym_subenv_op {
+    B200GYM_SUB_EPISODE = 0,
+    B200GYM_SUB_NORM_OBS = 1,
+    B200GYM_SUB_NORM_REWARD = 2,
+    B200GYM_SUB_CLIP_OBS = 3,
+    B200GYM_SUB_CLIP_REWARD = 4
+};
+typedef struct b200gym_subenv {
+    int32_t num_stages;
+    int32_t op[B200GYM_SUBENV_MAX_STAGES];
+    int32_t raw_reward_type;
+    int32_t int_reward_on_fall;
+    double p0[B200GYM_SUBENV_MAX_STAGES];
+    double p1[B200GYM_SUBENV_MAX_STAGES];
+    double *obs_stats_dev;
+    double *rew_stats_dev;
+    float *ep_return_dev;
+    int32_t *ep_length_dev;
+    int32_t clip_action;
+    float act_low[4];
+    float act_high[4];
+} b200gym_subenv;
+int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain);
+int b200gym_subenv_step(b200gym_t *h, float *obs_dev, double *reward_dev, const uint8_t *terminated_dev,
+                        const uint8_t *truncated_dev, float *final_obs_dev, double *final_obs64_dev,
+                        float *episode_r_dev, int32_t *episode_l_dev, void *stream);
+int b200gym_subenv_reset(b200gym_t *h, const uint8_t *mask_dev, float *obs_dev, void *stream);
+int b200gym_clip_actions(const float *in_dev, float *out_dev, int64_t n, int act_dim, const float *low_host,
+                         const float *high_host, void *stream);
+int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_out, float **episode_r_out,
+                                int32_t **episode_l_out);
+
+/*
  * `envs.action_space.sample()` of a batched action space, bit for bit, as ONE launch on `stream`: MultiDiscrete
  * (gym/spaces/multi_discrete.py:123: `(random(shape) * nvec).astype(int64)`, every element with the same n) and a
  * bounded float32 Box (gym/spaces/box.py:171-222: `uniform(low, high, size).astype(float32)`) -- the batches
