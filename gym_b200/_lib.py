@@ -55,9 +55,14 @@ class HostIO(ctypes.Structure):
     ]
 
 
-SUBENV_MAX_STAGES = 5
+SUBENV_MAX_STAGES = 8
+SUBENV_MAX_STACK = 64
+SUBENV_MAX_ACTION_STAGES = 2
 # enum b200gym_subenv_op
 SUB_EPISODE, SUB_NORM_OBS, SUB_NORM_REWARD, SUB_CLIP_OBS, SUB_CLIP_REWARD = 0, 1, 2, 3, 4
+SUB_FRAME_STACK, SUB_TIME_AWARE, SUB_FLATTEN = 5, 6, 7
+# enum b200gym_subenv_action_op
+ACT_CLIP, ACT_RESCALE = 0, 1
 
 
 class Subenv(ctypes.Structure):
@@ -76,6 +81,15 @@ class Subenv(ctypes.Structure):
         ("clip_action", ctypes.c_int32),
         ("act_low", ctypes.c_float * 4),
         ("act_high", ctypes.c_float * 4),
+        ("history", ctypes.c_void_p),
+        ("head", ctypes.c_void_p),
+        ("t", ctypes.c_void_p),
+        ("num_action_stages", ctypes.c_int32),
+        ("action_op", ctypes.c_int32 * SUBENV_MAX_ACTION_STAGES),
+        ("action_low", (ctypes.c_float * 4) * SUBENV_MAX_ACTION_STAGES),
+        ("action_high", (ctypes.c_float * 4) * SUBENV_MAX_ACTION_STAGES),
+        ("action_min", (ctypes.c_float * 4) * SUBENV_MAX_ACTION_STAGES),
+        ("action_max", (ctypes.c_float * 4) * SUBENV_MAX_ACTION_STAGES),
     ]
 
 
@@ -140,6 +154,10 @@ SIGNATURES = {
     "b200gym_subenv_set": (_i32, [_vp, ctypes.POINTER(Subenv)]),
     "b200gym_subenv_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200gym_subenv_reset": (_i32, [_vp, _vp, _vp, _vp]),
+    "b200gym_subenv_width": (_i32, [_vp]),
+    "b200gym_subenv_step_io": (_i32, [_vp] * 12),
+    "b200gym_subenv_reset_io": (_i32, [_vp] * 5),
+    "b200gym_subenv_actions": (_i32, [_vp] * 4),
     "b200gym_clip_actions": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "b200gym_subenv_host_buffers": (_i32, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp)]),
     "b200gym_box2d_overflows": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),

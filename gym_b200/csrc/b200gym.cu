@@ -117,9 +117,9 @@ struct b200gym {
     unsigned char *snap_scratch = nullptr;        // b200gym_clone: n rows
     // per-env wrapper chain (b200gym_subenv_set); the host-buffer path runs it inside its calls
     struct {
-        bool on = false, clip = false, norm_obs = false, episode = false;
+        bool on = false, out_f64 = false, episode = false;
         SubenvArgs args{};
-        float act_low[4] = {}, act_high[4] = {};
+        SubenvActions act{};                      // act.num == 0: no action stage
         double *final64 = nullptr;                // page-locked, mapped staging of the float64 final observations
         float *ep_r = nullptr;                    // ... of infos["final_info"][i]["episode"]["r"] / ["l"]
         int32_t *ep_l = nullptr;
@@ -132,7 +132,9 @@ struct b200gym {
         float *obs = nullptr, *fin = nullptr;
         double *reward = nullptr;
         uint8_t *term = nullptr, *trunc = nullptr;
+        float *out = nullptr;                     // [n][W] the chain's observations (reshaping chains)
     } sub;
+    int obs_w = 0;                                // width of the host-buffer path's observation staging
     mutable std::string err;
 };
 
@@ -1804,6 +1806,7 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     cudaFree(h->sub.reward);
     cudaFree(h->sub.term);
     cudaFree(h->sub.trunc);
+    cudaFree(h->sub.out);
     if (h->p2p.base) {
         for (int r = 0; r < h->p2p.world; r++)
             if (r != h->p2p.rank && h->p2p.peer[r]) cudaIpcCloseMemHandle(h->p2p.peer[r]);
@@ -2250,55 +2253,54 @@ extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int c
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------
-struct ActBounds {
-    float lo[4], hi[4];
-};
-
-// envs [first, first + count)
+// envs [first, first + count); a reshaping chain reads obs_in and fin and writes obs / fin_out / fin64, the others
+// work in place on obs
 __global__ void __launch_bounds__(kThreads) subenv_step_kernel(const SubenvArgs a, int64_t first, int64_t count,
-                                                               float *obs, double *reward, const uint8_t *term,
-                                                               const uint8_t *trunc, const float *fin, float *fin_out,
-                                                               double *fin64, float *ep_r, int32_t *ep_l) {
+                                                               const float *obs_in, float *obs, double *reward,
+                                                               const uint8_t *term, const uint8_t *trunc,
+                                                               const float *fin, float *fin_out, double *fin64,
+                                                               float *ep_r, int32_t *ep_l) {
     const int64_t k = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-    if (k < count) subenv_step_env(a, first + k, obs, reward, term, trunc, fin, fin_out, fin64, ep_r, ep_l);
+    if (k >= count) return;
+    if (a.reshape) subenv_step_env_io(a, first + k, obs_in, obs, reward, term, trunc, fin, fin_out, fin64, ep_r, ep_l);
+    else subenv_step_env(a, first + k, obs, reward, term, trunc, fin, fin_out, fin64, ep_r, ep_l);
 }
 
-__global__ void __launch_bounds__(kThreads) subenv_reset_kernel(const SubenvArgs a, const uint8_t *mask, float *obs) {
+__global__ void __launch_bounds__(kThreads) subenv_reset_kernel(const SubenvArgs a, const uint8_t *mask,
+                                                                const float *obs_in, float *obs) {
     const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-    if (i < a.n && (!mask || mask[i])) subenv_reset_env(a, i, obs);
+    if (i >= a.n || (mask && !mask[i])) return;
+    if (a.reshape) subenv_reset_env_io(a, i, obs_in, obs);
+    else subenv_reset_env(a, i, obs);
 }
 
-// ClipAction (clip_action.py:31-40): np.clip(action, low, high) in float32, before the env sees the action
-__global__ void __launch_bounds__(kThreads) clip_action_kernel(const float *in, float *out, int64_t total, int A,
-                                                               const ActBounds b) {
+// ClipAction (clip_action.py:31-40) and RescaleAction (rescale_action.py:62-82) in chain order, in float32, before
+// the env sees the action
+__global__ void __launch_bounds__(kThreads) subenv_action_kernel(const float *in, float *out, int64_t total, int A,
+                                                                 const SubenvActions b) {
     const int64_t e = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-    if (e < total) {
-        const int k = (int)(e % A);
-        out[e] = np_clipf(in[e], b.lo[k], b.hi[k]);
-    }
+    if (e < total) out[e] = subenv_action(b, (int)(e % A), in[e]);
 }
 
-static int launch_clip_actions(const b200gym *h, const float *in, float *out, int64_t rows, int A, const float *lo,
-                               const float *hi, cudaStream_t st) {
-    ActBounds b{};
-    for (int k = 0; k < A; k++) { b.lo[k] = lo[k]; b.hi[k] = hi[k]; }
+static int launch_actions(const b200gym *h, const float *in, float *out, int64_t rows, int A, const SubenvActions &b,
+                          cudaStream_t st) {
     const int64_t total = rows * A;
-    clip_action_kernel<<<blocks_for(total), kThreads, 0, st>>>(in, out, total, A, b);
+    subenv_action_kernel<<<blocks_for(total), kThreads, 0, st>>>(in, out, total, A, b);
     CK(h, cudaGetLastError());
     return 0;
 }
 
-static int launch_subenv_step(b200gym *h, int64_t first, int64_t count, float *obs, double *reward,
-                              const uint8_t *term, const uint8_t *trunc, const float *fin, float *fin_out,
-                              double *fin64, float *ep_r, int32_t *ep_l, cudaStream_t st) {
-    subenv_step_kernel<<<blocks_for(count), kThreads, 0, st>>>(h->sub.args, first, count, obs, reward, term, trunc, fin,
-                                                               fin_out, fin64, ep_r, ep_l);
+static int launch_subenv_step(b200gym *h, int64_t first, int64_t count, const float *obs_in, float *obs,
+                              double *reward, const uint8_t *term, const uint8_t *trunc, const float *fin,
+                              float *fin_out, double *fin64, float *ep_r, int32_t *ep_l, cudaStream_t st) {
+    subenv_step_kernel<<<blocks_for(count), kThreads, 0, st>>>(h->sub.args, first, count, obs_in, obs, reward, term,
+                                                               trunc, fin, fin_out, fin64, ep_r, ep_l);
     CK(h, cudaGetLastError());
     return 0;
 }
 
-static int launch_subenv_reset(b200gym *h, const uint8_t *mask, float *obs, cudaStream_t st) {
-    subenv_reset_kernel<<<blocks_for(h->n), kThreads, 0, st>>>(h->sub.args, mask, obs);
+static int launch_subenv_reset(b200gym *h, const uint8_t *mask, const float *obs_in, float *obs, cudaStream_t st) {
+    subenv_reset_kernel<<<blocks_for(h->n), kThreads, 0, st>>>(h->sub.args, mask, obs_in, obs);
     CK(h, cudaGetLastError());
     return 0;
 }
@@ -2306,7 +2308,9 @@ static int launch_subenv_reset(b200gym *h, const uint8_t *mask, float *obs, cuda
 extern "C" int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain) {
     if (!h) return fail(h, "b200gym_subenv_set: null handle");
     if (!chain) {
-        h->sub.on = h->sub.clip = h->sub.norm_obs = h->sub.episode = false;
+        if (h->host_ready && h->obs_w != h->D) return fail(h, "b200gym_subenv_set: the host buffers are sized for the chain");
+        h->sub.on = h->sub.out_f64 = h->sub.episode = false;
+        h->sub.act.num = 0;
         return 0;
     }
     if (!h->cfg.autoreset) return fail(h, "b200gym_subenv_set: a wrapper chain needs autoreset");
@@ -2320,6 +2324,9 @@ extern "C" int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain) {
     a.rew_stats = chain->rew_stats_dev;
     a.ep_return = chain->ep_return_dev;
     a.ep_length = chain->ep_length_dev;
+    a.history = chain->history_dev;
+    a.head = chain->head_dev;
+    a.tstep = chain->t_dev;
     if (chain->raw_reward_type < kRewardPy || chain->raw_reward_type > kRewardF32)
         return fail(h, "b200gym_subenv_set: unknown raw reward type %d", chain->raw_reward_type);
     a.raw_reward_type = chain->raw_reward_type;
@@ -2327,47 +2334,112 @@ extern "C" int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain) {
     unsigned seen = 0;
     for (int s = 0; s < a.num_stages; s++) {
         const int op = chain->op[s];
-        if (op < B200GYM_SUB_EPISODE || op > B200GYM_SUB_CLIP_REWARD || (seen >> op & 1u))
+        if (op < B200GYM_SUB_EPISODE || op > B200GYM_SUB_FLATTEN || (seen >> op & 1u))
             return fail(h, "b200gym_subenv_set: stage %d has an unknown or repeated op %d", s, op);
         seen |= 1u << op;
         if ((op == B200GYM_SUB_NORM_OBS && !a.obs_stats) || (op == B200GYM_SUB_NORM_REWARD && !a.rew_stats) ||
-            (op == B200GYM_SUB_EPISODE && (!a.ep_return || !a.ep_length)))
+            (op == B200GYM_SUB_EPISODE && (!a.ep_return || !a.ep_length)) ||
+            (op == B200GYM_SUB_FRAME_STACK && (!a.history || !a.head)) || (op == B200GYM_SUB_TIME_AWARE && !a.tstep))
             return fail(h, "b200gym_subenv_set: stage %d needs its state buffers", s);
+        if (op == B200GYM_SUB_FRAME_STACK &&
+            !(chain->p0[s] >= 1.0 && chain->p0[s] <= B200GYM_SUBENV_MAX_STACK && chain->p0[s] == (int)chain->p0[s]))
+            return fail(h, "b200gym_subenv_set: FrameStack needs 1 <= num_stack <= %d, got %g", B200GYM_SUBENV_MAX_STACK,
+                        chain->p0[s]);
         a.op[s] = op;
         a.p0[s] = chain->p0[s];
         a.p1[s] = chain->p1[s];
     }
-    if (chain->clip_action && h->A == 0) return fail(h, "b200gym_subenv_set: ClipAction needs a Box action space");
-    h->sub.args = a;
-    h->sub.clip = chain->clip_action != 0;
-    for (int k = 0; k < h->A && k < 4; k++) {
-        h->sub.act_low[k] = chain->act_low[k];
-        h->sub.act_high[k] = chain->act_high[k];
+    if (!(seen >> B200GYM_SUB_TIME_AWARE & 1u)) a.tstep = nullptr;
+    if (!subenv_resolve(a)) return fail(h, "b200gym_subenv_set: the output width %d is too large", a.W);
+    if (h->host_ready && h->obs_w != a.W)
+        return fail(h, "b200gym_subenv_set: a chain that changes the observation's width (%d -> %d) must be set before "
+                    "b200gym_host_buffers", h->D, a.W);
+    SubenvActions act{};
+    if (chain->num_action_stages < 0 || chain->num_action_stages > B200GYM_SUBENV_MAX_ACTION_STAGES)
+        return fail(h, "b200gym_subenv_set: %d action stages", chain->num_action_stages);
+    act.num = chain->num_action_stages;
+    for (int s = 0; s < act.num; s++) {
+        if (chain->action_op[s] != B200GYM_ACT_CLIP && chain->action_op[s] != B200GYM_ACT_RESCALE)
+            return fail(h, "b200gym_subenv_set: unknown action op %d", chain->action_op[s]);
+        act.op[s] = chain->action_op[s];
+        for (int k = 0; k < 4; k++) {
+            act.lo[s][k] = chain->action_low[s][k];
+            act.hi[s][k] = chain->action_high[s][k];
+            act.amin[s][k] = chain->action_min[s][k];
+            act.amax[s][k] = chain->action_max[s][k];
+        }
     }
-    h->sub.norm_obs = (seen >> B200GYM_SUB_NORM_OBS & 1u) != 0;
+    if (act.num == 0 && chain->clip_action) {
+        act.num = 1;
+        act.op[0] = kActClip;
+        for (int k = 0; k < 4; k++) {
+            act.lo[0][k] = chain->act_low[k];
+            act.hi[0][k] = chain->act_high[k];
+        }
+    }
+    if (act.num && h->A == 0) return fail(h, "b200gym_subenv_set: ClipAction / RescaleAction need a Box action space");
+    if (a.reshape && h->sub.final64 && !h->sub.out)
+        CK(h, cudaMalloc((void **)&h->sub.out, (size_t)h->n * a.W * sizeof(float)));
+    h->sub.args = a;
+    h->sub.act = act;
+    h->sub.out_f64 = a.out_f64 != 0;
     h->sub.episode = (seen >> B200GYM_SUB_EPISODE & 1u) != 0;
     h->sub.on = true;
     return 0;
 }
 
+extern "C" int b200gym_subenv_width(const b200gym_t *h) {
+    if (!h) return -1;
+    return h->sub.on ? h->sub.args.W : h->D;
+}
+
+extern "C" int b200gym_subenv_step_io(b200gym_t *h, const float *obs_in_dev, float *obs_dev, double *reward_dev,
+                                      const uint8_t *terminated_dev, const uint8_t *truncated_dev,
+                                      const float *final_obs_in_dev, float *final_obs_dev, double *final_obs64_dev,
+                                      float *episode_r_dev, int32_t *episode_l_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_subenv_step: null handle");
+    if (!h->sub.on) return fail(h, "b200gym_subenv_step: no wrapper chain is set");
+    if (!obs_in_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || !final_obs_in_dev ||
+        !final_obs_dev || (h->sub.out_f64 && !final_obs64_dev) || (h->sub.episode && (!episode_r_dev || !episode_l_dev)))
+        return fail(h, "b200gym_subenv_step: null buffer");
+    if (!h->sub.args.reshape && (obs_in_dev != obs_dev || final_obs_in_dev != final_obs_dev))
+        return fail(h, "b200gym_subenv_step_io: this chain works in place (obs_in == obs, final_obs_in == final_obs)");
+    DeviceGuard guard(h->device);
+    return launch_subenv_step(h, 0, h->n, obs_in_dev, obs_dev, reward_dev, terminated_dev, truncated_dev,
+                              final_obs_in_dev, final_obs_dev, final_obs64_dev, episode_r_dev, episode_l_dev,
+                              (cudaStream_t)stream);
+}
+
 extern "C" int b200gym_subenv_step(b200gym_t *h, float *obs_dev, double *reward_dev, const uint8_t *terminated_dev,
                                    const uint8_t *truncated_dev, float *final_obs_dev, double *final_obs64_dev,
                                    float *episode_r_dev, int32_t *episode_l_dev, void *stream) {
-    if (!h) return fail(h, "b200gym_subenv_step: null handle");
-    if (!h->sub.on) return fail(h, "b200gym_subenv_step: no wrapper chain is set");
-    if (!obs_dev || !reward_dev || !terminated_dev || !truncated_dev || !final_obs_dev ||
-        (h->sub.norm_obs && !final_obs64_dev) || (h->sub.episode && (!episode_r_dev || !episode_l_dev)))
-        return fail(h, "b200gym_subenv_step: null buffer");
+    if (h && h->sub.on && h->sub.args.W != h->D)
+        return fail(h, "b200gym_subenv_step: the chain changes the observation's width; use b200gym_subenv_step_io");
+    return b200gym_subenv_step_io(h, obs_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev,
+                                  final_obs_dev, final_obs64_dev, episode_r_dev, episode_l_dev, stream);
+}
+
+extern "C" int b200gym_subenv_reset_io(b200gym_t *h, const uint8_t *mask_dev, const float *obs_in_dev, float *obs_dev,
+                                       void *stream) {
+    if (!h || !obs_in_dev || !obs_dev) return fail(h, "b200gym_subenv_reset: null argument");
+    if (!h->sub.on) return fail(h, "b200gym_subenv_reset: no wrapper chain is set");
+    if (!h->sub.args.reshape && obs_in_dev != obs_dev)
+        return fail(h, "b200gym_subenv_reset_io: this chain works in place (obs_in == obs)");
     DeviceGuard guard(h->device);
-    return launch_subenv_step(h, 0, h->n, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev,
-                              final_obs_dev, final_obs64_dev, episode_r_dev, episode_l_dev, (cudaStream_t)stream);
+    return launch_subenv_reset(h, mask_dev, obs_in_dev, obs_dev, (cudaStream_t)stream);
 }
 
 extern "C" int b200gym_subenv_reset(b200gym_t *h, const uint8_t *mask_dev, float *obs_dev, void *stream) {
-    if (!h || !obs_dev) return fail(h, "b200gym_subenv_reset: null argument");
-    if (!h->sub.on) return fail(h, "b200gym_subenv_reset: no wrapper chain is set");
+    if (h && h->sub.on && h->sub.args.W != h->D)
+        return fail(h, "b200gym_subenv_reset: the chain changes the observation's width; use b200gym_subenv_reset_io");
+    return b200gym_subenv_reset_io(h, mask_dev, obs_dev, obs_dev, stream);
+}
+
+extern "C" int b200gym_subenv_actions(b200gym_t *h, const float *in_dev, float *out_dev, void *stream) {
+    if (!h || !in_dev || !out_dev) return fail(h, "b200gym_subenv_actions: null argument");
+    if (!h->sub.on || h->sub.act.num == 0) return fail(h, "b200gym_subenv_actions: the chain has no action stage");
     DeviceGuard guard(h->device);
-    return launch_subenv_reset(h, mask_dev, obs_dev, (cudaStream_t)stream);
+    return launch_actions(h, in_dev, out_dev, h->n, h->A, h->sub.act, (cudaStream_t)stream);
 }
 
 extern "C" int b200gym_clip_actions(const float *in_dev, float *out_dev, int64_t n, int act_dim, const float *low_host,
@@ -2377,7 +2449,14 @@ extern "C" int b200gym_clip_actions(const float *in_dev, float *out_dev, int64_t
     const int dev = device_of(out_dev);
     if (dev < 0) return fail(nullptr, "b200gym_clip_actions: out is not a device pointer");
     DeviceGuard guard(dev);
-    return launch_clip_actions(nullptr, in_dev, out_dev, n, act_dim, low_host, high_host, (cudaStream_t)stream);
+    SubenvActions b{};
+    b.num = 1;
+    b.op[0] = kActClip;
+    for (int k = 0; k < act_dim; k++) {
+        b.lo[0][k] = low_host[k];
+        b.hi[0][k] = high_host[k];
+    }
+    return launch_actions(nullptr, in_dev, out_dev, n, act_dim, b, (cudaStream_t)stream);
 }
 
 extern "C" int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_out, float **episode_r_out,
@@ -2386,11 +2465,12 @@ extern "C" int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_ou
         return fail(h, "b200gym_subenv_host_buffers: null argument");
     DeviceGuard guard(h->device);
     const size_t n = (size_t)h->n;
+    const size_t W = (size_t)b200gym_subenv_width(h);
     if (!h->sub.final64) {
-        CK(h, cudaHostAlloc((void **)&h->sub.final64, n * h->D * sizeof(double), cudaHostAllocMapped));
+        CK(h, cudaHostAlloc((void **)&h->sub.final64, n * W * sizeof(double), cudaHostAllocMapped));
         CK(h, cudaHostAlloc((void **)&h->sub.ep_r, n * sizeof(float), cudaHostAllocMapped));
         CK(h, cudaHostAlloc((void **)&h->sub.ep_l, n * sizeof(int32_t), cudaHostAllocMapped));
-        memset(h->sub.final64, 0, n * h->D * sizeof(double));
+        memset(h->sub.final64, 0, n * W * sizeof(double));
         memset(h->sub.ep_r, 0, n * sizeof(float));
         memset(h->sub.ep_l, 0, n * sizeof(int32_t));
         CK(h, cudaHostGetDevicePointer((void **)&h->sub.final64_dev, h->sub.final64, 0));
@@ -2401,6 +2481,7 @@ extern "C" int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_ou
         CK(h, cudaMalloc((void **)&h->sub.reward, n * sizeof(double)));
         CK(h, cudaMalloc((void **)&h->sub.term, n));
         CK(h, cudaMalloc((void **)&h->sub.trunc, n));
+        if (h->sub.on && h->sub.args.reshape) CK(h, cudaMalloc((void **)&h->sub.out, n * W * sizeof(float)));
     }
     *final_obs64_out = h->sub.final64;
     *episode_r_out = h->sub.ep_r;
@@ -2417,7 +2498,8 @@ static int ensure_host_io(b200gym *h) {
     if (h->host_ready) return 0;
     const size_t n = (size_t)h->n;
     const size_t act_bytes = h->A == 0 ? n * sizeof(int64_t) : n * h->A * sizeof(float);
-    const size_t obs_bytes = n * h->D * sizeof(float);
+    h->obs_w = b200gym_subenv_width(h);   // the chain's output width: a chain that changes it is set before this
+    const size_t obs_bytes = n * h->obs_w * sizeof(float);
     const unsigned fl = cudaHostAllocMapped;
     for (int k = 0; k < 2; k++) CK(h, cudaStreamCreateWithFlags(&h->hstream[k], cudaStreamNonBlocking));
     CK(h, cudaHostAlloc(&h->hio.actions, act_bytes, fl));
@@ -2481,9 +2563,9 @@ static int step_host_enqueue(b200gym *h, const void *actions_host, int action_dt
         cudaStream_t st = h->hstream[c & 1];
         CK(h, cudaMemcpyAsync((char *)h->dio.actions + lo * asz, (const char *)actions_host + lo * asz, cnt * asz,
                               cudaMemcpyHostToDevice, st));
-        if (h->sub.on && h->sub.clip) {
+        if (h->sub.on && h->sub.act.num) {
             float *act = (float *)h->dio.actions + lo * h->A;
-            if (launch_clip_actions(h, act, act, cnt, h->A, h->sub.act_low, h->sub.act_high, st)) return 1;
+            if (launch_actions(h, act, act, cnt, h->A, h->sub.act, st)) return 1;
         }
         a.first = lo;
         a.count = cnt;
@@ -2491,11 +2573,12 @@ static int step_host_enqueue(b200gym *h, const void *actions_host, int action_dt
         a.toi_count = h->toi_count ? h->toi_count + (c % kResetSlots) : nullptr;
         if (launch_step(h, a, action_dtype, st)) return 1;
         if (chain) {   // the chain over this chunk in HBM, then its dense outputs to the staging buffers in bulk
-            const size_t D = (size_t)h->D;
-            if (launch_subenv_step(h, lo, cnt, h->sub.obs, h->sub.reward, h->sub.term, h->sub.trunc, h->sub.fin,
+            const size_t W = (size_t)h->obs_w;
+            float *out = h->sub.args.reshape ? h->sub.out : h->sub.obs;
+            if (launch_subenv_step(h, lo, cnt, h->sub.obs, out, h->sub.reward, h->sub.term, h->sub.trunc, h->sub.fin,
                                    h->dio.final_obs, h->sub.final64_dev, h->sub.ep_r_dev, h->sub.ep_l_dev, st))
                 return 1;
-            CK(h, cudaMemcpyAsync(h->hio.obs + lo * D, h->sub.obs + lo * D, cnt * D * sizeof(float),
+            CK(h, cudaMemcpyAsync(h->hio.obs + lo * W, out + lo * W, cnt * W * sizeof(float),
                                   cudaMemcpyDeviceToHost, st));
             CK(h, cudaMemcpyAsync(h->hio.reward + lo, h->sub.reward + lo, cnt * sizeof(double), cudaMemcpyDeviceToHost,
                                   st));
@@ -2538,7 +2621,7 @@ extern "C" int b200gym_step_host(b200gym_t *h, const void *actions_host, int act
     if (invalid_out) *invalid_out = (int64_t)*h->h_invalid;
     *h->invalid_seen = 0ULL;   // reported (and the device counter cleared) with this call
     // results are in the mapped staging buffers; callers that brought their own arrays get a host copy
-    const size_t n = (size_t)h->n, osz = sizeof(float) * h->D;
+    const size_t n = (size_t)h->n, osz = sizeof(float) * h->obs_w;
     if (obs_host && obs_host != h->hio.obs) memcpy(obs_host, h->hio.obs, n * osz);
     if (reward_host && reward_host != h->hio.reward) memcpy(reward_host, h->hio.reward, n * sizeof(double));
     if (terminated_host && terminated_host != h->hio.terminated) memcpy(terminated_host, h->hio.terminated, n);
@@ -2559,14 +2642,20 @@ extern "C" int b200gym_reset_host(b200gym_t *h, const uint8_t *mask_host, const 
     cudaStream_t st = h->hstream[0];
     // the reset kernel writes the rows of the (masked) envs straight into the mapped staging buffer; rows of
     // envs that are not reset keep their content
-    if (obs_host && obs_host != h->hio.obs && mask_host) memcpy(h->hio.obs, obs_host, n * h->D * sizeof(float));
+    // (a reshaping chain: the reset rows land in the HBM copy sub.obs, the chain writes the staging rows)
+    const size_t osz = sizeof(float) * h->obs_w;
+    if (obs_host && obs_host != h->hio.obs && mask_host) memcpy(h->hio.obs, obs_host, n * osz);
+    const bool io = h->sub.on && h->sub.args.reshape;
+    if (io && !h->sub.obs)
+        return fail(h, "b200gym_reset_host: call b200gym_subenv_host_buffers before resetting with a wrapper chain");
     if (mask_host) CK(h, cudaMemcpyAsync(h->d_mask, mask_host, n, cudaMemcpyHostToDevice, st));
-    int rc = launch_reset(h, mask_host ? h->d_mask : nullptr, bounds_host, h->dio.obs, st);
-    if (!rc && h->sub.on) rc = launch_subenv_reset(h, mask_host ? h->d_mask : nullptr, h->dio.obs, st);
+    float *raw = io ? h->sub.obs : h->dio.obs;
+    int rc = launch_reset(h, mask_host ? h->d_mask : nullptr, bounds_host, raw, st);
+    if (!rc && h->sub.on) rc = launch_subenv_reset(h, mask_host ? h->d_mask : nullptr, raw, h->dio.obs, st);
     const cudaError_t e = cudaStreamSynchronize(st);
     if (rc) return 1;
     if (e != cudaSuccess) return fail(h, "b200gym_reset_host: %s", cudaGetErrorString(e));
-    if (obs_host && obs_host != h->hio.obs) memcpy(obs_host, h->hio.obs, n * h->D * sizeof(float));
+    if (obs_host && obs_host != h->hio.obs) memcpy(obs_host, h->hio.obs, n * osz);
     return 0;
 }
 

@@ -12,9 +12,16 @@ from ``gym_b200.wrappers``, whose wrappers wrap the *vector* env and keep statis
   chain in ``infos["final_observation"]``.
 
 The stages below stand for the reference's wrappers; the reference's own ``RecordEpisodeStatistics``, ``ClipAction``,
-``NormalizeObservation`` and ``NormalizeReward`` classes (bare, or ``functools.partial`` with keyword arguments) are
+``NormalizeObservation``, ``NormalizeReward``, ``FrameStack``, ``TimeAwareObservation``, ``FlattenObservation`` and
+``RescaleAction`` classes (bare where they take no argument, or ``functools.partial`` with keyword arguments) are
 accepted too.  ``ClipObservation`` / ``ClipReward`` stand for ``TransformObservation(env, lambda o: np.clip(o, lo, hi))``
 / ``TransformReward(env, lambda r: np.clip(r, lo, hi))``.
+
+``FrameStack``, ``TimeAwareObservation`` and ``FlattenObservation`` change the observation's shape and dtype; the
+chain resolves both at every position, and the env's observation spaces and output shapes follow.  Two deliberate
+departures: a terminal row of a FrameStack chain arrives as an ndarray equal to ``np.asarray`` of the reference's
+``LazyFrames``, and ``RescaleAction`` does not assert that actions lie in ``[min_action, max_action]`` (the engine
+computes what the reference computes under ``python -O``).
 """
 import functools
 import sys
@@ -23,9 +30,10 @@ import numpy as np
 
 from gym_b200 import _lib
 
-SUPPORTED = ("RecordEpisodeStatistics, ClipAction, NormalizeObservation, NormalizeReward, ClipObservation and "
-             "ClipReward (gym_b200.subenv), or the reference's RecordEpisodeStatistics, ClipAction, "
-             "NormalizeObservation and NormalizeReward classes")
+SUPPORTED = ("RecordEpisodeStatistics, ClipAction, NormalizeObservation, NormalizeReward, ClipObservation, "
+             "ClipReward, FrameStack, TimeAwareObservation, FlattenObservation and RescaleAction (gym_b200.subenv), or "
+             "the reference's classes of the same names")
+MAX_STACK = _lib.SUBENV_MAX_STACK   # FrameStack's num_stack
 
 # the Python type of each kind's raw reward (SyncVectorEnv stores them all as float64, but the wrappers see the scalar):
 # a Python number (CartPole, MountainCar*, Acrobot), np.float64 (Pendulum, LunarLander*; LunarLander's +-100 are Python
@@ -103,9 +111,75 @@ class ClipReward(_Clip):
     """``TransformReward(env, lambda r: np.clip(r, low, high))``."""
 
 
-_OWN = (RecordEpisodeStatistics, ClipAction, NormalizeObservation, NormalizeReward, ClipObservation, ClipReward)
+class FrameStack(_Stage):
+    """frame_stack.py:125-190: the last ``num_stack`` observations, in the dtype they have at this position (a reset
+    fills all of them with the reset observation).  ``lz4_compress=True`` is not supported."""
+
+    def __init__(self, num_stack, lz4_compress=False):
+        if lz4_compress:
+            raise ValueError("wrappers: FrameStack(lz4_compress=True) is not supported on the device")
+        if isinstance(num_stack, bool) or not isinstance(num_stack, (int, np.integer)) or not 1 <= num_stack <= MAX_STACK:
+            raise ValueError(f"wrappers: FrameStack needs an int 1 <= num_stack <= {MAX_STACK}, got {num_stack!r}")
+        super().__init__(num_stack=int(num_stack))
+
+
+class TimeAwareObservation(_Stage):
+    """time_aware_observation.py:24-71: appends the steps since the reset (a float64 observation, flattened)."""
+
+    def __init__(self):
+        super().__init__()
+
+
+class FlattenObservation(_Stage):
+    """flatten_observation.py / spaces/utils.py:138-141: flattens, rounding to the space's float32."""
+
+    def __init__(self):
+        super().__init__()
+
+
+def _action_bound(v, what):
+    """A RescaleAction bound that keeps the arithmetic in float32 -> float or float32 array."""
+    if type(v) in (float, int):   # not np.float64, a subclass of float
+        with np.errstate(over="ignore"):
+            return float(np.float32(v))    # np.zeros(A, float32) + v: a Python number is weak (NEP 50)
+    if isinstance(v, np.float32):
+        return float(v)
+    if isinstance(v, np.ndarray) and v.dtype == np.float32 and v.ndim <= 1:
+        return v.copy()
+    raise ValueError(f"wrappers: RescaleAction's {what} must be a Python number, an np.float32 or a float32 array of "
+                     f"at most one dimension (anything else makes the actions float64), got {v!r}")
+
+
+class RescaleAction(_Stage):
+    """rescale_action.py:30-82: maps [min_action, max_action] affinely onto the action space below it, in float32.
+    The range asserts of ``action()`` are not reproduced."""
+
+    def __init__(self, min_action, max_action):
+        lo, hi = _action_bound(min_action, "min_action"), _action_bound(max_action, "max_action")
+        try:
+            ok = bool(np.all(np.less_equal(lo, hi)))
+        except ValueError:
+            ok = False
+        if not ok:
+            raise ValueError(f"wrappers: RescaleAction needs min_action <= max_action, got {min_action!r} and "
+                             f"{max_action!r}")
+        super().__init__(min_action=lo, max_action=hi)
+
+    def describe(self):
+        def d(v):
+            return [float(x) for x in v] if isinstance(v, np.ndarray) else float(v)
+        return ["RescaleAction", {k: d(v) for k, v in sorted(self.kwargs.items())}]
+
+    def __repr__(self):
+        return "RescaleAction(" + ", ".join(f"{k}={v!r}" for k, v in sorted(self.describe()[1].items())) + ")"
+
+
+_OWN = (RecordEpisodeStatistics, ClipAction, NormalizeObservation, NormalizeReward, ClipObservation, ClipReward,
+        FrameStack, TimeAwareObservation, FlattenObservation, RescaleAction)
 _REFERENCE = {"RecordEpisodeStatistics": RecordEpisodeStatistics, "ClipAction": ClipAction,
-              "NormalizeObservation": NormalizeObservation, "NormalizeReward": NormalizeReward}
+              "NormalizeObservation": NormalizeObservation, "NormalizeReward": NormalizeReward,
+              "FrameStack": FrameStack, "TimeAwareObservation": TimeAwareObservation,
+              "FlattenObservation": FlattenObservation, "RescaleAction": RescaleAction}
 
 
 def _reference_stage(cls, kwargs):
@@ -127,6 +201,8 @@ def _stage(w):
     if isinstance(w, type) and issubclass(w, _OWN):
         if issubclass(w, _Clip):
             raise ValueError(f"wrappers: {w.__name__} needs its bounds, e.g. {w.__name__}(-10, 10)")
+        if w in (FrameStack, RescaleAction):
+            raise ValueError(f"wrappers: {w.__name__} needs its arguments")
         return w()
     cls, kwargs = w, {}
     if isinstance(w, functools.partial) and not w.args:
@@ -157,14 +233,21 @@ class Chain:
 
     The host resolves the dtype of the observation a ClipObservation sees: float32 (bounds rounded to float32) before
     NormalizeObservation, float64 after it.  The Python type of the reward can change from one env-step to the next (a
-    BipedalWalker fall), so the kernel tracks it per env from the raw type given here (csrc/subenv.cuh)."""
+    BipedalWalker fall), so the kernel tracks it per env from the raw type given here (csrc/subenv.cuh).
 
-    def __init__(self, stages, kind, obs_dim, action_space):
+    It also resolves the spaces the wrapped env reports (``observation_space``, ``action_space``), the observation's
+    shape and dtype at every position (``obs_shape``, ``final_f64``: the terminal rows are float64), and the action
+    stages in the order they apply (``act_stages``: the outermost wrapper first, each with the bounds of the space
+    below it)."""
+
+    def __init__(self, stages, kind, obs_dim, action_space, observation_space=None):
+        from gym_b200.spaces import Box
         self.stages = list(stages)
         self.kind, self.obs_dim = kind, int(obs_dim)
         self.clip_action = any(isinstance(s, ClipAction) for s in self.stages)
-        if self.clip_action and not hasattr(action_space, "low"):
-            raise ValueError(f"wrappers: ClipAction needs a Box action space, not {action_space!r}")
+        acts = [s for s in self.stages if isinstance(s, (ClipAction, RescaleAction))]
+        if acts and not hasattr(action_space, "low"):
+            raise ValueError(f"wrappers: {type(acts[0]).__name__} needs a Box action space, not {action_space!r}")
         self.norm_obs = any(isinstance(s, NormalizeObservation) for s in self.stages)
         self.norm_reward = any(isinstance(s, NormalizeReward) for s in self.stages)
         self.changes_rewards = any(isinstance(s, (NormalizeReward, ClipReward)) for s in self.stages)
@@ -175,14 +258,42 @@ class Chain:
         if self.clip_action:
             self.act_low = np.ascontiguousarray(action_space.low, dtype=np.float32)
             self.act_high = np.ascontiguousarray(action_space.high, dtype=np.float32)
+        # action stages, innermost first: each sees the space below it; the outermost one applies first
+        self.action_space = action_space
+        self.act_stages = []   # (op, low, high, min, max) float32 (A,) in the order they apply
+        for s in acts:
+            low = np.asarray(self.action_space.low, np.float32)
+            high = np.asarray(self.action_space.high, np.float32)
+            if isinstance(s, ClipAction):
+                self.act_stages.insert(0, (_lib.ACT_CLIP, low, high, low, high))
+                continue
+            shape = self.action_space.shape
+            try:
+                amin = np.zeros(shape, np.float32) + s.kwargs["min_action"]
+                amax = np.zeros(shape, np.float32) + s.kwargs["max_action"]
+            except ValueError:
+                raise ValueError(f"wrappers: {s!r} does not fit the action shape {shape}") from None
+            if amin.shape != shape or amax.shape != shape:
+                raise ValueError(f"wrappers: {s!r} does not fit the action shape {shape}")
+            assert amin.dtype == np.float32 and amax.dtype == np.float32
+            self.act_stages.insert(0, (_lib.ACT_RESCALE, low, high, amin, amax))
+            self.action_space = Box(low=amin, high=amax, shape=shape, dtype=np.float32)
+        # observation stages: the shape, dtype and space at every position
+        space = observation_space if observation_space is not None else Box(-np.inf, np.inf, (self.obs_dim,), np.float32)
+        shape, obs_f32 = (self.obs_dim,), True
+        self.norm_width = self.obs_dim      # width NormalizeObservation sees
+        self.stack = None                   # (num_stack, frame width, frame float64) of FrameStack
+        self.time_aware = False
+        self.reshape = False
         self.ops = []          # (op, p0, p1) of the device stages, in order
-        obs_f32 = True
         for s in self.stages:
             kw = s.kwargs
+            width = int(np.prod(shape))
             if isinstance(s, RecordEpisodeStatistics):
                 self.ops.append((_lib.SUB_EPISODE, 0.0, 0.0))
             elif isinstance(s, NormalizeObservation):
                 self.ops.append((_lib.SUB_NORM_OBS, kw["epsilon"], 0.0))
+                self.norm_width = width
                 obs_f32 = False
             elif isinstance(s, NormalizeReward):
                 self.ops.append((_lib.SUB_NORM_REWARD, kw["gamma"], kw["epsilon"]))
@@ -194,6 +305,29 @@ class Chain:
                 self.ops.append((_lib.SUB_CLIP_OBS, lo, hi))
             elif isinstance(s, ClipReward):
                 self.ops.append((_lib.SUB_CLIP_REWARD, kw["low"], kw["high"]))
+            elif isinstance(s, FrameStack):
+                k = kw["num_stack"]
+                self.ops.append((_lib.SUB_FRAME_STACK, float(k), 0.0))
+                self.stack = (k, width, not obs_f32)
+                space = Box(low=np.repeat(space.low[np.newaxis, ...], k, axis=0),
+                            high=np.repeat(space.high[np.newaxis, ...], k, axis=0), dtype=space.dtype)
+                shape = (k,) + shape
+            elif isinstance(s, TimeAwareObservation):
+                self.ops.append((_lib.SUB_TIME_AWARE, 0.0, 0.0))
+                self.time_aware = True
+                space = Box(np.append(space.low, 0.0), np.append(space.high, np.inf), dtype=np.float32)
+                shape, obs_f32 = (width + 1,), False
+            elif isinstance(s, FlattenObservation):
+                self.ops.append((_lib.SUB_FLATTEN, 0.0, 0.0))
+                space = Box(space.low.flatten(), space.high.flatten(), dtype=space.dtype)
+                assert space.dtype == np.float32
+                shape, obs_f32 = (width,), True
+            if isinstance(s, (FrameStack, TimeAwareObservation, FlattenObservation)):
+                self.reshape = True
+        self.observation_space = space
+        self.obs_shape = tuple(shape)
+        self.out_width = int(np.prod(shape))
+        self.final_f64 = not obs_f32
         self.state = None
 
     def describe(self):
@@ -201,8 +335,9 @@ class Chain:
         return [s.describe() for s in self.stages]
 
     def allocate(self, torch, n, device):
-        """The per-env state at its initial values (RunningMeanStd: mean 0, var 1, count 1e-4; returns 0)."""
-        d = self.obs_dim
+        """The per-env state at its initial values (RunningMeanStd: mean 0, var 1, count 1e-4; returns 0; FrameStack's
+        frames, head and TimeAwareObservation's t 0)."""
+        d = self.norm_width
         obs = torch.zeros((2 * d + 1, n), dtype=torch.float64, device=device)
         obs[d:2 * d] = 1.0
         obs[2 * d] = 1e-4
@@ -212,6 +347,13 @@ class Chain:
         self.state = {"obs_stats": obs, "rew_stats": rew,
                       "ep_return": torch.zeros(n, dtype=torch.float32, device=device),
                       "ep_length": torch.zeros(n, dtype=torch.int32, device=device)}
+        if self.stack is not None:
+            k, wf, f64 = self.stack
+            self.state["history"] = torch.zeros((k * wf, n), dtype=torch.float64 if f64 else torch.float32,
+                                                device=device)
+            self.state["head"] = torch.zeros(n, dtype=torch.int32, device=device)
+        if self.time_aware:
+            self.state["t"] = torch.zeros(n, dtype=torch.int64, device=device)
 
     def struct(self):
         c = _lib.Subenv()
@@ -225,10 +367,16 @@ class Chain:
         c.rew_stats = st["rew_stats"].data_ptr()
         c.ep_return = st["ep_return"].data_ptr()
         c.ep_length = st["ep_length"].data_ptr()
-        c.clip_action = 1 if self.clip_action else 0
-        if self.clip_action:
-            for k in range(len(self.act_low)):
-                c.act_low[k], c.act_high[k] = float(self.act_low[k]), float(self.act_high[k])
+        if "history" in st:
+            c.history, c.head = st["history"].data_ptr(), st["head"].data_ptr()
+        if "t" in st:
+            c.t = st["t"].data_ptr()
+        c.num_action_stages = len(self.act_stages)
+        for s, (op, low, high, amin, amax) in enumerate(self.act_stages):
+            c.action_op[s] = op
+            for k in range(len(low)):
+                c.action_low[s][k], c.action_high[s][k] = float(low[k]), float(high[k])
+                c.action_min[s][k], c.action_max[s][k] = float(amin[k]), float(amax[k])
         return c
 
     # snapshots: every per-env row follows its env; extras hold them env-major ((m, rows) and (m,))

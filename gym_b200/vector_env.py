@@ -10,7 +10,8 @@ device memory and streams.
 Two output backends:
 
 ``backend="torch"`` (default, the fast path)
-    ``step`` returns ``torch.cuda`` tensors: obs float32 (N, D), rewards float64
+    ``step`` returns ``torch.cuda`` tensors: obs float32 (N, D) (with per-env wrappers: (N,) +
+    ``single_observation_space.shape``), rewards float64
     (N,), terminated/truncated bool (N,).  No host synchronisation happens in
     ``step``.  ``infos`` always carries ``final_observation`` (dense (N, D)
     tensor, rows valid where the mask is set) and the ``_final_observation`` mask
@@ -159,7 +160,17 @@ class B200VectorEnv:
         self.discrete = hasattr(self.single_action_space, "n")
         self.act_dim = 0 if self.discrete else self.single_action_space.shape[0]
         self._sample_cache = None   # (single action space, its sample_actions plan)
-        self._chain = _subenv.Chain(stages, self.kind, self.obs_dim, self.single_action_space) if stages else None
+        self._chain = None
+        if stages:
+            # the chain's spaces are the wrapped env's (FrameStack / TimeAwareObservation / FlattenObservation reshape
+            # the observation, RescaleAction rescales the action space)
+            self._chain = _subenv.Chain(stages, self.kind, self.obs_dim, self.single_action_space,
+                                        self.single_observation_space)
+            self.single_observation_space = self._chain.observation_space
+            self.single_action_space = self._chain.action_space
+            self.observation_space = batch_space(self.single_observation_space, n=self.num_envs)
+            self.action_space = batch_space(self.single_action_space, n=self.num_envs)
+        self._obs_shape = tuple(self.single_observation_space.shape)   # of one env's output row
 
         lib = _lib.load()
         torch = _torch()
@@ -220,21 +231,27 @@ class B200VectorEnv:
         """One set of caller-owned output tensors (obs, reward, terminated, truncated, final_obs)."""
         torch = _torch()
         n, d, dev = self.num_envs, self.obs_dim, self.device
-        return dict(
-            obs=torch.zeros((n, d), dtype=torch.float32, device=dev),
+        shape = (n,) + self._obs_shape
+        out = dict(
+            obs=torch.zeros(shape, dtype=torch.float32, device=dev),
             reward=torch.zeros((n,), dtype=torch.float64, device=dev),
             terminated=torch.zeros((n,), dtype=torch.bool, device=dev),
             truncated=torch.zeros((n,), dtype=torch.bool, device=dev),
-            final_obs=torch.zeros((n, d), dtype=torch.float32, device=dev),
+            final_obs=torch.zeros(shape, dtype=torch.float32, device=dev),
             **self._chain_outputs(torch, lambda shape, dtype: torch.zeros(shape, dtype=dtype, device=dev)),
         )
+        if self._chain is not None and self._chain.reshape:
+            # a reshaping chain reads the step's own (n, D) rows and writes the outputs above
+            out["raw_obs"] = torch.zeros((n, d), dtype=torch.float32, device=dev)
+            out["raw_final_obs"] = torch.zeros((n, d), dtype=torch.float32, device=dev)
+        return out
 
     def _chain_outputs(self, torch, alloc):
-        """The outputs a wrapper chain adds: float64 final observations when it normalises them, the episode fields
-        when it records episode statistics."""
-        c, n, d, out = self._chain, self.num_envs, self.obs_dim, {}
-        if c is not None and c.norm_obs:
-            out["final_obs64"] = alloc((n, d), torch.float64)
+        """The outputs a wrapper chain adds: float64 final observations where the chain's terminal rows are float64,
+        the episode fields when it records episode statistics."""
+        c, n, out = self._chain, self.num_envs, {}
+        if c is not None and c.final_f64:
+            out["final_obs64"] = alloc((n,) + self._obs_shape, torch.float64)
         if c is not None and c.episode:
             out["ep_r"] = alloc((n,), torch.float32)
             out["ep_l"] = alloc((n,), torch.int32)
@@ -244,7 +261,7 @@ class B200VectorEnv:
         """numpy views of the library's page-locked staging buffers (b200gym_host_buffers)."""
         hio = _lib.HostIO()
         _lib.check(self._lib.b200gym_host_buffers(self._handle, ctypes.byref(hio)), self._handle)
-        n, d = self.num_envs, self.obs_dim
+        n, shape = self.num_envs, (self.num_envs,) + self._obs_shape
 
         def view(ptr, ctype, shape, dtype):
             count = int(np.prod(shape))
@@ -257,18 +274,18 @@ class B200VectorEnv:
             actions = view(hio.actions, ctypes.c_float, (n, self.act_dim), np.float32)
         self._hio = dict(
             actions=actions,
-            obs=view(hio.obs, ctypes.c_float, (n, d), np.float32),
+            obs=view(hio.obs, ctypes.c_float, shape, np.float32),
             reward=view(hio.reward, ctypes.c_double, (n,), np.float64),
             terminated=view(hio.terminated, ctypes.c_uint8, (n,), np.uint8),
             truncated=view(hio.truncated, ctypes.c_uint8, (n,), np.uint8),
-            final_obs=view(hio.final_obs, ctypes.c_float, (n, d), np.float32),
+            final_obs=view(hio.final_obs, ctypes.c_float, shape, np.float32),
         )
         if self._chain is not None:
             f64, ep_r, ep_l = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
             _lib.check(self._lib.b200gym_subenv_host_buffers(self._handle, ctypes.byref(f64), ctypes.byref(ep_r),
                                                              ctypes.byref(ep_l)), self._handle)
-            if self._chain.norm_obs:
-                self._hio["final_obs64"] = view(f64.value, ctypes.c_double, (n, d), np.float64)
+            if self._chain.final_f64:
+                self._hio["final_obs64"] = view(f64.value, ctypes.c_double, shape, np.float64)
             if self._chain.episode:
                 self._hio.update(ep_r=view(ep_r.value, ctypes.c_float, (n,), np.float32),
                                  ep_l=view(ep_l.value, ctypes.c_int32, (n,), np.int32))
@@ -335,11 +352,13 @@ class B200VectorEnv:
             bptr = ctypes.cast(barr, ctypes.c_void_p)
         if self.backend == "torch":
             out = self._out[self._flip]
-            _lib.check(self._lib.b200gym_reset(self._handle, None, bptr, ctypes.c_void_p(out["obs"].data_ptr()),
+            raw = out.get("raw_obs", out["obs"])
+            _lib.check(self._lib.b200gym_reset(self._handle, None, bptr, ctypes.c_void_p(raw.data_ptr()),
                                                self._stream()), self._handle)
             if self._chain is not None:
-                _lib.check(self._lib.b200gym_subenv_reset(self._handle, None, ctypes.c_void_p(out["obs"].data_ptr()),
-                                                          self._stream()), self._handle)
+                _lib.check(self._lib.b200gym_subenv_reset_io(self._handle, None, ctypes.c_void_p(raw.data_ptr()),
+                                                             ctypes.c_void_p(out["obs"].data_ptr()), self._stream()),
+                           self._handle)
             self._pending = out
         else:
             _torch().cuda.current_stream(self.device).synchronize()  # seeding ran on torch's stream
@@ -411,26 +430,26 @@ class B200VectorEnv:
             self._raise_snapshot_index_error()
             act, code = self._device_actions(actions)
             c = self._chain
-            if c is not None and c.clip_action:
-                clipped = _torch().empty_like(act)
-                _lib.check(self._lib.b200gym_clip_actions(ctypes.c_void_p(act.data_ptr()),
-                                                          ctypes.c_void_p(clipped.data_ptr()), self.num_envs,
-                                                          self.act_dim, c.act_low.ctypes.data, c.act_high.ctypes.data,
-                                                          self._stream()))
-                act = clipped
+            if c is not None and c.act_stages:   # ClipAction / RescaleAction, outermost first
+                staged = _torch().empty_like(act)
+                _lib.check(self._lib.b200gym_subenv_actions(self._handle, ctypes.c_void_p(act.data_ptr()),
+                                                            ctypes.c_void_p(staged.data_ptr()), self._stream()),
+                           self._handle)
+                act = staged
             self._flip ^= 1
             out = self._out[self._flip]
+
+            def ptr(k):
+                return ctypes.c_void_p(out[k].data_ptr()) if k in out else None
+            raw_obs = ptr("raw_obs") or ptr("obs")
+            raw_fin = ptr("raw_final_obs") or ptr("final_obs")
             _lib.check(self._lib.b200gym_step(
-                self._handle, ctypes.c_void_p(act.data_ptr()), code,
-                ctypes.c_void_p(out["obs"].data_ptr()), ctypes.c_void_p(out["reward"].data_ptr()),
-                ctypes.c_void_p(out["terminated"].data_ptr()), ctypes.c_void_p(out["truncated"].data_ptr()),
-                ctypes.c_void_p(out["final_obs"].data_ptr()), self._stream()), self._handle)
+                self._handle, ctypes.c_void_p(act.data_ptr()), code, raw_obs, ptr("reward"), ptr("terminated"),
+                ptr("truncated"), raw_fin, self._stream()), self._handle)
             if c is not None:
-                def ptr(k):
-                    return ctypes.c_void_p(out[k].data_ptr()) if k in out else None
-                _lib.check(self._lib.b200gym_subenv_step(
-                    self._handle, ptr("obs"), ptr("reward"), ptr("terminated"), ptr("truncated"), ptr("final_obs"),
-                    ptr("final_obs64"), ptr("ep_r"), ptr("ep_l"), self._stream()), self._handle)
+                _lib.check(self._lib.b200gym_subenv_step_io(
+                    self._handle, raw_obs, ptr("obs"), ptr("reward"), ptr("terminated"), ptr("truncated"), raw_fin,
+                    ptr("final_obs"), ptr("final_obs64"), ptr("ep_r"), ptr("ep_l"), self._stream()), self._handle)
             self._pending = out
             self._last_actions = act  # keep alive until the kernel has consumed it
         else:
@@ -474,7 +493,7 @@ class B200VectorEnv:
         if self.backend == "torch":
             o = self._pending
             if self.copy:
-                o = {k: v.clone() for k, v in o.items()}
+                o = {k: v.clone() for k, v in o.items() if not k.startswith("raw_")}
             episode = {"episode": {"r": o["ep_r"], "l": o["ep_l"], "t": self._episode_time()}} if "ep_r" in o else None
             infos = FinalInfos(o.get("final_obs64", o["final_obs"]), o["terminated"], o["truncated"], episode)
             return o["obs"], o["reward"], o["terminated"], o["truncated"], infos
@@ -791,7 +810,7 @@ class B200VectorEnv:
             if idx is None:
                 target.copy_(sobs)
             else:   # row n of the scratch takes the observations of skipped (out-of-range) entries
-                tmp = torch.empty((n + 1, self.obs_dim), dtype=torch.float32, device=self.device)
+                tmp = torch.empty((n + 1,) + self._obs_shape, dtype=torch.float32, device=self.device)
                 tmp[:n].copy_(prev)
                 tmp.index_copy_(0, self._in_range(idx, n), sobs)
                 target.copy_(tmp[:n])

@@ -297,7 +297,7 @@ class NormalizeObservation(VectorWrapper):
         self._torch = torch
         self.num_envs, self.is_vector_env = env.num_envs, True
         self.epsilon = float(epsilon)
-        d = env.single_observation_space.shape[0]
+        d = int(np.prod(env.single_observation_space.shape))   # statistics per element of the flattened row
         self.obs_rms = _RunningMeanStd(torch, d, env.unwrapped.device)
         self._out = [None, None]
         self._flip = 0
@@ -311,7 +311,8 @@ class NormalizeObservation(VectorWrapper):
         out = self._out[self._flip]
         env = self.env.unwrapped
         r, lib = self.obs_rms, env._lib
-        n, d = obs.shape
+        n = obs.shape[0]
+        d = obs.numel() // n
         st, sc = r.stats[r.cur], r.scratch[r.cur]
         with torch.cuda.device(obs.device):
             if update:

@@ -380,28 +380,56 @@ int b200gym_rms_apply_reward(const double *reward_dev, double *out_dev, double *
  * initialise to 0, 1, 1e-4), rew_stats float64 [4][n] (mean, var, count, discounted return: 0, 1, 1e-4, 0),
  * ep_return float32 [n], ep_length int32 [n].  clip_action: ClipAction on a Box action space, with the bounds given.
  *
- * b200gym_subenv_set      stores the chain in the handle (NULL removes it); needs autoreset
+ *   B200GYM_SUB_FRAME_STACK  FrameStack(num_stack = p0, 1..B200GYM_SUBENV_MAX_STACK): history of the frames, appended
+ *                            to on every step, filled num_stack times by every reset
+ *   B200GYM_SUB_TIME_AWARE   TimeAwareObservation: appends t (steps since the reset; the terminal row ends in the
+ *                            episode length), which makes the observation float64
+ *   B200GYM_SUB_FLATTEN      FlattenObservation: rounds the observation to float32 (the spaces are float32)
+ * The last three change the observation's width and dtype: the chain takes the step's D float32 values and returns
+ * W values (b200gym_subenv_width), float64 where the reference's are (the terminal rows then go to final_obs64).
+ * Their state: history_dev, SoA [num_stack * wf][n] (wf = the width at FrameStack's input) of float32, or of float64
+ * where the observation is float64 there; head_dev int32 [n] (the ring slot of the newest frame); t_dev int64 [n].
+ * NormalizeObservation's obs_stats is [2 * w + 1][n] with w the width at its position.
+ * Action stages (action_op, in the order they apply: the outermost wrapper first; num_action_stages 0 falls back
+ * to clip_action): B200GYM_ACT_CLIP np.clip(a, low, high); B200GYM_ACT_RESCALE low + (high - low) * ((a - min) /
+ * (max - min)), then np.clip(a, low, high), all in float32; low / high are the bounds of the space below the stage.
+ * The engine computes what the reference computes under `python -O`: RescaleAction's range asserts are not made.
+ *
+ * b200gym_subenv_set      stores the chain in the handle (NULL removes it); needs autoreset.  A chain whose
+ *                         output width differs from D must be set before b200gym_host_buffers
+ * b200gym_subenv_width    W of the chain set (D without one)
  * b200gym_subenv_step     ONE launch after b200gym_step over its outputs: rewards and observations in place, the
  *                         terminal rows of finishing envs read from final_obs (transformed in place, or written to
  *                         final_obs64 [n][D] as float64 when the chain normalises observations), episode_r / _l of
- *                         the finishing envs written
+ *                         the finishing envs written; fails for a chain with W != D
+ * b200gym_subenv_step_io  the same with the step's observations read from obs_in_dev [n][D] and written to obs_dev
+ *                         [n][W]; the terminal rows are read from final_obs_in_dev [n][D] and written to final_obs_dev
+ *                         [n][W] (float32) or final_obs64_dev [n][W] (float64)
  * b200gym_subenv_reset    after b200gym_reset: the observation stages on the (masked) reset rows, episode
- *                         accumulators zeroed; the statistics are kept
+ *                         accumulators zeroed; the statistics are kept (b200gym_subenv_reset_io: from obs_in_dev
+ *                         [n][D] to obs_dev [n][W])
+ * b200gym_subenv_actions  the chain's action stages over out[n][act_dim] = f(in) (in == out allowed)
  * b200gym_clip_actions    stateless: out[n][act_dim] = np.clip(in, low, high) in float32, NaN propagating
- * b200gym_subenv_host_buffers  page-locked staging of final_obs64 / episode_r / episode_l for the host-buffer path
- *                         (and HBM copies of the step's outputs); with a chain set, b200gym_step_host clips the
- *                         actions, steps into HBM, runs the chain there and copies the results to the staging buffers
- *                         in bulk, chunk by chunk, inside the same call (it needs this call first), and
- *                         b200gym_reset_host runs the chain reset
+ * b200gym_subenv_host_buffers  page-locked staging of final_obs64 [n][W] / episode_r / episode_l for the host-buffer
+ *                         path (and HBM copies of the step's outputs); with a chain set, b200gym_step_host applies
+ *                         the action stages, steps into HBM, runs the chain there and copies the results to the
+ *                         staging buffers ([n][W]) in bulk, chunk by chunk, inside the same call (it needs this call
+ *                         first), and b200gym_reset_host runs the chain reset
  */
-#define B200GYM_SUBENV_MAX_STAGES 5
+#define B200GYM_SUBENV_MAX_STAGES 8
+#define B200GYM_SUBENV_MAX_STACK 64
+#define B200GYM_SUBENV_MAX_ACTION_STAGES 2
 enum b200gym_subenv_op {
     B200GYM_SUB_EPISODE = 0,
     B200GYM_SUB_NORM_OBS = 1,
     B200GYM_SUB_NORM_REWARD = 2,
     B200GYM_SUB_CLIP_OBS = 3,
-    B200GYM_SUB_CLIP_REWARD = 4
+    B200GYM_SUB_CLIP_REWARD = 4,
+    B200GYM_SUB_FRAME_STACK = 5,
+    B200GYM_SUB_TIME_AWARE = 6,
+    B200GYM_SUB_FLATTEN = 7
 };
+enum b200gym_subenv_action_op { B200GYM_ACT_CLIP = 0, B200GYM_ACT_RESCALE = 1 };
 typedef struct b200gym_subenv {
     int32_t num_stages;
     int32_t op[B200GYM_SUBENV_MAX_STAGES];
@@ -416,12 +444,29 @@ typedef struct b200gym_subenv {
     int32_t clip_action;
     float act_low[4];
     float act_high[4];
+    void *history_dev;
+    int32_t *head_dev;
+    int64_t *t_dev;
+    int32_t num_action_stages;
+    int32_t action_op[B200GYM_SUBENV_MAX_ACTION_STAGES];
+    float action_low[B200GYM_SUBENV_MAX_ACTION_STAGES][4];
+    float action_high[B200GYM_SUBENV_MAX_ACTION_STAGES][4];
+    float action_min[B200GYM_SUBENV_MAX_ACTION_STAGES][4];
+    float action_max[B200GYM_SUBENV_MAX_ACTION_STAGES][4];
 } b200gym_subenv;
 int b200gym_subenv_set(b200gym_t *h, const b200gym_subenv *chain);
+int b200gym_subenv_width(const b200gym_t *h);
 int b200gym_subenv_step(b200gym_t *h, float *obs_dev, double *reward_dev, const uint8_t *terminated_dev,
                         const uint8_t *truncated_dev, float *final_obs_dev, double *final_obs64_dev,
                         float *episode_r_dev, int32_t *episode_l_dev, void *stream);
+int b200gym_subenv_step_io(b200gym_t *h, const float *obs_in_dev, float *obs_dev, double *reward_dev,
+                           const uint8_t *terminated_dev, const uint8_t *truncated_dev, const float *final_obs_in_dev,
+                           float *final_obs_dev, double *final_obs64_dev, float *episode_r_dev,
+                           int32_t *episode_l_dev, void *stream);
 int b200gym_subenv_reset(b200gym_t *h, const uint8_t *mask_dev, float *obs_dev, void *stream);
+int b200gym_subenv_reset_io(b200gym_t *h, const uint8_t *mask_dev, const float *obs_in_dev, float *obs_dev,
+                            void *stream);
+int b200gym_subenv_actions(b200gym_t *h, const float *in_dev, float *out_dev, void *stream);
 int b200gym_clip_actions(const float *in_dev, float *out_dev, int64_t n, int act_dim, const float *low_host,
                          const float *high_host, void *stream);
 int b200gym_subenv_host_buffers(b200gym_t *h, double **final_obs64_out, float **episode_r_out,
