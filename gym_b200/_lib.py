@@ -151,6 +151,7 @@ SIGNATURES = {
     "b200gym_rms_apply_reward": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
                                         _vp]),
     "b200gym_sample_space": (_i32, [_vp, _i64, _i32, _i64, _vp, _vp, _vp, _vp]),
+    "b200gym_sample_space_stream": (_i32, [_vp, _vp, _i64, _i32, _i64, _vp, _vp, _vp, _vp]),
     "b200gym_subenv_set": (_i32, [_vp, ctypes.POINTER(Subenv)]),
     "b200gym_subenv_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200gym_subenv_reset": (_i32, [_vp, _vp, _vp, _vp]),

@@ -1418,6 +1418,55 @@ static inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads -
 // (P: 48) cost more than moving the memory traffic off the compute warps saves
 static bool bulk_by_default(int kind) { return kind == B200GYM_CARTPOLE; }
 
+template <typename ActT>
+static constexpr int act_width_slot() { return sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2; }
+
+// The resident kernels' CTAs per SM (and kernel B's shared-memory attributes) for one action type, set up when the
+// handle is created rather than on its first step: that step may be the one a CUDA graph captures, and the capture
+// must hold nothing but launches
+template <int KIND, typename ActT>
+static int prepare_step_typed(b200gym *h) {
+    const int w = act_width_slot<ActT>();
+    if (h->kernel_choice == 3 || (h->kernel_choice == -1 && bulk_by_default(KIND))) {
+        const int smem = kBulkStages * BulkLayout<KIND, ActT>::kBytes;
+        int &occ = h->occ_bulk[KIND][w];
+        CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                   (int)cudaSharedmemCarveoutMaxShared));
+        CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent_bulk<KIND, ActT>, kThreads + 32, smem));
+        if (occ < 1) occ = 1;
+    }
+    if (h->kernel_choice != 0) {
+        for (int lean = 0; lean < 2; lean++) {
+            int &occ = h->occ[KIND][w][lean];
+            const auto kernel = lean ? step_kernel_persistent<KIND, ActT, true> : step_kernel_persistent<KIND, ActT, false>;
+            CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 0));
+            if (occ < 1) occ = 1;
+        }
+    }
+    return 0;
+}
+
+template <int KIND>
+static int prepare_step_kind(b200gym *h) {
+    if constexpr (Env<KIND>::A == 0)
+        return prepare_step_typed<KIND, long long>(h) || prepare_step_typed<KIND, int>(h) ||
+               prepare_step_typed<KIND, unsigned char>(h);
+    else
+        return prepare_step_typed<KIND, float>(h);
+}
+
+static int prepare_step(b200gym *h) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return prepare_step_kind<B200GYM_CARTPOLE>(h);
+    case B200GYM_MOUNTAINCAR: return prepare_step_kind<B200GYM_MOUNTAINCAR>(h);
+    case B200GYM_MOUNTAINCAR_CONT: return prepare_step_kind<B200GYM_MOUNTAINCAR_CONT>(h);
+    case B200GYM_PENDULUM: return prepare_step_kind<B200GYM_PENDULUM>(h);
+    case B200GYM_ACROBOT: return prepare_step_kind<B200GYM_ACROBOT>(h);
+    }
+    return 0;   // the Box2D tasks' kernels need no set-up
+}
+
 template <int KIND, typename ActT>
 static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
     int64_t done = 0;
@@ -1453,14 +1502,7 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
                        al(reinterpret_cast<const ActT *>(a.actions) + a.first * L::kActPerEnv);
         if (aligned) {
             const int smem = kBulkStages * L::kBytes;
-            int &occ = h->occ_bulk[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2];
-            if (occ == 0) {
-                CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-                CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                           (int)cudaSharedmemCarveoutMaxShared));
-                CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent_bulk<KIND, ActT>, kThreads + 32, smem));
-                if (occ < 1) occ = 1;
-            }
+            const int occ = h->occ_bulk[KIND][act_width_slot<ActT>()];   // prepare_step_typed, at create
             int64_t grid = (int64_t)h->sm_count * occ;
             if (grid > tiles) grid = tiles;
             step_kernel_persistent_bulk<KIND, ActT><<<(unsigned)grid, kThreads + 32, smem, st>>>(a, (int)tiles);
@@ -1477,11 +1519,7 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
             // the lean instantiation: no fused episode statistics, every index fits 32 bits
             const bool lean = h->kernel_choice != 1 && !a.ep_acc && h->n < (int64_t)1 << 30;
             const auto kernel = lean ? step_kernel_persistent<KIND, ActT, true> : step_kernel_persistent<KIND, ActT, false>;
-            int &occ = h->occ[KIND][sizeof(ActT) == 8 ? 0 : sizeof(ActT) == 4 ? 1 : 2][lean ? 1 : 0];
-            if (occ == 0) {
-                CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 0));
-                if (occ < 1) occ = 1;
-            }
+            const int occ = h->occ[KIND][act_width_slot<ActT>()][lean ? 1 : 0];   // prepare_step_typed, at create
             const int64_t all_tiles = (a.count + kThreads - 1) / kThreads;
             int64_t grid = (int64_t)h->sm_count * occ;
             if (grid > all_tiles) grid = all_tiles;
@@ -1642,6 +1680,28 @@ __global__ void __launch_bounds__(kSampleThreads) space_sample_kernel(const Samp
                      table);
 }
 
+// ... the stream variant (space_sample.cuh): the generator comes from the record (or the override) and the last CTA
+// to take a ticket writes the advanced state back, so one launch both reads and moves the stream
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads) space_sample_stream_kernel(const SampleArgs a, const SampleStream s,
+                                                                             T *__restrict__ out) {
+    __shared__ LcgJumpTable table;
+    __shared__ Pcg64 start;
+    const uint4 *src = reinterpret_cast<const uint4 *>(&kLcgJump);
+    uint4 *dst = reinterpret_cast<uint4 *>(&table);
+    for (int i = threadIdx.x; i < a.jump_digits * 32; i += kSampleThreads) dst[i] = src[i];
+    if (threadIdx.x == 0) start = sample_stream_start(s);   // overlaps the table's loads
+    __syncthreads();
+    const Pcg64 g = start;
+    // The ticket: this CTA's read of the record has returned (its value is in shared memory), so the last CTA to take
+    // one writes after every read.  Its result is only needed after the draws, which hide the round trip.
+    unsigned long long ticket = 0;
+    if (threadIdx.x == 0) ticket = atomicAdd(reinterpret_cast<unsigned long long *>(s.record + 4), 1ULL);
+    sample_thread<T>(a, g, a.hop_geo * g.inc, out, (int64_t)blockIdx.x * kSampleThreads + threadIdx.x,
+                     (int64_t)gridDim.x * kSampleThreads, table);
+    if (threadIdx.x == 0 && ticket == gridDim.x - 1ULL) sample_stream_finish(s, g);
+}
+
 // ---------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------
@@ -1760,6 +1820,11 @@ extern "C" int b200gym_create(const b200gym_config *cfg, int64_t num_envs, int d
     for (cudaError_t mi : ms) ms_ok = ms_ok && mi == cudaSuccess;
     if (!ms_ok || cudaDeviceSynchronize() != cudaSuccess) {
         fail(nullptr, "b200gym_create: device initialisation failed: %s", cudaGetErrorString(cudaGetLastError()));
+        b200gym_destroy(h);
+        return 1;
+    }
+    if (prepare_step(h)) {
+        fail(nullptr, "b200gym_create: step kernel set-up failed: %s", b200gym_last_error(h));
         b200gym_destroy(h);
         return 1;
     }
@@ -2213,18 +2278,15 @@ extern "C" int b200gym_rms_apply_reward(const double *reward_dev, double *out_de
     return 0;
 }
 
-extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int cols, int64_t n_choices,
-                                    const double *low_host, const double *high_host, void *out_dev, void *stream) {
-    if (!pcg64 || !out_dev || rows <= 0 || cols <= 0 || cols > kSampleMaxCols || n_choices < 0 ||
-        (n_choices > 0 && cols != 1) || (n_choices == 0 && (!low_host || !high_host)) ||
-        rows > INT64_MAX / kSampleMaxCols)
-        return fail(nullptr, "b200gym_sample_space: bad argument (MultiDiscrete needs cols = 1, a Box 1 <= cols <= %d "
-                             "and its bounds)", kSampleMaxCols);
-    if ((uintptr_t)out_dev % 16)
-        return fail(nullptr, "b200gym_sample_space: out is not 16-byte aligned");
-    SampleArgs a{};
-    a.start.state = make_u128(pcg64[0], pcg64[1]);
-    a.start.inc = make_u128(pcg64[2], pcg64[3]);
+// the arguments both sampling entry points share; `what` names the caller in the error
+static int sample_prepare(const char *what, int64_t rows, int cols, int64_t n_choices, const double *low_host,
+                          const double *high_host, void *out_dev, SampleArgs &a, int &dev) {
+    if (!out_dev || rows <= 0 || cols <= 0 || cols > kSampleMaxCols || n_choices < 0 || (n_choices > 0 && cols != 1) ||
+        (n_choices == 0 && (!low_host || !high_host)) || rows > INT64_MAX / kSampleMaxCols)
+        return fail(nullptr, "%s: bad argument (MultiDiscrete needs cols = 1, a Box 1 <= cols <= %d and its bounds)", what,
+                    kSampleMaxCols);
+    if ((uintptr_t)out_dev % 16) return fail(nullptr, "%s: out is not 16-byte aligned", what);
+    a = SampleArgs{};
     a.total = rows * cols;
     a.cols = cols;
     a.n_choices = (double)n_choices;
@@ -2233,12 +2295,22 @@ extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int c
             a.low[c] = low_host[c];
             a.high[c] = high_host[c];
             if (!std::isfinite(a.low[c]) || !std::isfinite(a.high[c]) || !std::isfinite(a.high[c] - a.low[c]))
-                return fail(nullptr, "b200gym_sample_space: column %d is not a bounded Box (low %g, high %g)", c,
-                            a.low[c], a.high[c]);
+                return fail(nullptr, "%s: column %d is not a bounded Box (low %g, high %g)", what, c, a.low[c], a.high[c]);
         }
     }
-    const int dev = device_of(out_dev);
-    if (dev < 0) return fail(nullptr, "b200gym_sample_space: out is not a device pointer");
+    dev = device_of(out_dev);
+    if (dev < 0) return fail(nullptr, "%s: out is not a device pointer", what);
+    return 0;
+}
+
+extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int cols, int64_t n_choices,
+                                    const double *low_host, const double *high_host, void *out_dev, void *stream) {
+    SampleArgs a;
+    int dev;
+    if (!pcg64) return fail(nullptr, "b200gym_sample_space: bad argument (null generator)");
+    if (sample_prepare("b200gym_sample_space", rows, cols, n_choices, low_host, high_host, out_dev, a, dev)) return 1;
+    a.start.state = make_u128(pcg64[0], pcg64[1]);
+    a.start.inc = make_u128(pcg64[2], pcg64[3]);
     DeviceGuard guard(dev);
     const int vec = n_choices > 0 ? 2 : 4;
     const int64_t blocks = sample_blocks(a.total, vec);
@@ -2248,6 +2320,37 @@ extern "C" int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int c
         space_sample_kernel<long long><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, (long long *)out_dev);
     else
         space_sample_kernel<float><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, (float *)out_dev);
+    CK(nullptr, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_sample_space_stream(uint64_t *record_dev, const uint64_t override_pcg64[4], int64_t rows, int cols,
+                                           int64_t n_choices, const double *low_host, const double *high_host,
+                                           void *out_dev, void *stream) {
+    SampleArgs a;
+    int dev;
+    if (!record_dev || (uintptr_t)record_dev % 16)
+        return fail(nullptr, "b200gym_sample_space_stream: the record must be a 16-byte aligned device buffer");
+    if (sample_prepare("b200gym_sample_space_stream", rows, cols, n_choices, low_host, high_host, out_dev, a, dev))
+        return 1;
+    if (device_of(record_dev) != dev)
+        return fail(nullptr, "b200gym_sample_space_stream: the record is not on the device of out");
+    SampleStream s{};
+    s.record = record_dev;
+    if (override_pcg64) {
+        s.use_override = 1;
+        for (int k = 0; k < 4; k++) s.override_words[k] = override_pcg64[k];
+    }
+    s.advance = lcg_jump_map((u128)a.total);
+    DeviceGuard guard(dev);
+    const int vec = n_choices > 0 ? 2 : 4;
+    const int64_t blocks = sample_blocks(a.total, vec);
+    sample_setup(a, blocks * kSampleThreads, vec);   // a.start is unused: the hop_plus it derives is recomputed on the device
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_choices > 0)
+        space_sample_stream_kernel<long long><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, s, (long long *)out_dev);
+    else
+        space_sample_stream_kernel<float><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, s, (float *)out_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
 }

@@ -11,6 +11,11 @@
 //     on the host.  sample_blocks sizes the grid for ~kSampleRounds rounds per thread, so the jumps cost well under
 //     one multiply per element next to the one of each draw.  The kernel first stages the rows of the table its
 //     offsets use in shared memory: the digits then cost one round trip to memory instead of one each.
+//   stream variant (space_sample_stream_kernel): the generator lives in a device record instead of the arguments, so a
+//     launch captured in a CUDA graph continues the stream at every replay.  Every CTA reads the record (or the
+//     caller's override), takes a ticket, and the last CTA to arrive writes back the state `total` draws later.  The
+//     arguments hold only maps that do not depend on inc (the hop's geo factor, the advance): a reseed that changes inc
+//     between captures cannot leave a graph with a stale hop.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -27,6 +32,7 @@ constexpr int kSampleThreads = 256;
 struct SampleArgs {
     Pcg64 start;                 // the generator before draw 0
     u128 hop_mult, hop_plus;     // state -> hop_mult * state + hop_plus: from after a thread's vector to its next one
+    u128 hop_geo;                // hop_plus = hop_geo * inc
     int64_t total;               // rows * cols
     int jump_digits;             // hex digits of the largest first-vector offset: the rows of kLcgJump in use
     int cols;
@@ -47,6 +53,7 @@ __host__ inline int64_t sample_blocks(int64_t total, int vec) {
 __host__ inline void sample_setup(SampleArgs &a, int64_t threads, int vec) {
     const LcgMap hop = lcg_jump_map((u128)(threads - 1) * (u128)vec);
     a.hop_mult = hop.mult;
+    a.hop_geo = hop.geo;
     a.hop_plus = hop.geo * a.start.inc;
     a.jump_digits = 0;
     for (uint64_t last = (uint64_t)(threads - 1) * (uint64_t)vec; last != 0; last >>= 4) a.jump_digits++;
@@ -59,16 +66,17 @@ __host__ __device__ __forceinline__ void store_vec(float *p, const float (&v)[4]
     *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
 }
 
-// the elements of thread `thread` of a grid of `threads` threads: T = long long (MultiDiscrete) or float (Box)
+// the elements of thread `thread` of a grid of `threads` threads, drawn from `start` (hop_plus: the hop's geo factor
+// times start.inc): T = long long (MultiDiscrete) or float (Box)
 template <typename T>
-__host__ __device__ __forceinline__ void sample_thread(const SampleArgs &a, T *out, int64_t thread, int64_t threads,
-                                                      const LcgJumpTable &table) {
+__host__ __device__ __forceinline__ void sample_thread(const SampleArgs &a, const Pcg64 &start, u128 hop_plus, T *out,
+                                                      int64_t thread, int64_t threads, const LcgJumpTable &table) {
     constexpr int VEC = 16 / sizeof(T);
     constexpr bool kDiscrete = std::is_same<T, long long>::value;
     const int64_t stride = threads * VEC;
     int64_t k0 = thread * VEC;
     if (k0 >= a.total) return;
-    Pcg64 g = a.start;
+    Pcg64 g = start;
     pcg64_jump_table(g, (uint64_t)k0, table);
     for (;;) {
         T v[VEC];
@@ -91,8 +99,41 @@ __host__ __device__ __forceinline__ void sample_thread(const SampleArgs &a, T *o
         }
         k0 += stride;
         if (k0 >= a.total) break;
-        g.state = a.hop_mult * g.state + a.hop_plus;
+        g.state = a.hop_mult * g.state + hop_plus;
     }
+}
+
+// ... from a.start, the generator passed by value
+template <typename T>
+__host__ __device__ __forceinline__ void sample_thread(const SampleArgs &a, T *out, int64_t thread, int64_t threads,
+                                                      const LcgJumpTable &table) {
+    sample_thread<T>(a, a.start, a.hop_plus, out, thread, threads, table);
+}
+
+// ---- the stream variant: the generator in a device record ----
+constexpr int kSampleRecordWords = 5;   // {state_hi, state_lo, inc_hi, inc_lo, ticket}
+
+struct SampleStream {
+    uint64_t *record;            // kSampleRecordWords words; the ticket is 0 between launches
+    int use_override;            // start from `override_words` instead of the record (and store it with its inc)
+    uint64_t override_words[4];
+    LcgMap advance;              // the map of `total` draws
+};
+
+// the generator a launch starts from
+__host__ __device__ inline Pcg64 sample_stream_start(const SampleStream &s) {
+    const uint64_t *w = s.use_override ? s.override_words : s.record;
+    return Pcg64{make_u128(w[0], w[1]), make_u128(w[2], w[3])};
+}
+
+// the record after the launch: `start` advanced by every draw of the batch, its inc, the ticket back at 0
+__host__ __device__ inline void sample_stream_finish(const SampleStream &s, Pcg64 start) {
+    pcg64_apply(start, s.advance);
+    s.record[0] = (uint64_t)(start.state >> 64);
+    s.record[1] = (uint64_t)start.state;
+    s.record[2] = (uint64_t)(start.inc >> 64);
+    s.record[3] = (uint64_t)start.inc;
+    s.record[4] = 0;
 }
 
 }  // namespace bgym

@@ -165,12 +165,18 @@ class ShardedVectorEnv:
         buf = self.buffers[self.env._flip]
         return buf.all_gather(self.group) if self.gather else buf.glob
 
+    def _no_capture(self, what):
+        from gym_b200.vector_env import refuse_capture
+        refuse_capture(f"ShardedVectorEnv.{what}()", "multi-GPU capture is not supported")
+
     def reset(self, *, seed=None, options=None):
+        self._no_capture("reset")
         # reset is off the hot path: always exchanged with the plain all-gather
         self.env.reset(seed=seed, options=options)
         return self._finish()["obs"], {}
 
     def step(self, actions_local):
+        self._no_capture("step")
         if self.p2p is not None:
             from gym_b200 import error
             from gym_b200.vector_env import FinalInfos

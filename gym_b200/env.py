@@ -12,7 +12,9 @@ single-env agents run unchanged; the throughput path is ``B200VectorEnv``.
 import numpy as np
 
 from gym_b200 import _lib, error
-from gym_b200.vector_env import B200VectorEnv, _unpickle
+from gym_b200.vector_env import B200VectorEnv, _unpickle, refuse_capture
+
+_NO_CAPTURE = "B200Env steps through host buffers and synchronises; capture a B200VectorEnv with backend='torch'"
 
 
 class B200Env:
@@ -31,10 +33,12 @@ class B200Env:
 
     # gym/core.py:86-151
     def reset(self, *, seed=None, options=None):
+        refuse_capture("B200Env.reset()", _NO_CAPTURE)
         obs, _ = self._vec.reset(seed=seed, options=options)
         return obs[0], {}
 
     def step(self, action):
+        refuse_capture("B200Env.step()", _NO_CAPTURE)
         v = self._vec
         if v.discrete:
             if not self.action_space.contains(action if not isinstance(action, np.ndarray) or action.shape == ()

@@ -18,6 +18,9 @@ Two output backends:
     -- a dense, sync-free form of the reference's object arrays
     (vector_env.py:235-258).  Output tensors are double-buffered: the tensors
     returned by step t stay valid until step t+2 (``copy=True`` clones instead).
+    ``step``, ``reset`` and ``sample_actions`` may be captured in a CUDA graph
+    (``torch.cuda.graph``): replays are bit-identical to eager calls, and what
+    cannot be captured raises ``error.Error`` (DESIGN.md §4.8).
 
 ``backend="numpy"`` (drop-in for CPU agents and for the parity tests)
     host buffers in, host buffers out, through ``b200gym_step_host``; returns
@@ -43,6 +46,19 @@ def _torch():
     return torch
 
 
+def capturing():
+    """True while torch's current CUDA stream is being captured into a graph (no CUDA call if CUDA is not up)."""
+    torch = _torch()
+    return torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()
+
+
+def refuse_capture(what, why):
+    """Raise ``error.Error`` for an operation that cannot be captured in a CUDA graph (before it makes any CUDA call,
+    so the env stays usable and the capture can be abandoned cleanly)."""
+    if capturing():
+        raise error.Error(f"{what} cannot be captured in a CUDA graph: {why}")
+
+
 def seed_words(seed):
     """Non-negative int < 2**128 -> (c_uint32 * 4) little-endian entropy words."""
     seed = int(seed)
@@ -63,15 +79,19 @@ def _unpickle(factory, args, kwargs, payload):
 
 class FinalInfos(dict):
     """``infos`` of the torch backend: the done masks (``_final_observation`` and, with per-env episode statistics,
-    ``_final_info``) are materialised on first access."""
+    ``_final_info``) are materialised on first access -- or at once while a CUDA graph is being captured, so that they
+    are outputs of the graph that every replay rewrites."""
 
-    def __init__(self, final_obs, terminated, truncated, final_info=None):
+    def __init__(self, final_obs, terminated, truncated, final_info=None, captured=None):
         super().__init__(final_observation=final_obs)
         self._t, self._u = terminated, truncated
         self._masks = ("_final_observation",)
         if final_info is not None:
             dict.__setitem__(self, "final_info", final_info)
             self._masks = ("_final_observation", "_final_info")
+        if capturing() if captured is None else captured:
+            for m in self._masks:
+                self._mask(m)
 
     def _mask(self, k):
         if not dict.__contains__(self, k):
@@ -160,6 +180,8 @@ class B200VectorEnv:
         self.discrete = hasattr(self.single_action_space, "n")
         self.act_dim = 0 if self.discrete else self.single_action_space.shape[0]
         self._sample_cache = None   # (single action space, its sample_actions plan)
+        self._sample_record = None  # the action-space stream on the device (sample_actions)
+        self._sample_mirror = None  # the host generator state the record holds, as far as the host knows
         self._chain = None
         if stages:
             # the chain's spaces are the wrapped env's (FrameStack / TimeAwareObservation / FlattenObservation reshape
@@ -214,6 +236,7 @@ class B200VectorEnv:
         self._has_reset = False
         self._state = _STATE_DEFAULT
         self._pending = None
+        self._captured = False   # whether the pending torch-backend step is being captured in a CUDA graph
         self._flip = 0
         self._out = None
         self._hio = None
@@ -223,6 +246,8 @@ class B200VectorEnv:
             self._t0 = time.perf_counter()
         if backend == "torch":
             self._out = [self._alloc_outputs(), self._alloc_outputs()]
+            # {state_hi, state_lo, inc_hi, inc_lo, ticket} of b200gym_sample_space_stream
+            self._sample_record = torch.zeros(8, dtype=torch.int64, device=self.device)
         else:
             self._map_host_buffers()
 
@@ -319,6 +344,8 @@ class B200VectorEnv:
                                                     self._stream()), self._handle)
             self._seeded = True
             return
+        refuse_capture("seed(<list>)", "per-env seeds are staged through host memory and synchronise; seed with an int "
+                       "or seed outside the capture")
         seeds = list(seed)
         assert len(seeds) == self.num_envs, "one seed per environment is required"
         ent = np.zeros((self.num_envs, 4), dtype=np.uint32)
@@ -344,6 +371,10 @@ class B200VectorEnv:
             raise error.AlreadyPendingCallError(
                 f"Calling `reset_async` while waiting for a pending call to `{self._state}` to complete",
                 self._state)
+        self._refuse_numpy_capture("reset")
+        if seed is not None and not isinstance(seed, (int, np.integer)):
+            refuse_capture("reset(seed=<list>)", "per-env seeds are staged through host memory and synchronise; "
+                           "seed with an int or reset outside the capture")
         bounds = _envs.parse_reset_bounds(self.kind, options)
         self.seed(seed)
         bptr = None
@@ -383,10 +414,19 @@ class B200VectorEnv:
         self.reset_async(seed=seed, options=options)
         return self.reset_wait(seed=seed, options=options)
 
+    def _refuse_numpy_capture(self, what):
+        if self.backend == "numpy":
+            refuse_capture(what, "backend='numpy' steps through page-locked host buffers and synchronises; capture "
+                           "an env with backend='torch'")
+
     # ------------------------------------------------------------------ step
-    def _device_actions(self, actions):
+    def _device_actions(self, actions, captured=False):
         """Bring `actions` to a contiguous device tensor of a dtype the kernel reads directly."""
         torch = _torch()
+        if captured and not (isinstance(actions, torch.Tensor) and actions.device == self.device):
+            raise error.Error(f"step() cannot be captured in a CUDA graph with actions that are not a CUDA tensor on "
+                              f"{self.device}: the host-to-device copy cannot be replayed (got "
+                              f"{type(actions).__name__}{' on ' + str(actions.device) if hasattr(actions, 'device') else ''})")
         if not isinstance(actions, torch.Tensor):
             actions = torch.as_tensor(np.asarray(actions))
         if self.discrete:
@@ -421,14 +461,17 @@ class B200VectorEnv:
                 self._state)
         if not self._has_reset:
             raise error.ResetNeeded("Cannot call env.step() before calling env.reset()")
+        self._refuse_numpy_capture("step")
         if self.backend == "torch":
+            self._captured = captured = capturing()
             # the reference asserts on an out-of-range Discrete action (cartpole.py:132); the device cannot raise and
             # this backend never waits for it, so the kernels flag it in host-visible memory and the error surfaces
-            # at the next call (no synchronisation unless the flag is up)
-            if self.discrete and self._lib.b200gym_invalid_seen(self._handle) == 1:
+            # at the next call (no synchronisation unless the flag is up; none at all while a graph is captured: an
+            # invalid action in a replay is reported by the next eager call)
+            if self.discrete and not captured and self._lib.b200gym_invalid_seen(self._handle) == 1:
                 self.check_actions()
             self._raise_snapshot_index_error()
-            act, code = self._device_actions(actions)
+            act, code = self._device_actions(actions, captured)
             c = self._chain
             if c is not None and c.act_stages:   # ClipAction / RescaleAction, outermost first
                 staged = _torch().empty_like(act)
@@ -495,7 +538,8 @@ class B200VectorEnv:
             if self.copy:
                 o = {k: v.clone() for k, v in o.items() if not k.startswith("raw_")}
             episode = {"episode": {"r": o["ep_r"], "l": o["ep_l"], "t": self._episode_time()}} if "ep_r" in o else None
-            infos = FinalInfos(o.get("final_obs64", o["final_obs"]), o["terminated"], o["truncated"], episode)
+            infos = FinalInfos(o.get("final_obs64", o["final_obs"]), o["terminated"], o["truncated"], episode,
+                               self._captured)
             return o["obs"], o["reward"], o["terminated"], o["truncated"], infos
         h = self._hio
         term = h["terminated"].view(np.bool_)   # the kernel writes 0/1 bytes
@@ -511,7 +555,7 @@ class B200VectorEnv:
             if "ep_r" in h:
                 ep_r, ep_l = (h["ep_r"].copy(), h["ep_l"].copy()) if self.copy else (h["ep_r"], h["ep_l"])
                 episode = {"episode": {"r": ep_r, "l": ep_l, "t": self._episode_time()}}
-            infos = FinalInfos(fo.copy() if self.copy else fo, term, trunc, episode)
+            infos = FinalInfos(fo.copy() if self.copy else fo, term, trunc, episode, False)
         elif self.autoreset:
             done = term | trunc
             if done.any():
@@ -541,6 +585,7 @@ class B200VectorEnv:
 
     def check_actions(self):
         """Number of out-of-range Discrete actions the device saw since the last check (syncs)."""
+        refuse_capture("check_actions()", "it synchronises")
         count = ctypes.c_int64(0)
         _lib.check(self._lib.b200gym_invalid_actions(self._handle, self._stream(), ctypes.byref(count)),
                    self._handle)
@@ -570,9 +615,13 @@ class B200VectorEnv:
         """``self.action_space.sample()``, drawn on the device: the same values bit for bit (int64 (N,) for Discrete
         kinds, float32 (N, A) for continuous ones) as a tensor on ``self.device``, enqueued on torch's current stream
         with no synchronisation, ready for ``step()``.  The space's generator ends where ``sample()`` would leave it,
-        so host and device sampling interleave freely.  ``backend="numpy"`` returns ``self.action_space.sample()``."""
+        so host and device sampling interleave freely.  ``backend="numpy"`` returns ``self.action_space.sample()``.
+
+        May be captured in a CUDA graph once an eager call has put the generator on the device: each replay draws the
+        next batch of the stream, which only the device follows until ``sync_action_space()`` (DESIGN §4.8)."""
         self._assert_open("sample_actions")
         space = self.action_space
+        self._refuse_numpy_capture("sample_actions")
         if self.backend == "numpy":
             return space.sample()
         n_choices, cols, low, high = self._sample_plan()
@@ -583,16 +632,48 @@ class B200VectorEnv:
         bit_generator = space.np_random.bit_generator
         state = pcg64_state(bit_generator)
         s, inc = state["state"]["state"], state["state"]["inc"]
+        # The draws come from the device record (b200gym_sample_space_stream), which the launch also advances, so a
+        # captured call continues the stream at every replay.  The mirror is what the host last left in the record:
+        # a host generator that differs from it (drawn from or reseeded on the host) is passed as the override.
+        in_sync = self._sample_mirror == (s, inc)
+        captured = capturing()
+        if captured:
+            if not in_sync:
+                raise error.Error("sample_actions() cannot be captured in a CUDA graph before the device holds the "
+                                  "action space's generator: call sample_actions() once outside the capture (after "
+                                  "any action_space.seed() or host draw)")
         mask = (1 << 64) - 1
-        words = (ctypes.c_uint64 * 4)(s >> 64, s & mask, inc >> 64, inc & mask)
+        words = None if in_sync else (ctypes.c_uint64 * 4)(s >> 64, s & mask, inc >> 64, inc & mask)
         torch = _torch()
         out = torch.empty(shape, dtype=torch.int64 if n_choices else torch.float32, device=self.device)
-        _lib.check(self._lib.b200gym_sample_space(words, self.num_envs, cols, n_choices,
-                                                  None if low is None else low.ctypes.data,
-                                                  None if high is None else high.ctypes.data,
-                                                  ctypes.c_void_p(out.data_ptr()), self._stream()))
-        pcg64_skip(bit_generator, state, out.numel())
+        _lib.check(self._lib.b200gym_sample_space_stream(ctypes.c_void_p(self._sample_record.data_ptr()), words,
+                                                         self.num_envs, cols, n_choices,
+                                                         None if low is None else low.ctypes.data,
+                                                         None if high is None else high.ctypes.data,
+                                                         ctypes.c_void_p(out.data_ptr()), self._stream()))
+        if not captured:   # a capture leaves the host where it is: replays advance the record alone
+            pcg64_skip(bit_generator, state, out.numel())
+            st = pcg64_state(bit_generator)["state"]
+            self._sample_mirror = (st["state"], st["inc"])
         return out
+
+    def sync_action_space(self):
+        """Move ``self.action_space``'s generator to where the device stream of ``sample_actions()`` is (synchronises).
+
+        Replays of a CUDA graph that captured ``sample_actions()`` advance that stream on the device only; until this
+        is called the host generator stays where the capture left it, and eager ``sample_actions()`` calls continue
+        the device stream, not the host one.  torch backend only."""
+        self._assert_open("sync_action_space")
+        refuse_capture("sync_action_space()", "it synchronises")
+        if self.backend == "numpy" or self._sample_mirror is None:
+            return   # the host generator is the stream
+        w = self._sample_record[:4].cpu().numpy().view(np.uint64)
+        s, inc = (int(w[0]) << 64) | int(w[1]), (int(w[2]) << 64) | int(w[3])
+        bit_generator = self.action_space.np_random.bit_generator
+        st = bit_generator.state   # the buffered 32-bit draw stays, as sample_actions() leaves it
+        st["state"] = {"state": s, "inc": inc}
+        bit_generator.state = st
+        self._sample_mirror = (s, inc)
 
     # ------------------------------------------------------------------ state access
     def get_state(self):
@@ -662,6 +743,7 @@ class B200VectorEnv:
 
     def set_state(self, state=None, elapsed=None, rng=None):
         self._assert_open("set_state")
+        refuse_capture("set_state()", "it synchronises")
         torch = _torch()
 
         def prep(x, dtype):
@@ -753,6 +835,7 @@ class B200VectorEnv:
 
     def _check_idle(self, what):
         self._assert_open(what)
+        refuse_capture(f"{what}()", "snapshots, restores and clones take host indices and synchronise")
         if self._state != _STATE_DEFAULT:
             raise error.AlreadyPendingCallError(f"Calling `{what}` while waiting for a pending call to `{self._state}` "
                                                 "to complete", self._state)

@@ -5,6 +5,10 @@
 * ``VectorListInfo``  gym/wrappers/vector_list_info.py:56-111
 * ``step_api_compatibility``  gym/utils/step_api_compatibility.py:24-161
 
+CUDA graphs: ``RecordEpisodeStatistics`` may be captured with the env it wraps (its ``"t"`` keeps the capture-time
+value on replays); the normalisers and ``VectorListInfo`` refuse to be captured -- the normalisers pick their
+statistics set by a host-side parity that a replay cannot flip, ``VectorListInfo`` synchronises.
+
 The first three run on the device through the C ABI -- ``RecordEpisodeStatistics`` inside the step
 kernel itself (no extra launch), the normalisers as two launches per step with one pass over the batch
 for the moments and, for sharded envs, an all-reduce of the 2 x dim batch sums in between -- with no
@@ -18,6 +22,10 @@ from collections import deque
 import numpy as np
 
 from gym_b200 import _lib
+from gym_b200.vector_env import refuse_capture
+
+_NORM_NO_CAPTURE = ("the running statistics are double-buffered by a host-side parity that replays would not flip, so "
+                    "they would stop updating; step the normaliser eagerly")
 
 
 def _p(t):
@@ -342,10 +350,12 @@ class NormalizeObservation(VectorWrapper):
         return self._normalize(obs, update=False)
 
     def reset(self, **kwargs):
+        refuse_capture("NormalizeObservation.reset()", _NORM_NO_CAPTURE)
         obs, info = self.env.reset(**kwargs)
         return self._normalize(obs), info
 
     def step(self, actions):
+        refuse_capture("NormalizeObservation.step()", _NORM_NO_CAPTURE)
         obs, rew, term, trunc, infos = self.env.step(actions)
         return self._normalize(obs), rew, term, trunc, infos
 
@@ -366,8 +376,13 @@ class NormalizeReward(VectorWrapper):
         self._flip = 0
         self._group, self._world = _shard_group(env, group)
 
+    def reset(self, **kwargs):
+        refuse_capture("NormalizeReward.reset()", _NORM_NO_CAPTURE)
+        return self.env.reset(**kwargs)
+
     def step(self, actions):
         torch = self._torch
+        refuse_capture("NormalizeReward.step()", _NORM_NO_CAPTURE)
         obs, rew, term, trunc, infos = self.env.step(actions)
         if self.returns is None or self.returns.shape != rew.shape:
             self.returns = torch.zeros_like(rew)
@@ -439,10 +454,12 @@ class VectorListInfo(VectorWrapper):
         return out
 
     def reset(self, **kwargs):
+        refuse_capture("VectorListInfo.reset()", "it copies infos to the host")
         obs, infos = self.env.reset(**kwargs)
         return obs, self._convert(infos)
 
     def step(self, actions):
+        refuse_capture("VectorListInfo.step()", "it copies infos to the host")
         obs, rew, term, trunc, infos = self.env.step(actions)
         return obs, rew, term, trunc, self._convert(infos)
 

@@ -489,6 +489,23 @@ int b200gym_sample_space(const uint64_t pcg64[4], int64_t rows, int cols, int64_
                          const double *high_host, void *out_dev, void *stream);
 
 /*
+ * b200gym_sample_space with the generator in a device record instead of the arguments, so that the launch can be
+ * captured in a CUDA graph and every replay continues the stream: ONE launch reads the record, samples, and writes
+ * the record back advanced by rows * cols draws.
+ *   record_dev       5 uint64 words on the device of out_dev, 16-byte aligned: {state_hi, state_lo, inc_hi, inc_lo}
+ *                    of the space's PCG64, then a ticket word that must be 0 before the first launch (every launch
+ *                    leaves it at 0).  Launches on one record must be ordered (one stream, or events between them).
+ *   override_pcg64   NULL: start from the record.  Otherwise {state_hi, state_lo, inc_hi, inc_lo} to start from instead
+ *                    (passed by value, e.g. after the host generator was reseeded); the record then ends at this
+ *                    generator advanced, with its inc.
+ * Everything the launch derives from inc is computed on the device from the generator it starts from, so a graph
+ * captured before a reseed stays consistent after it.  Other arguments and errors as b200gym_sample_space.
+ */
+int b200gym_sample_space_stream(uint64_t *record_dev, const uint64_t override_pcg64[4], int64_t rows, int cols,
+                                int64_t n_choices, const double *low_host, const double *high_host, void *out_dev,
+                                void *stream);
+
+/*
  * Box2D tasks: number of envs in which a touching (body, ground fixture) pair was ever dropped because the scene's
  * manifold table was full (8 pairs for LunarLander*, 10 for BipedalWalker*; real Box2D has no such limit).  The
  * dropped pair is treated as not touching -- the CPU oracle applies the identical rule -- so this counts
