@@ -144,7 +144,6 @@ SIGNATURES = {
     "b200gym_step_p2p": (_i32, [_vp, _vp, _i32, _vp, _vp, ctypes.POINTER(_i32)]),
     "b200gym_p2p_status": (_i32, [_vp, _vp, ctypes.POINTER(_i32)]),
     "b200gym_episode_stats": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp]),
-    "b200gym_set_episode_stats": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200gym_rms_moments": (_i32, [_vp, _i32, _i64, _i32, _vp, _vp, _vp]),
     "b200gym_return_moments": (_i32, [_vp, _vp, ctypes.c_double, _i64, _vp, _vp, _vp]),
     "b200gym_rms_apply_obs": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i32, _vp]),

@@ -59,18 +59,13 @@ struct b200gym {
     unsigned long long *invalid = nullptr;  // sticky device counter
     unsigned long long *invalid_seen = nullptr;      // page-locked, device-mapped word: set to 1 by any kernel that meets an
     unsigned long long *invalid_seen_dev = nullptr;  // invalid action (host-visible WITHOUT a synchronisation); device alias
-    struct {                                // caller-owned buffers of the fused RecordEpisodeStatistics (all null = off)
-        float *acc = nullptr; int32_t *len = nullptr; float *r = nullptr; int32_t *l = nullptr;
-        unsigned long long *ring = nullptr, *counter = nullptr; int ring_size = 0;
-    } ep;
     int sm_count = 132;
-    int occ[B200GYM_NUM_KINDS][3][2] = {};  // cached CTAs/SM of step_kernel_persistent per (kind, action width, lean)
+    int occ[B200GYM_NUM_KINDS][3] = {};     // cached CTAs/SM of step_kernel_persistent per (kind, action width)
     int occ_bulk[B200GYM_NUM_KINDS][3] = {};  // ... of step_kernel_persistent_bulk per (kind, action width)
-    int kernel_choice = -1;                 // -1: kernel B (bulk copies) where bulk_by_default picks it, else P's lean
-                                            // instantiation; 0: kernel A (one tile per CTA), 1: kernel P (resident grid,
-                                            // asynchronous prefetch, deferred resets), 2: P's lean instantiation where it
-                                            // applies (else P), 3: kernel B where it applies (else lean P);
-                                            // B200GYM_KERNEL=a|p|l|b overrides
+    int kernel_choice = -1;                 // -1: kernel B (bulk copies) where bulk_by_default picks it, else P;
+                                            // 0: kernel A (one tile per CTA), 1: kernel P (resident grid, asynchronous
+                                            // prefetch, deferred resets) where it applies, 2: kernel B where it applies
+                                            // (else P); B200GYM_KERNEL=a|p|b overrides (l: the same as p)
     int box2d_defer = 1;                    // Box2D tasks: 1 = the autoresets of a step run in a last, compacted kernel
                                             // (B200GYM_BOX2D_DEFER=0: inline).  With the TOI kernel it takes reset() +
                                             // its embedded world step off the critical path of the envs that crash in a
@@ -250,7 +245,7 @@ struct InPlaceSink {
 // The per-env work is one long dependent float64 chain and the SMs are latency-bound, but occupancy is not the
 // lever: at 32 registers (8 CTAs x 256 threads = 64 warps/SM) the hot loop spills the state across the division
 // slow-path calls, and those local-memory round trips cost more than the extra warps hide.  6 CTAs/SM of 256
-// threads leaves 40 registers a thread (64K registers per SM), which the lean loop fits without a spill.
+// threads leaves 40 registers a thread (64K registers per SM), which kernel P's loop fits without a spill.
 #ifndef B200_MIN_CTAS
 #define B200_MIN_CTAS 6
 #endif
@@ -399,14 +394,13 @@ struct PrefetchLayout {
     static constexpr int kBytes = kElapsedOff + kThreads * 4;
 };
 
-// LEAN (the single-GPU step without the fused RecordEpisodeStatistics, fewer than 2^31 envs): 32-bit env indices
-// (one IMAD.WIDE per address instead of a 64-bit add chain), no per-peer store loops, no episode accounting --
-// same arithmetic, same stores, fewer issue slots.
-template <int KIND, typename ActT, bool LEAN>
+// Single-GPU step of a handle of fewer than 2^30 envs (launch_step_typed checks): 32-bit env indices (one IMAD.WIDE
+// per address instead of a 64-bit add chain) and no per-peer store loops.
+template <int KIND, typename ActT>
 __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_persistent(const StepArgs a, const int num_tiles) {
     using E = Env<KIND>;
     using L = PrefetchLayout<KIND, ActT>;
-    using Idx = typename std::conditional<LEAN, uint32_t, int64_t>::type;
+    using Idx = uint32_t;
     // one stage of per-thread input slots holds the next tile in flight: a thread moves its slot into registers
     // before it refills it
     __shared__ __align__(16) unsigned char in_mem[L::kBytes];
@@ -417,7 +411,7 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
     __syncthreads();
 
     const ActT *actions = reinterpret_cast<const ActT *>(a.actions);
-    const DirectSinkT<!LEAN> sink{a};
+    const DirectSinkT<false> sink{a};
     const Idx first = (Idx)a.first, count = (Idx)a.count;
 
     auto prefetch = [&](int tile) {
@@ -456,7 +450,7 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
         float a0 = 0.0f;
         decode_action<KIND>(av, action_int, a0);
         bool need = false;
-        if (in_range) need = advance_env<KIND, !LEAN>(a, sink, i, s, elapsed, action_int, a0);
+        if (in_range) need = advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0);
         const unsigned m = __ballot_sync(0xffffffffu, need);
         if (m != 0u) {
             bool inline_reset = __popc(m) >= 12;          // dense enough: reset right here
@@ -717,7 +711,7 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
             long long action_int = 0;
             float a0 = 0.0f;
             decode_action<KIND>(av, action_int, a0);
-            const bool need = advance_env<KIND, false>(a, sink, i, s, elapsed, action_int, a0);
+            const bool need = advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0);
             const unsigned m = __ballot_sync(0xffffffffu, need);
             PH_CLOCK(w2);
             PH_ACC(kPhAdvance, w1, w2);
@@ -1413,7 +1407,7 @@ static inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads -
 // ---------------------------------------------------------------------------
 // dispatch
 // ---------------------------------------------------------------------------
-// Kernel B by default where it measured faster than lean P (DESIGN §4.1): CartPole, at 2^18, 2^20 and 2^23 envs.  The other
+// Kernel B by default where it measured faster than kernel P (DESIGN §4.1): CartPole, at 2^18, 2^20 and 2^23 envs.  The other
 // kinds are slower with it at 2^18 envs -- one partly filled wave, latency-bound, where B's 32 compute warps per SM
 // (P: 48) cost more than moving the memory traffic off the compute warps saves
 static bool bulk_by_default(int kind) { return kind == B200GYM_CARTPOLE; }
@@ -1427,7 +1421,7 @@ static constexpr int act_width_slot() { return sizeof(ActT) == 8 ? 0 : sizeof(Ac
 template <int KIND, typename ActT>
 static int prepare_step_typed(b200gym *h) {
     const int w = act_width_slot<ActT>();
-    if (h->kernel_choice == 3 || (h->kernel_choice == -1 && bulk_by_default(KIND))) {
+    if (h->kernel_choice == 2 || (h->kernel_choice == -1 && bulk_by_default(KIND))) {
         const int smem = kBulkStages * BulkLayout<KIND, ActT>::kBytes;
         int &occ = h->occ_bulk[KIND][w];
         CK(h, cudaFuncSetAttribute(step_kernel_persistent_bulk<KIND, ActT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -1437,12 +1431,9 @@ static int prepare_step_typed(b200gym *h) {
         if (occ < 1) occ = 1;
     }
     if (h->kernel_choice != 0) {
-        for (int lean = 0; lean < 2; lean++) {
-            int &occ = h->occ[KIND][w][lean];
-            const auto kernel = lean ? step_kernel_persistent<KIND, ActT, true> : step_kernel_persistent<KIND, ActT, false>;
-            CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 0));
-            if (occ < 1) occ = 1;
-        }
+        int &occ = h->occ[KIND][w];
+        CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, step_kernel_persistent<KIND, ActT>, kThreads, 0));
+        if (occ < 1) occ = 1;
     }
     return 0;
 }
@@ -1491,9 +1482,10 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
             h->p2p_barrier_fused = fused_barrier;
         }
     }
-    const bool resident = a.npeer == 0 && a.count >= (int64_t)h->sm_count * kThreads;
-    const bool bulk = h->kernel_choice == 3 || (h->kernel_choice == -1 && bulk_by_default(KIND));
-    if (done == 0 && resident && bulk && !a.ep_acc && h->n < (int64_t)1 << 30) {
+    // the resident kernels index envs in 32 bits; larger handles step on kernel A
+    const bool resident = a.npeer == 0 && a.count >= (int64_t)h->sm_count * kThreads && h->n < (int64_t)1 << 30;
+    const bool bulk = h->kernel_choice == 2 || (h->kernel_choice == -1 && bulk_by_default(KIND));
+    if (done == 0 && resident && bulk) {
         // kernel B: whole tiles, every row a bulk copy touches 16-byte aligned
         using L = BulkLayout<KIND, ActT>;
         const auto al = [](const void *p) { return (uintptr_t)p % 16 == 0; };
@@ -1516,14 +1508,11 @@ static int launch_step_typed(b200gym *h, const StepArgs &a, cudaStream_t st) {
         using L = PrefetchLayout<KIND, ActT>;
         const bool aligned = !L::kActAsync || ((uintptr_t)a.actions % L::kActBytes == 0);
         if (aligned) {
-            // the lean instantiation: no fused episode statistics, every index fits 32 bits
-            const bool lean = h->kernel_choice != 1 && !a.ep_acc && h->n < (int64_t)1 << 30;
-            const auto kernel = lean ? step_kernel_persistent<KIND, ActT, true> : step_kernel_persistent<KIND, ActT, false>;
-            const int occ = h->occ[KIND][act_width_slot<ActT>()][lean ? 1 : 0];   // prepare_step_typed, at create
+            const int occ = h->occ[KIND][act_width_slot<ActT>()];   // prepare_step_typed, at create
             const int64_t all_tiles = (a.count + kThreads - 1) / kThreads;
             int64_t grid = (int64_t)h->sm_count * occ;
             if (grid > all_tiles) grid = all_tiles;
-            kernel<<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
+            step_kernel_persistent<KIND, ActT><<<(unsigned)grid, kThreads, 0, st>>>(a, (int)all_tiles);
             CK(h, cudaGetLastError());
             done = a.count;
         }
@@ -1759,7 +1748,7 @@ extern "C" int b200gym_create(const b200gym_config *cfg, int64_t num_envs, int d
     {
         const char *kc = getenv("B200GYM_KERNEL");
         if (kc && (kc[0] == 'a' || kc[0] == 'p' || kc[0] == 'l' || kc[0] == 'b'))
-            h->kernel_choice = kc[0] == 'a' ? 0 : kc[0] == 'p' ? 1 : kc[0] == 'l' ? 2 : 3;
+            h->kernel_choice = kc[0] == 'a' ? 0 : kc[0] == 'b' ? 2 : 1;
         const char *pfb = getenv("B200GYM_P2P_FUSE_BARRIER");
         if (pfb && (pfb[0] == '0' || pfb[0] == '1')) h->p2p_fuse = pfb[0] - '0';
         const char *btd = getenv("B200GYM_BOX2D_TOI_DEFER");
@@ -1945,8 +1934,6 @@ static StepArgs make_args(b200gym *h, const void *actions, float *obs, double *r
     a.p2p_step = 0; a.p2p_timeout_ns = 0; a.p2p_world = 0; a.p2p_rank = 0;
     a.npeer = 0;
     a.bulk_sink = 0;
-    a.ep_acc = h->ep.acc; a.ep_len = h->ep.len; a.ep_r = h->ep.r; a.ep_l = h->ep.l;
-    a.ep_ring = h->ep.ring; a.ep_counter = h->ep.counter; a.ep_ring_size = h->ep.ring_size;
     return a;
 }
 
@@ -2172,20 +2159,6 @@ extern "C" int b200gym_p2p_status(b200gym_t *h, void *stream, int *timed_out_pee
 }
 
 // ---- stateless device utilities for the vector-aware wrappers (SURVEY.md 8f) -----------------------
-extern "C" int b200gym_set_episode_stats(b200gym_t *h, float *return_acc_dev, int32_t *length_acc_dev, float *episode_r_dev,
-                                         int32_t *episode_l_dev, uint64_t *ring_dev, uint64_t *counter_dev, int ring_size) {
-    if (!h) return fail(h, "b200gym_set_episode_stats: null handle");
-    if (!return_acc_dev) {   // off
-        h->ep = {};
-        return 0;
-    }
-    if (!length_acc_dev || !episode_r_dev || !episode_l_dev || !counter_dev || ring_size < 0 || (ring_size > 0 && !ring_dev))
-        return fail(h, "b200gym_set_episode_stats: bad argument");
-    h->ep.acc = return_acc_dev; h->ep.len = length_acc_dev; h->ep.r = episode_r_dev; h->ep.l = episode_l_dev;
-    h->ep.ring = (unsigned long long *)ring_dev; h->ep.counter = (unsigned long long *)counter_dev; h->ep.ring_size = ring_size;
-    return 0;
-}
-
 extern "C" int b200gym_episode_stats(const double *reward_dev, const uint8_t *terminated_dev, const uint8_t *truncated_dev,
                                      float *return_acc_dev, int32_t *length_acc_dev, float *episode_r_dev,
                                      int32_t *episode_l_dev, uint8_t *episode_mask_dev, uint64_t *ring_dev,

@@ -47,16 +47,6 @@ struct StepArgs {
     int32_t *toi_list;
     int32_t *toi_count;
     uint32_t *toi_mid;
-    // fused all-gather (multi-GPU): every result is ALSO stored into the same rows of the peers'
-    // gather buffers over NVLink (peer-mapped pointers, slice offset already applied)
-    // RecordEpisodeStatistics fused into the step (b200gym_set_episode_stats; nullptr = off): float32 return and
-    // int32 length accumulators, infos["episode"]["r"/"l"] rows of finishing envs, ring of recent episodes
-    float *ep_acc;
-    int32_t *ep_len;
-    float *ep_r;
-    int32_t *ep_l;
-    unsigned long long *ep_ring, *ep_counter;
-    int32_t ep_ring_size;
     // fused all-gather: the step barrier in kernel G's tail (null = the separate p2p_sync_kernel / no exchange).  The
     // last CTA of the launch to finish its pushes publishes "my rows of step `p2p_step` are in your buffers" to every
     // peer and waits for theirs, so the exchange costs no launch of its own
@@ -68,6 +58,8 @@ struct StepArgs {
     int32_t p2p_world, p2p_rank;
     int32_t bulk_sink;   // 1: use kernel G's staged bulk stores even without peers (host path: the output arrays are
                          // mapped host memory, where many small stores are what hurts)
+    // fused all-gather (multi-GPU): every result is ALSO stored into the same rows of the peers'
+    // gather buffers over NVLink (peer-mapped pointers, slice offset already applied)
     int32_t npeer;
     float *peer_obs[B200GYM_MAX_PEERS];
     double *peer_reward[B200GYM_MAX_PEERS];
@@ -115,30 +107,6 @@ __device__ __forceinline__ void store_scalars_all(const StepArgs &a, I i, double
     }
 }
 
-// RecordEpisodeStatistics.step (gym/wrappers/record_episode_statistics.py:103-151) for env i, fused into the step
-// kernels: `episode_returns += rewards` on a float32 array with float64 rewards (add in float64, round to float32),
-// `episode_lengths += 1`; on terminated | truncated emit both, append to the ring (return_queue / length_queue),
-// start over from zero.
-template <typename I>
-__device__ __forceinline__ void episode_account(const StepArgs &a, I i, double reward, bool done) {
-    if (!a.ep_acc) return;
-    const float ret = (float)((double)a.ep_acc[i] + reward);
-    const int32_t len = a.ep_len[i] + 1;
-    if (done) {
-        a.ep_r[i] = ret;
-        a.ep_l[i] = len;
-        const unsigned long long slot = atomicAdd(a.ep_counter, 1ULL);
-        if (a.ep_ring_size > 0)   // one 64-bit store per episode {length : return bits}: a slot never mixes two episodes
-            a.ep_ring[slot % (unsigned long long)a.ep_ring_size] =
-                ((unsigned long long)(uint32_t)len << 32) | (unsigned long long)__float_as_uint(ret);
-        a.ep_acc[i] = 0.0f;
-        a.ep_len[i] = 0;
-    } else {
-        a.ep_acc[i] = ret;
-        a.ep_len[i] = len;
-    }
-}
-
 // Where the results of env i go.  DirectSink: straight to the caller's arrays (and, when peers are mapped,
 // to theirs) with per-thread stores; final_obs rows (info["final_observation"]) are never peer-mapped.  The kernels that stage their outputs in shared memory have sinks of their own
 // (b200gym.cu: StagedSink, InPlaceSink).
@@ -183,7 +151,7 @@ __device__ __forceinline__ void decode_action(ActT av, long long &action_int, fl
 // Phase 1, by the thread that owns env i (its inputs are in registers): Env.step, TimeLimit,
 // stores of reward / flags / final_obs, and -- unless the episode ended -- of the new state and
 // observation.  Returns true when the env must be reset by phase 2.
-template <int KIND, bool EP = true, typename Sink, typename I>
+template <int KIND, typename Sink, typename I>
 __device__ __forceinline__ bool advance_env(const StepArgs &a, const Sink &sink, I i, double (&s)[bgym::Env<KIND>::S],
                                             int32_t elapsed, long long action_int, float a0) {
     using E = bgym::Env<KIND>;
@@ -225,7 +193,6 @@ __device__ __forceinline__ bool advance_env(const StepArgs &a, const Sink &sink,
     const bool needs_reset = (terminated || truncated) && a.autoreset;   // sync_vector_env.py:152-156
 
     sink.scalars(i, reward, terminated ? 1 : 0, truncated ? 1 : 0);
-    if constexpr (EP) episode_account(a, i, reward, terminated || truncated);
     if (needs_reset) {
         sink.template final_obs<E::D>(i, obs);                            // info["final_observation"]
     } else {
@@ -332,7 +299,6 @@ __device__ __noinline__ void lunar_finish(const StepArgs &a, int64_t i, int64_t 
     elapsed += 1;                                                        // time_limit.py:51
     const bool truncated = (a.max_steps > 0) && (elapsed >= a.max_steps);
     store_scalars_all(a, i, reward, terminated ? 1 : 0, truncated ? 1 : 0);
-    episode_account(a, i, reward, terminated || truncated);
     bool deferred = false;
     if ((terminated || truncated) && a.autoreset) {                      // sync_vector_env.py:152-156
         if (a.final_obs) store_row<8>(a.final_obs, i, obs);
@@ -469,7 +435,6 @@ __device__ __noinline__ void walker_finish(const StepArgs &a, int64_t i, int64_t
     elapsed += 1;                                                        // time_limit.py:51
     const bool truncated = (a.max_steps > 0) && (elapsed >= a.max_steps);
     store_scalars_all(a, i, reward, terminated ? 1 : 0, truncated ? 1 : 0);
-    episode_account(a, i, reward, terminated || truncated);
     bool deferred = false;
     if ((terminated || truncated) && a.autoreset) {                      // sync_vector_env.py:152-156
         if (a.final_obs) store_row<24>(a.final_obs, i, obs);

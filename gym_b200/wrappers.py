@@ -9,9 +9,9 @@ CUDA graphs: ``RecordEpisodeStatistics`` may be captured with the env it wraps (
 value on replays); the normalisers and ``VectorListInfo`` refuse to be captured -- the normalisers pick their
 statistics set by a host-side parity that a replay cannot flip, ``VectorListInfo`` synchronises.
 
-The first three run on the device through the C ABI -- ``RecordEpisodeStatistics`` inside the step
-kernel itself (no extra launch), the normalisers as two launches per step with one pass over the batch
-for the moments and, for sharded envs, an all-reduce of the 2 x dim batch sums in between -- with no
+The first three run on the device through the C ABI -- ``RecordEpisodeStatistics`` as one launch per
+step over the rewards and flags the wrapped env returned, the normalisers as two launches per step with one pass
+over the batch for the moments and, for sharded envs, an all-reduce of the 2 x dim batch sums in between -- with no
 Python loop over the batch and no host synchronisation; the last two are host-side adapters.  They wrap
 a ``B200VectorEnv`` with ``backend="torch"`` (or a ``ShardedVectorEnv``).
 """
@@ -164,41 +164,19 @@ class RecordEpisodeStatistics(VectorWrapper):
         self.episode_lengths.zero_()
         return out
 
-    def _fused_target(self):
-        """The engine handle whose step kernel can do the bookkeeping itself: the wrapped env must be the
-        B200VectorEnv proper (torch backend) -- not a sharded env returning gathered global tensors, not another
-        wrapper that changes rewards, and without a per-env wrapper chain that changes them (gym_b200.subenv: the step
-        kernel would account the raw rewards, before the chain transforms them)."""
-        from gym_b200.vector_env import B200VectorEnv
-        e = self.env
-        if not (isinstance(e, B200VectorEnv) and e.backend == "torch" and e.num_envs == self.num_envs):
-            return None
-        return None if (e._chain is not None and e._chain.changes_rewards) else e
-
     def step(self, actions):
         self._flip ^= 1
         k = self._flip
-        fused = self._fused_target()
-        if fused is not None:
-            # one call that only stores pointers; the step kernel launched next does the accounting
-            _lib.check(fused._lib.b200gym_set_episode_stats(
-                fused._handle, _p(self.episode_returns), _p(self.episode_lengths), _p(self._ep_r[k]), _p(self._ep_l[k]),
-                _p(self._ring), _p(self._counter), self.deque_size), fused._handle)
-            try:
-                obs, rew, term, trunc, infos = self.env.step(actions)
-            finally:
-                fused._lib.b200gym_set_episode_stats(fused._handle, None, None, None, None, None, None, 0)
-            mask = term | trunc
-        else:
-            obs, rew, term, trunc, infos = self.env.step(actions)
-            env = self.env.unwrapped
-            _lib.check(env._lib.b200gym_episode_stats(
-                _p(rew), _p(term), _p(trunc), _p(self.episode_returns), _p(self.episode_lengths), _p(self._ep_r[k]),
-                _p(self._ep_l[k]), _p(self._ep_m[k]), _p(self._ring), _p(self._counter),
-                self.deque_size, self.num_envs, env._stream()))
-            mask = self._ep_m[k]
+        obs, rew, term, trunc, infos = self.env.step(actions)
+        # one launch over the rewards and flags step() returned: what a per-env wrapper chain or another wrapper made
+        # of them is what gets summed
+        env = self.env.unwrapped
+        _lib.check(env._lib.b200gym_episode_stats(
+            _p(rew), _p(term), _p(trunc), _p(self.episode_returns), _p(self.episode_lengths), _p(self._ep_r[k]),
+            _p(self._ep_l[k]), _p(self._ep_m[k]), _p(self._ring), _p(self._counter),
+            self.deque_size, self.num_envs, env._stream()))
         infos["episode"] = {"r": self._ep_r[k], "l": self._ep_l[k], "t": round(time.perf_counter() - self.t0, 6)}
-        infos["_episode"] = mask
+        infos["_episode"] = self._ep_m[k]
         return obs, rew, term, trunc, infos
 
     # snapshots: the per-env accumulators follow the envs, the ring and the counter are saved and restored whole

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200GYM_VERSION 2
+#define B200GYM_VERSION 3
 
 /* Environment kinds: the dynamics classes on the hot path. */
 enum b200gym_kind {
@@ -311,22 +311,18 @@ int b200gym_p2p_status(b200gym_t *h, void *stream, int *timed_out_peer);
  * device buffers; the stateless utilities report errors through b200gym_last_error(NULL) and run on the
  * device their buffers live on.
  *
- * RecordEpisodeStatistics (gym/wrappers/record_episode_statistics.py:79-151), fused INTO the step kernels:
- * after b200gym_set_episode_stats() every step launch also keeps the float32 return / int32 length
- * accumulators (`episode_returns += rewards` on a float32 array: add in float64, round to float32),
- * writes infos["episode"]["r"/"l"] for the envs whose episode ended in that step (the `_episode` mask is
- * terminated | truncated) and appends them to a ring of `ring_size` recent episodes (return_queue /
- * length_queue); *counter_dev counts finished episodes.  ring_dev[k] = (uint64)length << 32 | float32 bits
- * of the return, one store per episode into slot (episode number mod ring_size); episodes that finish in
- * the same step are numbered in no particular order (the reference appends them in env order), and when
- * more than ring_size finish at once the ring keeps an arbitrary ring_size of them.  The pointers may be
- * changed between steps (double buffering of the r / l rows); return_acc_dev == NULL switches it off.
- * No extra launch, no extra pass over reward / flags.
+ * RecordEpisodeStatistics (gym/wrappers/record_episode_statistics.py:79-151) as one launch over the n
+ * (reward, terminated, truncated) device arrays a step returned -- a B200VectorEnv's own outputs, the gathered
+ * global tensors of a sharded env, or the rewards of a wrapper chain.  It keeps the float32 return / int32
+ * length accumulators (`episode_returns += rewards` on a float32 array: add in float64, round to float32),
+ * writes infos["episode"]["r"/"l"] for the envs whose episode ended in that step and the `_episode` mask
+ * (terminated | truncated), and appends those episodes to a ring of `ring_size` recent episodes
+ * (return_queue / length_queue); *counter_dev counts finished episodes, also when ring_size is 0.
+ * ring_dev[k] = (uint64)length << 32 | float32 bits of the return, one store per episode into slot (episode
+ * number mod ring_size); episodes that finish in the same step are numbered in no particular order (the
+ * reference appends them in env order), and when more than ring_size finish at once the ring keeps an
+ * arbitrary ring_size of them.
  */
-int b200gym_set_episode_stats(b200gym_t *h, float *return_acc_dev, int32_t *length_acc_dev, float *episode_r_dev,
-                              int32_t *episode_l_dev, uint64_t *ring_dev, uint64_t *counter_dev, int ring_size);
-/* The same bookkeeping as ONE stand-alone launch over arbitrary (reward, terminated, truncated) device arrays --
- * e.g. the gathered global tensors of a sharded env; also writes the `_episode` mask. */
 int b200gym_episode_stats(const double *reward_dev, const uint8_t *terminated_dev, const uint8_t *truncated_dev,
                           float *return_acc_dev, int32_t *length_acc_dev, float *episode_r_dev, int32_t *episode_l_dev,
                           uint8_t *episode_mask_dev, uint64_t *ring_dev, uint64_t *counter_dev,

@@ -1,7 +1,7 @@
 #!/bin/bash
 # Where the time of the CartPole step goes on one H100 (DESIGN §4.1): the memory floor (scripts/membench.cu, the
 # step's bytes with no arithmetic), the compute floor (scripts/cartpole_floors.py, state resident in L2), and the
-# kernels themselves (bench.py headline and 2^23 strong-scaling line): lean P and the default (kernel B).
+# kernels themselves (bench.py headline and 2^23 strong-scaling line): kernel P and the default (kernel B).
 # Usage, from the repository root after build(): scripts/h100_floors.sh OUT_DIR
 OUT="${1:?usage: scripts/h100_floors.sh OUT_DIR}"
 mkdir -p "$OUT"
@@ -12,7 +12,7 @@ rm -rf "$T"
 for k in l b; do
   B200GYM_KERNEL=$k timeout 300 python scripts/cartpole_floors.py | tee -a "$OUT/floors_compute.jsonl"
 done
-# "l": lean P; "default": kernel B (bench.py labels only the letters a|p|l)
+# "l": kernel P; "default": kernel B (bench.py labels only the letters a|p|l)
 for v in l default; do
   if [ "$v" = default ]; then
     timeout 600 python bench.py --steps 400 --warmup 50 --no-cpu-baseline --no-e2e 2>/dev/null | tail -1 > "$OUT/floors_bench_$v.json"

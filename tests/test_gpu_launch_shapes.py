@@ -29,12 +29,11 @@ NTHREADS = os.cpu_count() or 1
 # at 49 every B CTA walks >= 7 tiles; at 96 every B CTA walks >= 13 and every P CTA >= 12.
 SHAPES = {"bulk_shape": 49, "persistent_shape": 96}
 
-# engine variants: kernel A (the reference for the others), B, P, and P's lean instantiation
+# engine variants: kernel A (the reference for the others), B and P
 VARIANTS = {
     "a": dict(B200GYM_KERNEL="a"),
     "b": dict(B200GYM_KERNEL="b"),
     "p": dict(B200GYM_KERNEL="p"),
-    "l": dict(B200GYM_KERNEL="l"),
 }
 
 
@@ -270,7 +269,7 @@ def test_invalid_actions_in_later_round_tiles(env_id, dtype):
 
 # (env_id, N, max_episode_steps, action dtype, steps).  CartPole at 2^20 runs kernel B; at max_episode_steps=37 every
 # env that survives 37 steps truncates, at step 37 all at once and from then on in nearly every step, over three
-# cycles.  The other kinds at 2^18 run lean P and run past their TimeLimit once.
+# cycles.  The other kinds at 2^18 run kernel P and run past their TimeLimit once.
 BENCH_CASES = [
     pytest.param("CartPole-v1", 1 << 20, None, "int64", 64, id="CartPole-2^20-int64"),
     pytest.param("CartPole-v1", 1 << 20, None, "uint8", 64, id="CartPole-2^20-uint8"),

@@ -330,13 +330,13 @@ def test_persistent_kernel_equals_simple_kernel(env_id, tiles_per_sm, monkeypatc
     N = 132 * 256 * 9 + 178 if tiles_per_sm == 9 else tiles_per_sm * sms * 256 + 176
     T = 90
     envs = {}
-    for k in ("a", "p", "l"):   # "l": the lean instantiation of kernel P (32-bit indices, no peer / episode code)
+    for k in ("a", "p"):
         monkeypatch.setenv("B200GYM_KERNEL", k)
         envs[k] = gym_b200.vector.make(env_id, N, max_episode_steps=40)
     monkeypatch.delenv("B200GYM_KERNEL")
     obs = {k: e.reset(seed=99)[0] for k, e in envs.items()}
-    assert torch.equal(obs["a"], obs["p"]) and torch.equal(obs["a"], obs["l"])
-    ea, ep, el_ = envs["a"], envs["p"], envs["l"]
+    assert torch.equal(obs["a"], obs["p"])
+    ea, ep = envs["a"], envs["p"]
     acts = torch.as_tensor(_actions(env_id, np.random.default_rng(11), T, N, wild=True), device=ea.device)
     dtypes = [torch.int64, torch.int32, torch.uint8] if ea.discrete else [torch.float32]
     n_done = 0
@@ -344,17 +344,15 @@ def test_persistent_kernel_equals_simple_kernel(env_id, tiles_per_sm, monkeypatc
         a = acts[t].to(dtypes[t % len(dtypes)])
         ra = ea.step(a)
         m = ra[4]["_final_observation"]
-        for name, e in (("p", ep), ("l", el_)):
-            rb = e.step(a)
-            for x, y in zip(ra[:4], rb[:4]):
-                assert torch.equal(x, y), f"kernel {name} step {t}"
-            assert torch.equal(m, rb[4]["_final_observation"])
-            assert torch.equal(ra[4]["final_observation"][m], rb[4]["final_observation"][m])
+        rb = ep.step(a)
+        for x, y in zip(ra[:4], rb[:4]):
+            assert torch.equal(x, y), f"kernel p step {t}"
+        assert torch.equal(m, rb[4]["_final_observation"])
+        assert torch.equal(ra[4]["final_observation"][m], rb[4]["final_observation"][m])
         n_done += int(m.sum())
     assert n_done >= 2 * N
-    for x, y, z in zip(ea.get_state(), ep.get_state(), el_.get_state()):
+    for x, y in zip(ea.get_state(), ep.get_state()):
         assert torch.equal(x, y), "kernel p state"
-        assert torch.equal(x, z), "kernel l state"
     for e in envs.values():
         e.close()
 

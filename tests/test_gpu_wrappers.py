@@ -50,38 +50,43 @@ def test_record_episode_statistics():
     env.close()
 
 
-def test_fused_episode_statistics_equal_the_standalone_kernel():
-    """RecordEpisodeStatistics inside the step kernel (no extra launch) vs the stand-alone launch over the returned
-    tensors (what a sharded env's gathered outputs go through): same accumulators, rows, masks and counters, for a
-    classic-control kind, a Box2D kind (their own step kernels carry the same fused bookkeeping) and float rewards."""
+def test_episode_statistics_equal_a_numpy_restatement():
+    """Every step's accumulators, episode rows, `_episode` mask and episode count against
+    record_episode_statistics.py:116-139 restated in numpy over the rewards and flags step() returned, for a
+    classic-control kind, float rewards with a short TimeLimit and a Box2D kind."""
     import gym_b200
     import torch
-    from gym_b200.wrappers import RecordEpisodeStatistics, VectorWrapper
+    from gym_b200.wrappers import RecordEpisodeStatistics
     for env_id, N, T, kw in (("CartPole-v1", 3000, 80, {}), ("Pendulum-v1", 1500, 60, dict(max_episode_steps=17)),
                              ("LunarLander-v2", 512, 140, {})):
-        fused = RecordEpisodeStatistics(gym_b200.vector.make(env_id, N, **kw), deque_size=0)
-        plain = RecordEpisodeStatistics(VectorWrapper(gym_b200.vector.make(env_id, N, **kw)), deque_size=0)
-        assert fused._fused_target() is not None and plain._fused_target() is None
-        fused.reset(seed=21)
-        plain.reset(seed=21)
+        env = RecordEpisodeStatistics(gym_b200.vector.make(env_id, N, **kw), deque_size=0)
+        env.reset(seed=21)
+        ret = np.zeros(N, np.float32)
+        length = np.zeros(N, np.int32)
+        count = 0
         gen = torch.Generator(device="cuda").manual_seed(3)
-        inner = fused.env
+        inner = env.env
         for t in range(T):
             if inner.discrete:
                 a = torch.randint(0, inner.single_action_space.n, (N,), device="cuda", generator=gen)
             else:
                 a = torch.rand((N, inner.act_dim), device="cuda", generator=gen) * 4 - 2
-            fa, fb = fused.step(a), plain.step(a)
-            assert torch.equal(fa[1], fb[1]) and torch.equal(fa[2], fb[2]) and torch.equal(fa[3], fb[3])
-            m = fa[4]["_episode"]
-            assert torch.equal(m, fb[4]["_episode"])
-            assert torch.equal(fa[4]["episode"]["r"][m], fb[4]["episode"]["r"][m])
-            assert torch.equal(fa[4]["episode"]["l"][m], fb[4]["episode"]["l"][m])
-            assert torch.equal(fused.episode_returns, plain.episode_returns)
-            assert torch.equal(fused.episode_lengths, plain.episode_lengths)
-        assert fused.episode_count == plain.episode_count > 0
-        fused.close()
-        plain.close()
+            _, rew, term, trunc, infos = env.step(a)
+            r = rew.cpu().numpy()
+            assert r.dtype == np.float64
+            done = (term | trunc).cpu().numpy()
+            ret = (ret.astype(np.float64) + r).astype(np.float32)   # float32 array += float64 rewards
+            length = length + np.int32(1)
+            assert np.array_equal(infos["_episode"].cpu().numpy(), done), t
+            assert np.array_equal(infos["episode"]["r"].cpu().numpy()[done].view(np.int32), ret[done].view(np.int32)), t
+            assert np.array_equal(infos["episode"]["l"].cpu().numpy()[done], length[done]), t
+            count += int(done.sum())
+            ret[done] = 0
+            length[done] = 0
+            assert np.array_equal(env.episode_returns.cpu().numpy().view(np.int32), ret.view(np.int32)), t
+            assert np.array_equal(env.episode_lengths.cpu().numpy(), length), t
+        assert env.episode_count == count > 0
+        env.close()
 
 
 def test_normalize_observation_and_reward():
