@@ -55,6 +55,15 @@ class HostIO(ctypes.Structure):
     ]
 
 
+# B200GYM_RMS_WORK_SIZE(dim): float64 words of the normalisers' moments work buffer
+RMS_MAX_CTAS = 1056
+NORM_WIDTHS = (1, 2, 3, 4, 6, 8, 24)
+
+
+def rms_work_size(dim):
+    return 1 + 2 * int(dim) * RMS_MAX_CTAS
+
+
 SUBENV_MAX_STAGES = 8
 SUBENV_MAX_STACK = 64
 SUBENV_MAX_ACTION_STAGES = 2
@@ -144,8 +153,8 @@ SIGNATURES = {
     "b200gym_step_p2p": (_i32, [_vp, _vp, _i32, _vp, _vp, ctypes.POINTER(_i32)]),
     "b200gym_p2p_status": (_i32, [_vp, _vp, ctypes.POINTER(_i32)]),
     "b200gym_episode_stats": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp]),
-    "b200gym_rms_moments": (_i32, [_vp, _i32, _i64, _i32, _vp, _vp, _vp]),
-    "b200gym_return_moments": (_i32, [_vp, _vp, ctypes.c_double, _i64, _vp, _vp, _vp]),
+    "b200gym_rms_moments": (_i32, [_vp, _i32, _i64, _i32, _vp, _vp, _vp, _vp]),
+    "b200gym_return_moments": (_i32, [_vp, _vp, ctypes.c_double, _i64, _vp, _vp, _vp, _vp]),
     "b200gym_rms_apply_obs": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i32, _vp]),
     "b200gym_rms_apply_reward": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
                                         _vp]),

@@ -1249,28 +1249,44 @@ __global__ void __launch_bounds__(kThreads) episode_stats_kernel(const double *r
 // two launches per step and ONE pass over the batch for the moments.
 //   launch 1 (moments): the batch is read as a flat [n*D] stream; the CTA size is a multiple of D, so every
 //     thread stays on one column and the loads are perfectly coalesced whatever D is.  Per column: sum and sum of
-//     squares of the deviations from a pivot (the current running mean: numerically tame), float64, reduced through
-//     shared-memory atomics to one global atomic per CTA and column.
+//     squares of the deviations from a pivot (the current running mean: numerically tame), float64.  The sums are
+//     reduced in a fixed order, so a launch is reproducible bit for bit: a tree over the CTA's threads of each
+//     column, one partial per CTA and column in the workspace, and the last CTA to take the ticket adds the
+//     partials in CTA order (strided over its threads, then the same tree) into scratch.  The order depends on n
+//     and D only.
 //   (between the launches a sharded env all-reduces the 2*D sums across GPUs: torch.distributed, 8 * 2 * D bytes)
 //   launch 2 (apply): every CTA folds the batch moments into the running ones (Chan et al., normalize.py:32-46) on
 //     its own -- D <= 24 columns, a few dozen flops -- normalises its share of the batch with the NEW statistics
 //     (normalize.py:83-95) and CTA 0 publishes them.  Statistics and scratch are double-buffered by step parity, so
 //     no CTA can read a half-updated value.
-// stats layout (float64, caller-owned): [2][2*D + 1] = {mean[D], var[D], count}; scratch: [2][2*D] = {sum[D], sumsq[D]}.
+// stats layout (float64, caller-owned): [2][2*D + 1] = {mean[D], var[D], count}; scratch: [2][2*D] = {sum[D], sumsq[D]};
+// work: [1 + 2*D*kNormMaxCtas] = {CTA ticket (zero bits between launches), partials[CTA][2*D]}.
 constexpr int kMaxNormDim = 24;
+constexpr int kNormMaxCtas = B200GYM_RMS_MAX_CTAS;
+constexpr int kNormMaxBlock = 256;
 
-__device__ __forceinline__ int norm_block(int D) { return (D == 3 || D == 6 || D == 24) ? 192 : 256; }
+// sh[.][c + D*j], j < blockDim.x / D (a power of two for every accepted D) -> sh[.][c], pairs at a fixed distance
+__device__ __forceinline__ void norm_tree(double (*sh)[kNormMaxBlock], int D) {
+    const int tid = threadIdx.x;
+    for (int h = blockDim.x / D / 2; h > 0; h >>= 1) {
+        if (tid < h * D) {
+            sh[0][tid] += sh[0][tid + h * D];
+            sh[1][tid] += sh[1][tid + h * D];
+        }
+        __syncthreads();
+    }
+}
 
 template <typename T, bool RETURNS>
-__global__ void rms_moments_kernel(const T *x, double *returns, const double *reward, double gamma, int64_t total, int D,
-                                   const double *stats, double *scratch) {
-    __shared__ double sh[2][kMaxNormDim];
+__global__ void __launch_bounds__(kNormMaxBlock) rms_moments_kernel(const T *x, double *returns, const double *reward,
+                                                                    double gamma, int64_t total, int D,
+                                                                    const double *stats, double *scratch, double *work) {
+    __shared__ double sh[2][kNormMaxBlock];
+    __shared__ bool last;
     const int tid = threadIdx.x;
-    if (tid < D) { sh[0][tid] = 0.0; sh[1][tid] = 0.0; }
-    __syncthreads();
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;      // a multiple of D: the column of a thread is fixed
     const int64_t start = (int64_t)blockIdx.x * blockDim.x + tid;
-    const int col = (int)(start % D);
+    const int col = tid % D;                                     // = start % D: blockDim.x is a multiple of D
     const double pivot = stats[col];
     double s = 0.0, q = 0.0;
     for (int64_t k = start; k < total; k += stride) {
@@ -1285,13 +1301,38 @@ __global__ void rms_moments_kernel(const T *x, double *returns, const double *re
         s += v;
         q += v * v;
     }
-    atomicAdd(&sh[0][col], s);
-    atomicAdd(&sh[1][col], q);
+    sh[0][tid] = s;
+    sh[1][tid] = q;
     __syncthreads();
+    norm_tree(sh, D);
+    unsigned int *ticket = reinterpret_cast<unsigned int *>(work);
+    double *partials = work + 1;
     if (tid < D) {
-        atomicAdd(&scratch[tid], sh[0][tid]);
-        atomicAdd(&scratch[D + tid], sh[1][tid]);
+        partials[(int64_t)blockIdx.x * 2 * D + tid] = sh[0][tid];
+        partials[(int64_t)blockIdx.x * 2 * D + D + tid] = sh[1][tid];
+        __threadfence();                                         // the partials are visible before the ticket is taken
     }
+    __syncthreads();
+    if (tid == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    // the last CTA: thread tid adds the partials of CTAs tid / D, tid / D + m, ... in order (m = blockDim.x / D)
+    s = 0.0;
+    q = 0.0;
+    for (int b = tid / D; b < (int)gridDim.x; b += blockDim.x / D) {
+        s += __ldcg(&partials[(int64_t)b * 2 * D + col]);
+        q += __ldcg(&partials[(int64_t)b * 2 * D + D + col]);
+    }
+    sh[0][tid] = s;
+    sh[1][tid] = q;
+    __syncthreads();
+    norm_tree(sh, D);
+    if (tid < D) {
+        scratch[tid] += sh[0][tid];
+        scratch[D + tid] += sh[1][tid];
+    }
+    if (tid == 0) *ticket = 0u;                                  // ready for the next launch (stream order)
 }
 
 // update_mean_var_count_from_moments (normalize.py:32-46) for column d, from the pivoted batch sums
@@ -2180,13 +2221,13 @@ static int norm_dims_ok(int dim) { return dim == 1 || dim == 2 || dim == 3 || di
 
 static unsigned norm_grid(int64_t total, int block) {
     int64_t g = (total + block - 1) / block;
-    if (g > 1056) g = 1056;       // 132 SMs x 8: one resident wave, grid-stride beyond
+    if (g > kNormMaxCtas) g = kNormMaxCtas;       // 132 SMs x 8: one resident wave, grid-stride beyond
     return (unsigned)(g < 1 ? 1 : g);
 }
 
 extern "C" int b200gym_rms_moments(const void *x_dev, int is_f64, int64_t n, int dim, const double *stats_dev,
-                                   double *scratch_dev, void *stream) {
-    if (!x_dev || !stats_dev || !scratch_dev || n <= 0 || !norm_dims_ok(dim))
+                                   double *scratch_dev, double *work_dev, void *stream) {
+    if (!x_dev || !stats_dev || !scratch_dev || !work_dev || n <= 0 || !norm_dims_ok(dim))
         return fail(nullptr, "b200gym_rms_moments: bad argument (dim must be one of 1, 2, 3, 4, 6, 8, 24)");
     const int dev = device_of(x_dev);
     if (dev < 0) return fail(nullptr, "b200gym_rms_moments: x is not a device pointer");
@@ -2195,24 +2236,24 @@ extern "C" int b200gym_rms_moments(const void *x_dev, int is_f64, int64_t n, int
     const int64_t total = n * dim;
     cudaStream_t st = (cudaStream_t)stream;
     if (is_f64)
-        rms_moments_kernel<double, false><<<norm_grid(total, block), block, 0, st>>>((const double *)x_dev, nullptr, nullptr,
-                                                                                   0.0, total, dim, stats_dev, scratch_dev);
+        rms_moments_kernel<double, false><<<norm_grid(total, block), block, 0, st>>>(
+            (const double *)x_dev, nullptr, nullptr, 0.0, total, dim, stats_dev, scratch_dev, work_dev);
     else
-        rms_moments_kernel<float, false><<<norm_grid(total, block), block, 0, st>>>((const float *)x_dev, nullptr, nullptr,
-                                                                                  0.0, total, dim, stats_dev, scratch_dev);
+        rms_moments_kernel<float, false><<<norm_grid(total, block), block, 0, st>>>(
+            (const float *)x_dev, nullptr, nullptr, 0.0, total, dim, stats_dev, scratch_dev, work_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
 }
 
 extern "C" int b200gym_return_moments(double *returns_dev, const double *reward_dev, double gamma, int64_t n,
-                                      const double *stats_dev, double *scratch_dev, void *stream) {
-    if (!returns_dev || !reward_dev || !stats_dev || !scratch_dev || n <= 0)
+                                      const double *stats_dev, double *scratch_dev, double *work_dev, void *stream) {
+    if (!returns_dev || !reward_dev || !stats_dev || !scratch_dev || !work_dev || n <= 0)
         return fail(nullptr, "b200gym_return_moments: bad argument");
     const int dev = device_of(returns_dev);
     if (dev < 0) return fail(nullptr, "b200gym_return_moments: returns is not a device pointer");
     DeviceGuard guard(dev);
-    rms_moments_kernel<double, true><<<norm_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(nullptr, returns_dev, reward_dev, gamma,
-                                                                                         n, 1, stats_dev, scratch_dev);
+    rms_moments_kernel<double, true><<<norm_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(
+        nullptr, returns_dev, reward_dev, gamma, n, 1, stats_dev, scratch_dev, work_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
 }
@@ -2222,7 +2263,7 @@ extern "C" int b200gym_rms_apply_obs(const float *obs_dev, float *out_dev, int64
                                      double batch_count, double epsilon, int update, void *stream) {
     if (!obs_dev || !out_dev || !stats_dev || !stats_next_dev || !scratch_dev || !scratch_next_dev || n <= 0 ||
         !norm_dims_ok(dim))
-        return fail(nullptr, "b200gym_rms_apply_obs: bad argument");
+        return fail(nullptr, "b200gym_rms_apply_obs: bad argument (dim must be one of 1, 2, 3, 4, 6, 8, 24)");
     const int dev = device_of(obs_dev);
     if (dev < 0) return fail(nullptr, "b200gym_rms_apply_obs: obs is not a device pointer");
     DeviceGuard guard(dev);

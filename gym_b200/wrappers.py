@@ -230,7 +230,8 @@ class _RunningMeanStd:
     """Device copy of RunningMeanStd's state (normalize.py:8-29): mean 0, var 1, count epsilon.
 
     ``stats[2][2*d + 1]`` = {mean, var, count} and ``scratch[2][2*d]`` = this step's batch sums, both
-    double-buffered by step parity (include/b200gym.h); ``cur`` is the set holding the current statistics."""
+    double-buffered by step parity (include/b200gym.h); ``cur`` is the set holding the current statistics.
+    ``work`` holds the moments launch's per-CTA partial sums (zero between launches, not part of the state)."""
 
     def __init__(self, torch, d, device, epsilon=1e-4):
         self.d = int(d)
@@ -238,6 +239,7 @@ class _RunningMeanStd:
         self.stats[:, self.d:2 * self.d] = 1.0
         self.stats[:, 2 * self.d] = epsilon
         self.scratch = torch.zeros((2, 2 * self.d), dtype=torch.float64, device=device)
+        self.work = torch.zeros(_lib.rms_work_size(self.d), dtype=torch.float64, device=device)
         self.cur = 0
 
     @property
@@ -254,20 +256,31 @@ class _RunningMeanStd:
 
 
 def _shard_group(env, group):
-    """(process group, world size) when the batch statistics must be combined across GPUs: the wrapped env is this
-    rank's shard of a global batch (``first_index``/``ShardedVectorEnv(gather=None)``) and torch.distributed is up."""
+    """The process group when the batch statistics must be combined across GPUs (None otherwise): the wrapped env is
+    this rank's shard of a global batch (``first_index``/``ShardedVectorEnv(gather=None)``) and torch.distributed is
+    up."""
     if group is False:
-        return None, 1
+        return None
     try:
         import torch.distributed as dist
     except Exception:
-        return None, 1
+        return None
     if not (dist.is_available() and dist.is_initialized()):
-        return None, 1
+        return None
     if group is None and not getattr(env, "shards_global_batch", False):
-        return None, 1
-    g = None if group in (None, True) else group
-    return (g if g is not None else dist.group.WORLD), dist.get_world_size(g)
+        return None
+    return dist.group.WORLD if group in (None, True) else group
+
+
+def _batch_count(torch, env, group):
+    """Rows of the global batch: this shard's rows summed over the group (shards may differ in size)."""
+    n = env.num_envs
+    if group is None:
+        return float(n)
+    import torch.distributed as dist
+    t = torch.tensor([n], dtype=torch.float64, device=env.unwrapped.device)
+    dist.all_reduce(t, group=group)
+    return float(t.item())
 
 
 class NormalizeObservation(VectorWrapper):
@@ -275,7 +288,12 @@ class NormalizeObservation(VectorWrapper):
 
     ``group``: a torch.distributed process group (or True for the default one) when ``env`` is ONE RANK'S SHARD of
     a global batch: the per-column batch sums are all-reduced over the group before the running statistics are
-    updated (normalize.py:32-46 applied to the global batch), so every rank normalises with the same numbers."""
+    updated (normalize.py:32-46 applied to the global batch), so every rank normalises with the same numbers; the
+    batch count is the shards' env counts summed over the group, so the shards may differ in size.
+
+    Rows must have 1, 2, 3, 4, 6, 8 or 24 elements (``ValueError`` otherwise).  The batch moments are float64 sums
+    in a fixed order (the same batch gives the same statistics bit for bit); the reference's are float32 ``np.mean``
+    / ``np.var`` of float32 observations, and its outputs float64 where these are float32 (DESIGN.md §4.9)."""
 
     def __init__(self, env, epsilon=1e-8, group=None):
         super().__init__(env)
@@ -284,10 +302,14 @@ class NormalizeObservation(VectorWrapper):
         self.num_envs, self.is_vector_env = env.num_envs, True
         self.epsilon = float(epsilon)
         d = int(np.prod(env.single_observation_space.shape))   # statistics per element of the flattened row
+        if d not in _lib.NORM_WIDTHS:
+            raise ValueError(f"NormalizeObservation: observation rows of {d} elements; the device kernels take "
+                             f"{', '.join(map(str, _lib.NORM_WIDTHS))}")
         self.obs_rms = _RunningMeanStd(torch, d, env.unwrapped.device)
         self._out = [None, None]
         self._flip = 0
-        self._group, self._world = _shard_group(env, group)
+        self._group = _shard_group(env, group)
+        self._count = _batch_count(torch, env, self._group)
 
     def _normalize(self, obs, update=True):
         torch = self._torch
@@ -302,12 +324,12 @@ class NormalizeObservation(VectorWrapper):
         st, sc = r.stats[r.cur], r.scratch[r.cur]
         with torch.cuda.device(obs.device):
             if update:
-                _lib.check(lib.b200gym_rms_moments(_p(obs), 0, n, d, _p(st), _p(sc), env._stream()))
+                _lib.check(lib.b200gym_rms_moments(_p(obs), 0, n, d, _p(st), _p(sc), _p(r.work), env._stream()))
                 if self._group is not None:
                     import torch.distributed as dist
                     dist.all_reduce(sc, group=self._group)
             _lib.check(lib.b200gym_rms_apply_obs(_p(obs), _p(out), n, d, _p(st), _p(r.stats[r.cur ^ 1]), _p(sc),
-                                                 _p(r.scratch[r.cur ^ 1]), float(n * self._world), self.epsilon,
+                                                 _p(r.scratch[r.cur ^ 1]), self._count, self.epsilon,
                                                  1 if update else 0, env._stream()))
         if update:
             r.cur ^= 1
@@ -352,7 +374,8 @@ class NormalizeReward(VectorWrapper):
         self.returns = None
         self._out = [None, None]
         self._flip = 0
-        self._group, self._world = _shard_group(env, group)
+        self._group = _shard_group(env, group)
+        self._count = _batch_count(torch, env, self._group)
 
     def reset(self, **kwargs):
         refuse_capture("NormalizeReward.reset()", _NORM_NO_CAPTURE)
@@ -373,13 +396,14 @@ class NormalizeReward(VectorWrapper):
         n = rew.shape[0]
         st, sc = r.stats[r.cur], r.scratch[r.cur]
         with torch.cuda.device(rew.device):
-            _lib.check(lib.b200gym_return_moments(_p(self.returns), _p(rew), self.gamma, n, _p(st), _p(sc), env._stream()))
+            _lib.check(lib.b200gym_return_moments(_p(self.returns), _p(rew), self.gamma, n, _p(st), _p(sc), _p(r.work),
+                                                  env._stream()))
             if self._group is not None:
                 import torch.distributed as dist
                 dist.all_reduce(sc, group=self._group)
             _lib.check(lib.b200gym_rms_apply_reward(_p(rew), _p(out), _p(self.returns), _p(term), _p(trunc), n, _p(st),
                                                     _p(r.stats[r.cur ^ 1]), _p(sc), _p(r.scratch[r.cur ^ 1]),
-                                                    float(n * self._world), self.epsilon, env._stream()))
+                                                    self._count, self.epsilon, env._stream()))
         r.cur ^= 1
         return obs, out, term, trunc, infos
 

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200GYM_VERSION 3
+#define B200GYM_VERSION 4
 
 /* Environment kinds: the dynamics classes on the hot path. */
 enum b200gym_kind {
@@ -334,6 +334,9 @@ int b200gym_episode_stats(const double *reward_dev, const uint8_t *terminated_de
  *           writes set `cur ^ 1` (initialise set 0 to mean 0, var 1, count 1e-4: normalize.py:11-15)
  *   scratch float64 [2][2*dim]     = per-column sums of (x - mean) and (x - mean)^2 of THIS step's batch,
  *           accumulated into set `cur` (zero on first use; the apply launch clears the other set)
+ *   work    float64 [B200GYM_RMS_WORK_SIZE(dim)] = the moments launch's per-CTA partial sums and CTA ticket; zero
+ *           before first use, left ready for the next launch; one per stream of moments launches
+ * The sums are added in an order that depends on n and dim only: the same inputs give the same bits every launch.
  * b200gym_rms_moments      one coalesced pass over x [n][dim] (float32, or float64 with is_f64): sums into scratch
  * b200gym_return_moments   NormalizeReward.step's `returns = returns * gamma + reward` (normalize.py:130) fused
  *                          with the same pass over `returns`
@@ -344,10 +347,12 @@ int b200gym_episode_stats(const double *reward_dev, const uint8_t *terminated_de
  *                          returns[terminated | truncated] = 0 (:135-136)
  * dim must be one of 1, 2, 3, 4, 6, 8, 24 (the observation sizes of the in-scope envs).
  */
+#define B200GYM_RMS_MAX_CTAS 1056
+#define B200GYM_RMS_WORK_SIZE(dim) (1 + 2 * (dim) * B200GYM_RMS_MAX_CTAS)
 int b200gym_rms_moments(const void *x_dev, int is_f64, int64_t n, int dim, const double *stats_dev, double *scratch_dev,
-                        void *stream);
+                        double *work_dev, void *stream);
 int b200gym_return_moments(double *returns_dev, const double *reward_dev, double gamma, int64_t n, const double *stats_dev,
-                           double *scratch_dev, void *stream);
+                           double *scratch_dev, double *work_dev, void *stream);
 int b200gym_rms_apply_obs(const float *obs_dev, float *out_dev, int64_t n, int dim, const double *stats_dev,
                           double *stats_next_dev, const double *scratch_dev, double *scratch_next_dev, double batch_count,
                           double epsilon, int update, void *stream);

@@ -31,9 +31,9 @@ def test_library_builds_and_exports_every_declared_symbol():
     assert sorted(_lib.SIGNATURES) == declared
 
 
-def test_abi_version_and_shape_queries_need_no_device():
+def test_abi_version_4_and_shape_queries_need_no_device():
     lib = _lib.load()
-    assert lib.b200gym_version() == 3   # 3: b200gym_set_episode_stats removed
+    assert lib.b200gym_version() == 4   # 4: the moments launches take a work buffer (fixed-order sums)
     assert [lib.b200gym_obs_dim(k) for k in range(9)] == [4, 2, 2, 3, 6, 8, 24, 8, 24]
     assert [lib.b200gym_act_dim(k) for k in range(9)] == [0, 0, 1, 1, 0, 0, 4, 2, 4]
     assert [lib.b200gym_num_actions(k) for k in range(9)] == [2, 3, 0, 0, 3, 4, 0, 0, 0]
