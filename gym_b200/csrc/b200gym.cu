@@ -297,6 +297,16 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel(
         reset_env<KIND>(a, DirectSink{a}, a.first + (int64_t)blockIdx.x * blockDim.x + reset_list[threadIdx.x]);
 }
 
+// --- rollout kernel: T steps per launch, one thread per environment ---------------------------------------------
+// Thread i runs env i's T steps with the state and TimeLimit counter in registers (rollout_env); at every step a warp
+// reads one coalesced action row and writes coalesced output rows of slice t.  A finishing env is reset inline, by
+// its own lane, before its next step: the step kernels' deferred reset list does not apply
+template <int KIND, typename ActT>
+__global__ void __launch_bounds__(kThreads) rollout_kernel(const StepArgs a, const int32_t T, float *last_obs) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.n) rollout_env<KIND, ActT>(a, i, T, last_obs);
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -1661,6 +1671,61 @@ static int launch_step(b200gym *h, const StepArgs &a, int action_dtype, cudaStre
 }
 
 template <int KIND>
+static int launch_rollout_kind(b200gym *h, const StepArgs &a, int action_dtype, int32_t T, float *last_obs,
+                               cudaStream_t st) {
+    if constexpr (Env<KIND>::A == 0) {
+        switch (action_dtype) {
+        case B200GYM_ACT_I64: rollout_kernel<KIND, long long><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs); break;
+        case B200GYM_ACT_I32: rollout_kernel<KIND, int><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs); break;
+        case B200GYM_ACT_U8: rollout_kernel<KIND, unsigned char><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs); break;
+        default: return fail(h, "Discrete env needs an integer action dtype (got code %d)", action_dtype);
+        }
+    } else {
+        if (action_dtype != B200GYM_ACT_F32) return fail(h, "Box env needs float32 actions (got dtype code %d)", action_dtype);
+        rollout_kernel<KIND, float><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs);
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+static size_t action_size(int action_dtype);
+
+// A Box2D rollout: the step sequence of launch_step_box2d once per step, into slice t; those steps are bound by
+// their arithmetic (milliseconds at 2^16 envs), so keeping the state on chip would save nothing measurable
+static int launch_rollout_box2d(b200gym *h, const StepArgs &a, int action_dtype, int32_t T, float *last_obs,
+                                cudaStream_t st) {
+    const int64_t n = h->n, D = h->D;
+    const size_t act_row = (size_t)n * std::max(h->A, 1) * action_size(action_dtype);
+    StepArgs s = a;
+    for (int32_t t = 0; t < T; t++) {
+        s.actions = static_cast<const unsigned char *>(a.actions) + (size_t)t * act_row;
+        s.obs = a.obs + t * n * D;
+        s.reward = a.reward + t * n;
+        s.terminated = a.terminated + t * n;
+        s.truncated = a.truncated + t * n;
+        s.final_obs = a.final_obs ? a.final_obs + t * n * D : nullptr;
+        if (launch_step_box2d(h, s, action_dtype, st)) return 1;
+    }
+    CK(h, cudaMemcpyAsync(last_obs, s.obs, (size_t)n * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+static int launch_rollout(b200gym *h, const StepArgs &a, int action_dtype, int32_t T, float *last_obs, cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_kind<B200GYM_CARTPOLE>(h, a, action_dtype, T, last_obs, st);
+    case B200GYM_MOUNTAINCAR: return launch_rollout_kind<B200GYM_MOUNTAINCAR>(h, a, action_dtype, T, last_obs, st);
+    case B200GYM_MOUNTAINCAR_CONT: return launch_rollout_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, action_dtype, T, last_obs, st);
+    case B200GYM_PENDULUM: return launch_rollout_kind<B200GYM_PENDULUM>(h, a, action_dtype, T, last_obs, st);
+    case B200GYM_ACROBOT: return launch_rollout_kind<B200GYM_ACROBOT>(h, a, action_dtype, T, last_obs, st);
+    case B200GYM_LUNARLANDER:
+    case B200GYM_LUNARLANDER_CONT:
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE: return launch_rollout_box2d(h, a, action_dtype, T, last_obs, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+template <int KIND>
 static void launch_reset_kind(b200gym *h, const uint8_t *mask, const double *bounds, float *obs, cudaStream_t st) {
     double lo, hi;
     Env<KIND>::default_bounds(lo, hi);
@@ -1987,6 +2052,18 @@ extern "C" int b200gym_step(b200gym_t *h, const void *actions_dev, int action_dt
     DeviceGuard guard(h->device);
     const StepArgs a = make_args(h, actions_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
     return launch_step(h, a, action_dtype, (cudaStream_t)stream);
+}
+
+extern "C" int b200gym_rollout(b200gym_t *h, const void *actions_dev, int action_dtype, int32_t T, float *obs_dev,
+                               double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                               float *last_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout: null handle");
+    if (T < 1) return fail(h, "b200gym_rollout: T must be at least 1 (got %d)", T);
+    if (!actions_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || !last_obs_dev)
+        return fail(h, "b200gym_rollout: null buffer");
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    return launch_rollout(h, a, action_dtype, T, last_obs_dev, (cudaStream_t)stream);
 }
 
 extern "C" int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out) {

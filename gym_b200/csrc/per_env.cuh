@@ -220,6 +220,98 @@ __device__ __forceinline__ void reset_env(const StepArgs &a, const Sink &sink, I
     sink.template obs<E::D>(i, obs);
 }
 
+// ---- rollouts (b200gym_rollout) ---------------------------------------------------------------------------------
+
+// A store the rollout's outputs make once and never read back: evict-first on the device, where T steps of outputs
+// are far larger than L2; a plain store in the host build
+template <typename T>
+__device__ __forceinline__ void store_once(T *p, T v) {
+#ifdef __CUDA_ARCH__
+    __stcs(p, v);
+#else
+    *p = v;
+#endif
+}
+
+// The sink of one rollout step: the state and TimeLimit counter go to the thread's registers, the outputs to the rows
+// of slice t (the pointers are advanced by one slice per step), and on the last step the observation also to `last`,
+// the handle's own observation buffer
+template <int KIND>
+struct RolloutSink {
+    double (&s)[bgym::Env<KIND>::S];
+    int32_t &el;
+    float *o;
+    double *r;
+    uint8_t *te, *tr;
+    float *fin;    // null: no final observations
+    float *last;   // null but on the last step
+    template <int D, typename I>
+    __device__ __forceinline__ void obs_row(float *base, I i, const float (&v)[D]) const {
+        if constexpr (D == 4) {
+            store_once(reinterpret_cast<float4 *>(base) + i, make_float4(v[0], v[1], v[2], v[3]));
+        } else if constexpr (D == 2) {
+            store_once(reinterpret_cast<float2 *>(base) + i, make_float2(v[0], v[1]));
+        } else {
+#pragma unroll
+            for (int k = 0; k < D; k++) store_once(base + i * D + k, v[k]);
+        }
+    }
+    template <int D, typename I>
+    __device__ __forceinline__ void obs(I i, const float (&v)[D]) const {
+        obs_row<D>(o, i, v);
+        if (last) store_row<D>(last, i, v);
+    }
+    template <typename I>
+    __device__ __forceinline__ void scalars(I i, double reward, uint8_t term, uint8_t trunc) const {
+        store_once(r + i, reward);
+        store_once(te + i, term);
+        store_once(tr + i, trunc);
+    }
+    template <int S, typename I>
+    __device__ __forceinline__ void state(I, const double (&v)[S]) const {
+#pragma unroll
+        for (int k = 0; k < S; k++) s[k] = v[k];
+    }
+    template <typename I>
+    __device__ __forceinline__ void elapsed(I, int32_t e) const { el = e; }
+    template <int D, typename I>
+    __device__ __forceinline__ void final_obs(I i, const float (&v)[D]) const {
+        if (fin) obs_row<D>(fin, i, v);
+    }
+};
+
+// T steps of env i (rollout_kernel), the same as T launches of kernel A: advance_env and, when the episode ended,
+// reset_env, with the state and TimeLimit counter loaded once and stored once.  a.actions, a.obs, a.reward,
+// a.terminated, a.truncated and a.final_obs hold slice 0 of [T][n] arrays; CartPole's autoreset=False flag byte stays
+// in global memory, where advance_env keeps it
+template <int KIND, typename ActT>
+__device__ __forceinline__ void rollout_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs) {
+    using E = bgym::Env<KIND>;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    RolloutSink<KIND> sink{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr};
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(__ldg(act + i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.o += n * E::D;
+        sink.r += n;
+        sink.te += n;
+        sink.tr += n;
+        if (sink.fin) sink.fin += n * E::D;
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the
 // observation row.  References as in lunar_reset_env.
 template <int KIND>

@@ -420,11 +420,13 @@ class B200VectorEnv:
                            "an env with backend='torch'")
 
     # ------------------------------------------------------------------ step
-    def _device_actions(self, actions, captured=False):
-        """Bring `actions` to a contiguous device tensor of a dtype the kernel reads directly."""
+    def _device_actions(self, actions, captured=False, steps=False):
+        """Bring `actions` to a contiguous device tensor of a dtype the kernel reads directly.  steps=True: a leading
+        time axis of length >= 1, with the shape checked exactly (rollout)."""
         torch = _torch()
+        what = "rollout()" if steps else "step()"
         if captured and not (isinstance(actions, torch.Tensor) and actions.device == self.device):
-            raise error.Error(f"step() cannot be captured in a CUDA graph with actions that are not a CUDA tensor on "
+            raise error.Error(f"{what} cannot be captured in a CUDA graph with actions that are not a CUDA tensor on "
                               f"{self.device}: the host-to-device copy cannot be replayed (got "
                               f"{type(actions).__name__}{' on ' + str(actions.device) if hasattr(actions, 'device') else ''})")
         if not isinstance(actions, torch.Tensor):
@@ -446,7 +448,12 @@ class B200VectorEnv:
                 actions = actions.to(torch.float32)  # the Box dtype (e.g. pendulum.py:113-115)
             code = _lib.ACT_F32
             shape = (self.num_envs, self.act_dim)
-        if actions.numel() != int(np.prod(shape)):
+        if steps:
+            if actions.dim() != len(shape) + 1 or tuple(actions.shape[1:]) != shape or actions.shape[0] < 1:
+                raise error.InvalidAction(f"expected actions of shape (T, {', '.join(map(str, shape))}) with T >= 1, "
+                                          f"got {tuple(actions.shape)}")
+            shape = (actions.shape[0],) + shape
+        elif actions.numel() != int(np.prod(shape)):
             raise error.InvalidAction(f"expected actions of shape {shape}, got {tuple(actions.shape)}")
         if actions.device != self.device:
             actions = actions.to(self.device, non_blocking=True)
@@ -582,6 +589,50 @@ class B200VectorEnv:
         """One SyncVectorEnv.step: (obs, rewards, terminateds, truncateds, infos)."""
         self.step_async(actions)
         return self.step_wait()
+
+    def rollout(self, actions):
+        """T steps with actions known in advance -> ``(obs, rewards, terminateds, truncateds, infos)``, each with a
+        leading T axis: what ``[self.step(a) for a in actions]`` returns, stacked, bit for bit, and the env left as those
+        calls leave it.  ``actions``: (T, N) integers (Discrete) or (T, N, A) float32 (Box).  The outputs are new
+        tensors that belong to the caller; ``infos["final_observation"]`` is (T, N, D), valid where
+        ``infos["_final_observation"]`` (T, N) is set.  The classic-control kinds run the T steps in one launch with
+        each env's state in registers (DESIGN.md §4.10).  May be captured in a CUDA graph."""
+        self._assert_open("rollout")
+        if self.backend == "numpy":
+            raise error.Error("rollout() needs backend='torch': backend='numpy' steps through host buffers")
+        if self._chain is not None:
+            raise error.Error("rollout() cannot run per-env wrappers (wrappers=): the chain runs after every step, "
+                              "and the fused rollout kernel has no step boundary to run it at")
+        if self._state != _STATE_DEFAULT:
+            raise error.AlreadyPendingCallError(
+                f"Calling `rollout` while waiting for a pending call to `{self._state}` to complete.", self._state)
+        if not self._has_reset:
+            raise error.ResetNeeded("Cannot call env.rollout() before calling env.reset()")
+        torch = _torch()
+        captured = capturing()
+        # the same poll as step_async: an invalid action of an earlier call raises here (not while capturing)
+        if self.discrete and not captured and self._lib.b200gym_invalid_seen(self._handle) == 1:
+            self.check_actions()
+        self._raise_snapshot_index_error()
+        act, code = self._device_actions(actions, captured, steps=True)
+        T, n, dev = int(act.shape[0]), self.num_envs, self.device
+        shape = (T, n) + self._obs_shape
+        obs = torch.empty(shape, dtype=torch.float32, device=dev)
+        reward = torch.empty((T, n), dtype=torch.float64, device=dev)
+        term = torch.empty((T, n), dtype=torch.bool, device=dev)
+        trunc = torch.empty((T, n), dtype=torch.bool, device=dev)
+        # without autoreset step() hands out a final_observation buffer that nothing writes
+        final_obs = (torch.empty if self.autoreset else torch.zeros)(shape, dtype=torch.float32, device=dev)
+        # the last observations also go to the next set of the double buffer, where snapshot() / clone() read them
+        self._flip ^= 1
+        last = self._out[self._flip]["obs"]
+        _lib.check(self._lib.b200gym_rollout(
+            self._handle, ctypes.c_void_p(act.data_ptr()), code, T, ctypes.c_void_p(obs.data_ptr()),
+            ctypes.c_void_p(reward.data_ptr()), ctypes.c_void_p(term.data_ptr()), ctypes.c_void_p(trunc.data_ptr()),
+            ctypes.c_void_p(final_obs.data_ptr()) if self.autoreset else None, ctypes.c_void_p(last.data_ptr()),
+            self._stream()), self._handle)
+        self._last_actions = act  # keep alive until the kernel has consumed it
+        return obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
 
     def check_actions(self):
         """Number of out-of-range Discrete actions the device saw since the last check (syncs)."""

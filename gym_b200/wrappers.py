@@ -49,6 +49,13 @@ class VectorWrapper:
     def step(self, actions):
         return self.env.step(actions)
 
+    def rollout(self, actions):
+        """Refused: a wrapper acts after every step, which a fused rollout of the env it wraps would skip (the
+        statistics would not be recorded, the observations not normalised).  Step the wrapper instead."""
+        from gym_b200 import error
+        raise error.Error(f"{type(self).__name__} does not support rollout(): it acts after every step, and a fused "
+                          "rollout of the wrapped env would skip it; call step() T times instead")
+
     def close(self, **kwargs):
         return self.env.close(**kwargs)
 

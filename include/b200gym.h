@@ -154,6 +154,28 @@ int b200gym_step(b200gym_t *h, const void *actions_dev, int action_dtype, float 
                  double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
                  float *final_obs_dev, void *stream);
 
+/*
+ * T consecutive b200gym_step calls with actions known in advance (random-action data collection, planning from
+ * cloned states, replaying recorded episodes): SyncVectorEnv.step_wait (gym/vector/sync_vector_env.py:135-169) T
+ * times, with every slice bit for bit what the t-th b200gym_step writes and the handle left in the state those T calls
+ * leave it in (state, TimeLimit counters, CartPole flags, PCG64 records).
+ *   actions_dev    [T][n] integers of `action_dtype`, or [T][n][act_dim] float32
+ *   T              >= 1
+ *   obs_dev        [T][n][obs_dim] float32   post-autoreset observations
+ *   reward_dev     [T][n] float64
+ *   terminated_dev, truncated_dev [T][n] uint8 (0/1)
+ *   final_obs_dev  [T][n][obs_dim] float32 or NULL: rows written only where terminated|truncated and cfg.autoreset
+ *   last_obs_dev   [n][obs_dim] float32: also receives slice T-1 of obs_dev (the caller's "last observation" buffer)
+ * Classic-control kinds: ONE launch, one thread per env, the state and TimeLimit counter loaded once and stored once,
+ * a finishing env reset inline before its next step.  Box2D kinds: the b200gym_step sequence once per step.
+ * Out-of-range Discrete actions are handled per step as b200gym_step handles them: that env is left untouched for
+ * that step (NaN reward, current observation), counted by b200gym_invalid_actions(), and carries on with the next
+ * row.  Offsets into the [T][n] arrays are 64-bit.
+ */
+int b200gym_rollout(b200gym_t *h, const void *actions_dev, int action_dtype, int32_t T, float *obs_dev,
+                    double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                    float *last_obs_dev, void *stream);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
