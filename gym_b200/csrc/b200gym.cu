@@ -307,6 +307,28 @@ __global__ void __launch_bounds__(kThreads) rollout_kernel(const StepArgs a, con
     if (i < a.n) rollout_env<KIND, ActT>(a, i, T, last_obs);
 }
 
+// ... with the actions drawn from the action space's stream as the kernel goes (rollout_sampled_env): the stream
+// comes from the record (or the override) and the last CTA to take a ticket writes it back T * n draws later, as in
+// space_sample_stream_kernel
+template <int KIND>
+__global__ void __launch_bounds__(kThreads) rollout_sampled_kernel(const StepArgs a, const int32_t T, float *last_obs,
+                                                                   const RolloutDraws d, const SampleStream s) {
+    __shared__ LcgJumpTable table;   // rows [0, jump_digits) of kLcgJump
+    __shared__ Pcg64 start;
+    const uint4 *src = reinterpret_cast<const uint4 *>(&kLcgJump);
+    uint4 *dst = reinterpret_cast<uint4 *>(&table);
+    for (int k = threadIdx.x; k < d.jump_digits * 32; k += kThreads) dst[k] = src[k];
+    if (threadIdx.x == 0) start = sample_stream_start(s);
+    __syncthreads();
+    const Pcg64 g = start;
+    // this CTA's read of the record has returned, so the last CTA to take a ticket writes after every read
+    unsigned long long ticket = 0;
+    if (threadIdx.x == 0) ticket = atomicAdd(reinterpret_cast<unsigned long long *>(s.record + 4), 1ULL);
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.n) rollout_sampled_env<KIND>(a, i, T, last_obs, d, g, table);
+    if (threadIdx.x == 0 && ticket == gridDim.x - 1ULL) sample_stream_finish(s, g);
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -2444,6 +2466,71 @@ extern "C" int b200gym_sample_space_stream(uint64_t *record_dev, const uint64_t 
         space_sample_stream_kernel<float><<<(unsigned)blocks, kSampleThreads, 0, st>>>(a, s, (float *)out_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
+}
+
+// ---- rollouts of random actions (b200gym_rollout_sampled) ----
+template <int KIND>
+static int launch_rollout_sampled_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const RolloutDraws &d,
+                                       const SampleStream &s, cudaStream_t st) {
+    rollout_sampled_kernel<KIND><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs, d, s);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_rollout_sampled(b200gym_t *h, uint64_t *record_dev, const uint64_t override_pcg64[4],
+                                       int64_t n_choices, const double *low_host, const double *high_host, int32_t T,
+                                       void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                       uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                       float *last_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout_sampled: null handle");
+    if (T < 1) return fail(h, "b200gym_rollout_sampled: T must be at least 1 (got %d)", T);
+    if (!record_dev || !actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || !last_obs_dev)
+        return fail(h, "b200gym_rollout_sampled: null buffer");
+    if ((uintptr_t)record_dev % 16)
+        return fail(h, "b200gym_rollout_sampled: the record must be a 16-byte aligned device buffer");
+    if ((n_choices > 0) != (h->A == 0))
+        return fail(h, "b200gym_rollout_sampled: %s", h->A == 0 ? "a Discrete env needs n_choices >= 1"
+                                                                : "a Box env needs n_choices = 0 and its bounds");
+    const int cols = std::max(h->A, 1);
+    const int64_t draws_n = (int64_t)T * h->n;   // rows of the [T][n][cols] action output
+    SampleArgs sa;
+    int dev;
+    if (sample_prepare("b200gym_rollout_sampled", draws_n, cols, n_choices, low_host, high_host, actions_out_dev, sa,
+                       dev))
+        return fail(h, "%s", b200gym_last_error(nullptr));
+    if (dev != h->device || device_of(record_dev) != h->device)
+        return fail(h, "b200gym_rollout_sampled: the record and the action output must be on the handle's device %d",
+                    h->device);
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (h->is_lunar || h->is_walker) {
+        // T consecutive sample() calls are T * n * cols consecutive draws in C order, which is the [T][n][cols] layout:
+        // one sampling launch fills every slice, then the Box2D rollout steps through them
+        if (b200gym_sample_space_stream(record_dev, override_pcg64, draws_n, cols, n_choices, low_host, high_host,
+                                        actions_out_dev, stream))
+            return fail(h, "%s", b200gym_last_error(nullptr));
+        return launch_rollout_box2d(h, a, h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32, T, last_obs_dev, st);
+    }
+    SampleStream s{};
+    s.record = record_dev;
+    if (override_pcg64) {
+        s.use_override = 1;
+        for (int k = 0; k < 4; k++) s.override_words[k] = override_pcg64[k];
+    }
+    s.advance = lcg_jump_map((u128)sa.total);
+    const LcgMap hop = lcg_jump_map((u128)(h->n - 1));
+    RolloutDraws d{hop.mult, hop.geo, n_choices > 0 ? (double)n_choices : sa.low[0], n_choices > 0 ? 0.0 : sa.high[0], 0};
+    for (uint64_t last = (uint64_t)(h->n - 1); last != 0; last >>= 4) d.jump_digits++;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_sampled_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, d, s, st);
+    case B200GYM_MOUNTAINCAR: return launch_rollout_sampled_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, d, s, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_sampled_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, d, s, st);
+    case B200GYM_PENDULUM: return launch_rollout_sampled_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, d, s, st);
+    case B200GYM_ACROBOT: return launch_rollout_sampled_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, d, s, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------

@@ -9,6 +9,7 @@
 #pragma once
 
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/b200gym.h"
 #include "envs.cuh"
@@ -280,12 +281,41 @@ struct RolloutSink {
     }
 };
 
-// T steps of env i (rollout_kernel), the same as T launches of kernel A: advance_env and, when the episode ended,
-// reset_env, with the state and TimeLimit counter loaded once and stored once.  a.actions, a.obs, a.reward,
-// a.terminated, a.truncated and a.final_obs hold slice 0 of [T][n] arrays; CartPole's autoreset=False flag byte stays
-// in global memory, where advance_env keeps it
-template <int KIND, typename ActT>
-__device__ __forceinline__ void rollout_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs) {
+// Where a rollout's actions come from.  Row t of the [T][n] array at a.actions holds the actions of step t; the
+// driver walks it with one pointer, `row`.  ReadActions: the caller wrote it (b200gym_rollout), so env i's action is
+// read from it
+struct ReadActions {
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const { return __ldg(row + i); }
+    __device__ __forceinline__ void next() const {}
+};
+
+// DrawActions: the rollout fills it (b200gym_rollout_sampled), drawing from the batched action space's stream.  Every
+// classic kind has one action element per env (Discrete, or Box of shape (1,)), so env i's action of step t is draw
+// t * n + i: g starts before draw i, takes one draw per step and then hops the n - 1 draws of the other envs
+// (state -> hop_mult * state + hop_plus).  The value drawn is stored to the row and decoded like a value read from it
+struct DrawActions {
+    bgym::Pcg64 g;
+    bgym::u128 hop_mult, hop_plus;
+    double p0, p1;   // Discrete: n_choices (p1 unused); Box(1): low, high
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) {
+        ActT v;
+        if constexpr (std::is_same<ActT, long long>::value) v = bgym::sample_multidiscrete(g, p0);
+        else v = bgym::sample_box(g, p0, p1);
+        store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+    __device__ __forceinline__ void next() { g.state = hop_mult * g.state + hop_plus; }
+};
+
+// T steps of env i (rollout_kernel, rollout_sampled_kernel), the same as T launches of kernel A: advance_env and,
+// when the episode ended, reset_env, with the state and TimeLimit counter loaded once and stored once; the actions
+// come from `src`.  a.actions, a.obs, a.reward, a.terminated, a.truncated and a.final_obs hold slice 0 of [T][n]
+// arrays; CartPole's autoreset=False flag byte stays in global memory, where advance_env keeps it
+template <int KIND, typename ActT, typename Src = ReadActions>
+__device__ __forceinline__ void rollout_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                            Src src = Src{}) {
     using E = bgym::Env<KIND>;
     const int64_t n = a.n;
     double s[E::S];
@@ -298,8 +328,9 @@ __device__ __forceinline__ void rollout_env(const StepArgs &a, int64_t i, int32_
         if (t == T - 1) sink.last = last_obs;
         long long action_int = 0;
         float a0 = 0.0f;
-        decode_action<KIND>(__ldg(act + i), action_int, a0);
+        decode_action<KIND>(src.action(act, i), action_int, a0);
         if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        src.next();
         act += n;
         sink.o += n * E::D;
         sink.r += n;
@@ -310,6 +341,27 @@ __device__ __forceinline__ void rollout_env(const StepArgs &a, int64_t i, int32_
 #pragma unroll
     for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
     a.elapsed[i] = elapsed;
+}
+
+// What every thread of a rollout_sampled_kernel launch shares: the map of n - 1 draws (independent of inc, like
+// SampleArgs.hop_geo, so that a graph replayed after a reseed cannot hold a stale hop) and the plan of the single
+// action space
+struct RolloutDraws {
+    bgym::u128 hop_mult, hop_geo;
+    double p0, p1;      // as DrawActions
+    int jump_digits;    // hex digits of n - 1: the rows of kLcgJump the first jumps use
+};
+
+// ... with the actions drawn from `start`, the generator before draw 0 of the launch, into a.actions: a table jump
+// to draw i, then DrawActions
+template <int KIND>
+__device__ __forceinline__ void rollout_sampled_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                    const RolloutDraws &d, const bgym::Pcg64 &start,
+                                                    const bgym::LcgJumpTable &table) {
+    using ActT = typename std::conditional<bgym::Env<KIND>::A == 0, long long, float>::type;
+    DrawActions src{start, d.hop_mult, d.hop_geo * start.inc, d.p0, d.p1};
+    bgym::pcg64_jump_table(src.g, (uint64_t)i, table);
+    rollout_env<KIND, ActT>(a, i, T, last_obs, src);
 }
 
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the

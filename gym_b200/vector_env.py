@@ -597,25 +597,74 @@ class B200VectorEnv:
         tensors that belong to the caller; ``infos["final_observation"]`` is (T, N, D), valid where
         ``infos["_final_observation"]`` (T, N) is set.  The classic-control kinds run the T steps in one launch with
         each env's state in registers (DESIGN.md §4.10).  May be captured in a CUDA graph."""
-        self._assert_open("rollout")
+        captured = self._rollout_guards("rollout")
+        act, code = self._device_actions(actions, captured, steps=True)
+        T = int(act.shape[0])
+        obs, reward, term, trunc, final_obs, last = self._rollout_outputs(T)
+        _lib.check(self._lib.b200gym_rollout(
+            self._handle, ctypes.c_void_p(act.data_ptr()), code, T, ctypes.c_void_p(obs.data_ptr()),
+            ctypes.c_void_p(reward.data_ptr()), ctypes.c_void_p(term.data_ptr()), ctypes.c_void_p(trunc.data_ptr()),
+            ctypes.c_void_p(final_obs.data_ptr()) if self.autoreset else None, ctypes.c_void_p(last.data_ptr()),
+            self._stream()), self._handle)
+        self._last_actions = act  # keep alive until the kernel has consumed it
+        return obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
+
+    def rollout_sampled(self, T):
+        """T steps of random actions -> ``(actions, obs, rewards, terminateds, truncateds, infos)``, each with a leading
+        T axis: bit for bit what ``a = self.sample_actions(); self.step(a)`` repeated T times returns, stacked, with
+        the env and the action space's generator left where that loop leaves them.  ``actions`` is int64 (T, N) for
+        Discrete kinds and float32 (T, N, A) for Box kinds; the other five are as ``rollout()`` returns them.  The
+        outputs are new tensors that belong to the caller.  The classic-control kinds draw the actions inside the
+        rollout kernel, next to each env's state, so they are written once and never read back (DESIGN.md §4.11).
+
+        May be captured in a CUDA graph once the device holds the generator, as ``sample_actions()``: each replay
+        continues the stream on the device, and ``sync_action_space()`` brings the host generator there."""
+        captured = self._rollout_guards("rollout_sampled")
+        n_choices, cols, low, high, bit_generator, state, words = self._sample_begin("rollout_sampled()", captured)
+        if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
+            raise ValueError(f"rollout_sampled(T) needs an integer 1 <= T < 2**31, got {T!r}")
+        T = int(T)
+        torch = _torch()
+        n = self.num_envs
+        actions = torch.empty((T, n) if n_choices else (T, n, cols), dtype=torch.int64 if n_choices else torch.float32,
+                              device=self.device)
+        obs, reward, term, trunc, final_obs, last = self._rollout_outputs(T)
+        _lib.check(self._lib.b200gym_rollout_sampled(
+            self._handle, ctypes.c_void_p(self._sample_record.data_ptr()), words, n_choices,
+            None if low is None else low.ctypes.data, None if high is None else high.ctypes.data, T,
+            ctypes.c_void_p(actions.data_ptr()), ctypes.c_void_p(obs.data_ptr()), ctypes.c_void_p(reward.data_ptr()),
+            ctypes.c_void_p(term.data_ptr()), ctypes.c_void_p(trunc.data_ptr()),
+            ctypes.c_void_p(final_obs.data_ptr()) if self.autoreset else None, ctypes.c_void_p(last.data_ptr()),
+            self._stream()), self._handle)
+        self._sample_end(bit_generator, state, actions.numel(), captured)
+        return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
+
+    def _rollout_guards(self, what):
+        """The refusals of rollout() / rollout_sampled(), all raised before any CUDA call -> whether a CUDA graph is
+        being captured."""
+        self._assert_open(what)
         if self.backend == "numpy":
-            raise error.Error("rollout() needs backend='torch': backend='numpy' steps through host buffers")
+            raise error.Error(f"{what}() needs backend='torch': backend='numpy' steps through host buffers")
         if self._chain is not None:
-            raise error.Error("rollout() cannot run per-env wrappers (wrappers=): the chain runs after every step, "
+            raise error.Error(f"{what}() cannot run per-env wrappers (wrappers=): the chain runs after every step, "
                               "and the fused rollout kernel has no step boundary to run it at")
         if self._state != _STATE_DEFAULT:
             raise error.AlreadyPendingCallError(
-                f"Calling `rollout` while waiting for a pending call to `{self._state}` to complete.", self._state)
+                f"Calling `{what}` while waiting for a pending call to `{self._state}` to complete.", self._state)
         if not self._has_reset:
-            raise error.ResetNeeded("Cannot call env.rollout() before calling env.reset()")
-        torch = _torch()
+            raise error.ResetNeeded(f"Cannot call env.{what}() before calling env.reset()")
         captured = capturing()
         # the same poll as step_async: an invalid action of an earlier call raises here (not while capturing)
         if self.discrete and not captured and self._lib.b200gym_invalid_seen(self._handle) == 1:
             self.check_actions()
         self._raise_snapshot_index_error()
-        act, code = self._device_actions(actions, captured, steps=True)
-        T, n, dev = int(act.shape[0]), self.num_envs, self.device
+        return captured
+
+    def _rollout_outputs(self, T):
+        """(obs, reward, terminated, truncated, final_obs) with a leading T axis, new tensors, and the handle's buffer
+        that receives the last observations."""
+        torch = _torch()
+        n, dev = self.num_envs, self.device
         shape = (T, n) + self._obs_shape
         obs = torch.empty(shape, dtype=torch.float32, device=dev)
         reward = torch.empty((T, n), dtype=torch.float64, device=dev)
@@ -625,14 +674,7 @@ class B200VectorEnv:
         final_obs = (torch.empty if self.autoreset else torch.zeros)(shape, dtype=torch.float32, device=dev)
         # the last observations also go to the next set of the double buffer, where snapshot() / clone() read them
         self._flip ^= 1
-        last = self._out[self._flip]["obs"]
-        _lib.check(self._lib.b200gym_rollout(
-            self._handle, ctypes.c_void_p(act.data_ptr()), code, T, ctypes.c_void_p(obs.data_ptr()),
-            ctypes.c_void_p(reward.data_ptr()), ctypes.c_void_p(term.data_ptr()), ctypes.c_void_p(trunc.data_ptr()),
-            ctypes.c_void_p(final_obs.data_ptr()) if self.autoreset else None, ctypes.c_void_p(last.data_ptr()),
-            self._stream()), self._handle)
-        self._last_actions = act  # keep alive until the kernel has consumed it
-        return obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
+        return obs, reward, term, trunc, final_obs, self._out[self._flip]["obs"]
 
     def check_actions(self):
         """Number of out-of-range Discrete actions the device saw since the last check (syncs)."""
@@ -675,6 +717,23 @@ class B200VectorEnv:
         self._refuse_numpy_capture("sample_actions")
         if self.backend == "numpy":
             return space.sample()
+        captured = capturing()
+        n_choices, cols, low, high, bit_generator, state, words = self._sample_begin("sample_actions()", captured)
+        shape = (self.num_envs,) if n_choices else (self.num_envs, cols)
+        torch = _torch()
+        out = torch.empty(shape, dtype=torch.int64 if n_choices else torch.float32, device=self.device)
+        _lib.check(self._lib.b200gym_sample_space_stream(ctypes.c_void_p(self._sample_record.data_ptr()), words,
+                                                         self.num_envs, cols, n_choices,
+                                                         None if low is None else low.ctypes.data,
+                                                         None if high is None else high.ctypes.data,
+                                                         ctypes.c_void_p(out.data_ptr()), self._stream()))
+        self._sample_end(bit_generator, state, out.numel(), captured)
+        return out
+
+    def _sample_begin(self, what, captured):
+        """The launch arguments of a draw from the device record of the action space's stream (sample_actions(),
+        rollout_sampled()) -> (n_choices, cols, low, high, bit generator, its state, override words or None)."""
+        space = self.action_space
         n_choices, cols, low, high = self._sample_plan()
         shape = (self.num_envs,) if n_choices else (self.num_envs, cols)
         if (type(space).__name__ != ("MultiDiscrete" if n_choices else "Box") or tuple(space.shape) != shape
@@ -683,30 +742,25 @@ class B200VectorEnv:
         bit_generator = space.np_random.bit_generator
         state = pcg64_state(bit_generator)
         s, inc = state["state"]["state"], state["state"]["inc"]
-        # The draws come from the device record (b200gym_sample_space_stream), which the launch also advances, so a
-        # captured call continues the stream at every replay.  The mirror is what the host last left in the record:
-        # a host generator that differs from it (drawn from or reseeded on the host) is passed as the override.
+        # The draws come from the device record, which the launch also advances, so a captured call continues the
+        # stream at every replay.  The mirror is what the host last left in the record: a host generator that differs
+        # from it (drawn from or reseeded on the host) is passed as the override.
         in_sync = self._sample_mirror == (s, inc)
-        captured = capturing()
         if captured:
             if not in_sync:
-                raise error.Error("sample_actions() cannot be captured in a CUDA graph before the device holds the "
-                                  "action space's generator: call sample_actions() once outside the capture (after "
+                raise error.Error(f"{what} cannot be captured in a CUDA graph before the device holds the "
+                                  f"action space's generator: call {what} once outside the capture (after "
                                   "any action_space.seed() or host draw)")
         mask = (1 << 64) - 1
         words = None if in_sync else (ctypes.c_uint64 * 4)(s >> 64, s & mask, inc >> 64, inc & mask)
-        torch = _torch()
-        out = torch.empty(shape, dtype=torch.int64 if n_choices else torch.float32, device=self.device)
-        _lib.check(self._lib.b200gym_sample_space_stream(ctypes.c_void_p(self._sample_record.data_ptr()), words,
-                                                         self.num_envs, cols, n_choices,
-                                                         None if low is None else low.ctypes.data,
-                                                         None if high is None else high.ctypes.data,
-                                                         ctypes.c_void_p(out.data_ptr()), self._stream()))
+        return n_choices, cols, low, high, bit_generator, state, words
+
+    def _sample_end(self, bit_generator, state, count, captured):
+        """After an eager launch that drew `count` elements: the host generator skips them and the mirror follows."""
         if not captured:   # a capture leaves the host where it is: replays advance the record alone
-            pcg64_skip(bit_generator, state, out.numel())
+            pcg64_skip(bit_generator, state, count)
             st = pcg64_state(bit_generator)["state"]
             self._sample_mirror = (st["state"], st["inc"])
-        return out
 
     def sync_action_space(self):
         """Move ``self.action_space``'s generator to where the device stream of ``sample_actions()`` is (synchronises).

@@ -56,6 +56,12 @@ class VectorWrapper:
         raise error.Error(f"{type(self).__name__} does not support rollout(): it acts after every step, and a fused "
                           "rollout of the wrapped env would skip it; call step() T times instead")
 
+    def rollout_sampled(self, T):
+        """Refused, as rollout(): step the wrapper with ``sample_actions()`` instead."""
+        from gym_b200 import error
+        raise error.Error(f"{type(self).__name__} does not support rollout_sampled(): it acts after every step, and a "
+                          "fused rollout of the wrapped env would skip it; call step(sample_actions()) T times instead")
+
     def close(self, **kwargs):
         return self.env.close(**kwargs)
 

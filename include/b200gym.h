@@ -176,6 +176,28 @@ int b200gym_rollout(b200gym_t *h, const void *actions_dev, int action_dtype, int
                     double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
                     float *last_obs_dev, void *stream);
 
+/*
+ * b200gym_rollout of random actions: T times `actions = action_space.sample(); step(actions)` of the batched action
+ * space, with the draws made by the rollout itself.  Every slice is bit for bit what T pairs of
+ * b200gym_sample_space_stream (rows = n) and b200gym_step write, and the handle and the record are left where those
+ * calls leave them: the record ends T * n * max(act_dim, 1) draws later, with the ticket at 0.
+ *   record_dev, override_pcg64   as b200gym_sample_space_stream; the record must be on the handle's device
+ *   n_choices, low_host, high_host  the single action space, as b200gym_sample_space: Discrete kinds n_choices >= 1;
+ *                  Box kinds n_choices = 0 and the act_dim bounds
+ *   T              >= 1
+ *   actions_out_dev  16-byte aligned, on the handle's device: [T][n] int64 (Discrete) or [T][n][act_dim] float32 (Box)
+ *                  receives the actions drawn
+ *   obs_dev ... last_obs_dev   as b200gym_rollout
+ * Classic-control kinds: ONE launch; thread i carries the space's generator next to env i's state and draws its
+ * actions t * n + i of the stream as it goes, so the actions are written but never read back.  Box2D kinds: one
+ * b200gym_sample_space_stream launch of T * n rows, then the b200gym_rollout sequence.  Offsets and stream deltas are
+ * 64-bit.
+ */
+int b200gym_rollout_sampled(b200gym_t *h, uint64_t *record_dev, const uint64_t override_pcg64[4], int64_t n_choices,
+                            const double *low_host, const double *high_host, int32_t T, void *actions_out_dev,
+                            float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                            float *final_obs_dev, float *last_obs_dev, void *stream);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
