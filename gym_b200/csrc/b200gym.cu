@@ -329,6 +329,51 @@ __global__ void __launch_bounds__(kThreads) rollout_sampled_kernel(const StepArg
     if (threadIdx.x == 0 && ticket == gridDim.x - 1ULL) sample_stream_finish(s, g);
 }
 
+// ... with the actions computed by each env's linear policy from the observation of the step before
+// (rollout_linear_env); SUMMARY: no per-step outputs, one episode summary per env
+template <int KIND, bool SUMMARY>
+__global__ void __launch_bounds__(kThreads) rollout_linear_kernel(const StepArgs a, const int32_t T, float *last_obs,
+                                                                  const LinearPolicyArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < a.n) rollout_linear_env<KIND, SUMMARY>(a, i, T, last_obs, p);
+}
+
+// One step's actions of a Box2D linear-policy rollout, before that step's launches: env i's policy at its observation
+// row obs[i] (K logits over D inputs, linear_logits), into actions[i] (int64 argmax_first if DISCRETE, else K float32).
+// fold / init: the episode summary of b200gym_rollout_linear, folded from the step before's reward and flags
+template <int K, int D, bool DISCRETE>
+__global__ void __launch_bounds__(kThreads) linear_policy_kernel(const float *obs, void *actions,
+                                                                 const LinearPolicyArgs p, const double *reward,
+                                                                 const uint8_t *term, const uint8_t *trunc, int64_t n,
+                                                                 int32_t t_prev, int act, int init) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (init) {
+        p.returns[i] = 0.0;
+        p.lengths[i] = 0;
+        p.ended[i] = 0;
+    } else if (t_prev >= 0 && !p.ended[i]) {   // step t_prev is the first episode end or before it
+        p.returns[i] = p.returns[i] + reward[i];
+        p.lengths[i] = t_prev + 1;
+        p.ended[i] = (term[i] | trunc[i]) != 0;
+    }
+    if (!act) return;
+    float o[D], w[K * D], b[K], z[K];
+#pragma unroll
+    for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
+#pragma unroll
+    for (int k = 0; k < K * D; k++) w[k] = __ldg(p.weight + i * p.w_stride + k);
+#pragma unroll
+    for (int j = 0; j < K; j++) b[j] = __ldg(p.bias + i * p.b_stride + j);
+    linear_logits<K, D>(w, b, o, z);
+    if constexpr (DISCRETE) {
+        static_cast<long long *>(actions)[i] = argmax_first<K>(z);
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; j++) static_cast<float *>(actions)[i * K + j] = z[j];
+    }
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -2529,6 +2574,113 @@ extern "C" int b200gym_rollout_sampled(b200gym_t *h, uint64_t *record_dev, const
         return launch_rollout_sampled_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, d, s, st);
     case B200GYM_PENDULUM: return launch_rollout_sampled_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, d, s, st);
     case B200GYM_ACROBOT: return launch_rollout_sampled_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, d, s, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+// ---- closed-loop rollouts of a linear policy (b200gym_rollout_linear) ----
+template <int KIND>
+static int launch_rollout_linear_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                      const LinearPolicyArgs &p, bool summary, cudaStream_t st) {
+    if (summary) rollout_linear_kernel<KIND, true><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs, p);
+    else rollout_linear_kernel<KIND, false><<<blocks_for(h->n), kThreads, 0, st>>>(a, T, last_obs, p);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// A Box2D linear-policy rollout: per step, one linear_policy_kernel launch from the observation rows of the step
+// before (first_obs for step 0), then launch_step_box2d into slice t.  Summary mode: every step runs in one scratch
+// slice, and the policy launch of step t + 1 (or one last launch) folds step t into the summary
+static int launch_rollout_linear_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                       const float *first_obs, const LinearPolicyArgs &p, bool summary,
+                                       cudaStream_t st) {
+    const int64_t n = h->n, D = h->D, cols = std::max(h->A, 1);
+    using Policy = void (*)(const float *, void *, const LinearPolicyArgs, const double *, const uint8_t *,
+                            const uint8_t *, int64_t, int32_t, int, int);
+    Policy policy;
+    switch (h->cfg.kind) {
+    case B200GYM_LUNARLANDER: policy = linear_policy_kernel<4, 8, true>; break;
+    case B200GYM_LUNARLANDER_CONT: policy = linear_policy_kernel<2, 8, false>; break;
+    default: policy = linear_policy_kernel<4, 24, false>; break;   // BipedalWalker(Hardcore)
+    }
+    const size_t act_row = (size_t)n * cols * (h->A == 0 ? sizeof(long long) : sizeof(float));
+    const int action_dtype = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
+    StepArgs s = a;
+    void *scratch = nullptr;
+    if (summary) {   // one slice of every per-step output, 16-byte aligned pieces
+        const size_t obs_bytes = ((size_t)n * D * sizeof(float) + 15) / 16 * 16, act_bytes = (act_row + 15) / 16 * 16;
+        const size_t r_bytes = ((size_t)n * sizeof(double) + 15) / 16 * 16, f_bytes = ((size_t)n + 15) / 16 * 16;
+        CK(h, cudaMallocAsync(&scratch, obs_bytes + act_bytes + r_bytes + 2 * f_bytes, st));
+        unsigned char *base = static_cast<unsigned char *>(scratch);
+        s.obs = reinterpret_cast<float *>(base);
+        s.actions = base + obs_bytes;
+        s.reward = reinterpret_cast<double *>(base + obs_bytes + act_bytes);
+        s.terminated = base + obs_bytes + act_bytes + r_bytes;
+        s.truncated = s.terminated + f_bytes;
+        s.final_obs = nullptr;
+    }
+    const unsigned blocks = (unsigned)blocks_for(n);
+    int rc = 0;
+    for (int32_t t = 0; t < T && !rc; t++) {
+        const float *obs_in = t == 0 ? first_obs : s.obs;
+        if (!summary) {
+            s.actions = static_cast<const unsigned char *>(a.actions) + (size_t)t * act_row;
+            s.obs = a.obs + t * n * D;
+            s.reward = a.reward + t * n;
+            s.terminated = a.terminated + t * n;
+            s.truncated = a.truncated + t * n;
+            s.final_obs = a.final_obs ? a.final_obs + t * n * D : nullptr;
+        }
+        policy<<<blocks, kThreads, 0, st>>>(obs_in, const_cast<void *>(s.actions), p, s.reward, s.terminated,
+                                            s.truncated, n, summary ? t - 1 : -1, 1, summary && t == 0);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "linear_policy_kernel: launch failed");
+        else rc = launch_step_box2d(h, s, action_dtype, st);
+    }
+    if (!rc && summary) {
+        policy<<<blocks, kThreads, 0, st>>>(s.obs, nullptr, p, s.reward, s.terminated, s.truncated, n, T - 1, 0, 0);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "linear_policy_kernel: launch failed");
+    }
+    if (!rc && cudaMemcpyAsync(last_obs, s.obs, (size_t)n * D * sizeof(float), cudaMemcpyDeviceToDevice, st))
+        rc = fail(h, "b200gym_rollout_linear: copy of the last observations failed");
+    if (scratch) cudaFreeAsync(scratch, st);
+    return rc;
+}
+
+extern "C" int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env,
+                                      int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                      uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                      double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev,
+                                      float *last_obs_dev, const float *first_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout_linear: null handle");
+    if (T < 1) return fail(h, "b200gym_rollout_linear: T must be at least 1 (got %d)", T);
+    if (!weight_dev || !bias_dev || !last_obs_dev) return fail(h, "b200gym_rollout_linear: null buffer");
+    const bool summary = returns_dev != nullptr;
+    if (summary ? (!lengths_dev || !ended_dev || actions_out_dev || obs_dev || reward_dev || terminated_dev ||
+                   truncated_dev || final_obs_dev)
+                : (!actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || lengths_dev ||
+                   ended_dev))
+        return fail(h, "b200gym_rollout_linear: give either the per-step outputs or returns, lengths and ended");
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "b200gym_rollout_linear: a Box2D env needs first_obs_dev");
+    const int64_t K = h->A == 0 ? h->NACT : h->A;
+    LinearPolicyArgs p{weight_dev, bias_dev, per_env ? K * h->D : 0, per_env ? K : 0, returns_dev, lengths_dev,
+                       ended_dev};
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_linear_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, p, summary, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_linear_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, p, summary, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_linear_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, p, summary, st);
+    case B200GYM_PENDULUM: return launch_rollout_linear_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, p, summary, st);
+    case B200GYM_ACROBOT: return launch_rollout_linear_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, p, summary, st);
+    case B200GYM_LUNARLANDER:
+    case B200GYM_LUNARLANDER_CONT:
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_linear_box2d(h, a, T, last_obs_dev, first_obs_dev, p, summary, st);
     }
     return fail(h, "bad kind %d", h->cfg.kind);
 }

@@ -279,6 +279,14 @@ struct RolloutSink {
     __device__ __forceinline__ void final_obs(I i, const float (&v)[D]) const {
         if (fin) obs_row<D>(fin, i, v);
     }
+    // on to the rows of the next slice
+    __device__ __forceinline__ void next(int64_t n) {
+        o += n * bgym::Env<KIND>::D;
+        r += n;
+        te += n;
+        tr += n;
+        if (fin) fin += n * bgym::Env<KIND>::D;
+    }
 };
 
 // Where a rollout's actions come from.  Row t of the [T][n] array at a.actions holds the actions of step t; the
@@ -362,6 +370,164 @@ __device__ __forceinline__ void rollout_sampled_env(const StepArgs &a, int64_t i
     DrawActions src{start, d.hop_mult, d.hop_geo * start.inc, d.p0, d.p1};
     bgym::pcg64_jump_table(src.g, (uint64_t)i, table);
     rollout_env<KIND, ActT>(a, i, T, last_obs, src);
+}
+
+// ---- closed-loop rollouts of a linear policy (b200gym_rollout_linear) ---------------------------------------------
+
+// The logits z of the linear policy (weight (K, D) row-major, bias (K,)) at the float32 observation o: z[j] starts at
+// bias[j] and adds weight[j, k] * o[k] for k = 0 .. D-1 in that order, every product and every sum rounded to float32
+// (the library is built with -fmad=false and the host build with -ffp-contract=off, so nothing is fused)
+template <int K, int D>
+__device__ __forceinline__ void linear_logits(const float *w, const float *b, const float (&o)[D], float (&z)[K]) {
+#pragma unroll
+    for (int j = 0; j < K; j++) {
+        float v = b[j];
+#pragma unroll
+        for (int k = 0; k < D; k++) v = v + w[j * D + k] * o[k];
+        z[j] = v;
+    }
+}
+
+// np.argmax(z): the index of the first NaN if any logit is NaN, otherwise of the first maximum
+template <int K>
+__device__ __forceinline__ int argmax_first(const float (&z)[K]) {
+    float m = z[0];
+    int best = 0;
+#pragma unroll
+    for (int j = 1; j < K; j++) {
+        if (m == m && (z[j] != z[j] || z[j] > m)) {
+            m = z[j];
+            best = j;
+        }
+    }
+    return best;
+}
+
+// The number of logits of a linear policy of kind KIND: the Discrete kinds' choices, the Box kinds' act_dim
+template <int KIND>
+constexpr int linear_logit_count() {
+    return bgym::Env<KIND>::A == 0 ? bgym::Env<KIND>::NACT : bgym::Env<KIND>::A;
+}
+
+// LinearActions: the rollout computes them (b200gym_rollout_linear) from `o`, the observation the env last returned,
+// which LinearSink keeps current: argmax_first of the logits for a Discrete kind, the logits themselves for a Box kind.
+// The action is stored to the row unless SUMMARY (no per-step outputs) and decoded like a value read from it
+template <int KIND, bool SUMMARY>
+struct LinearActions {
+    static constexpr int K = linear_logit_count<KIND>(), D = bgym::Env<KIND>::D;
+    float w[K * D], b[K];
+    const float (&o)[D];
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
+        float z[K];
+        linear_logits<K, D>(w, b, o, z);
+        ActT v;
+        if constexpr (bgym::Env<KIND>::A == 0) v = (ActT)argmax_first<K>(z);
+        else v = z[0];
+        if constexpr (!SUMMARY) store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+};
+
+// The sink of a linear-policy rollout: RolloutSink's, plus every observation the step produces (the step's own, or the
+// reset observation after an autoreset) copied to `seen`, the policy's input of the next step.  SUMMARY: nothing is
+// stored per step but the last observation; the reward and flags are folded into the episode summary in registers
+template <int KIND, bool SUMMARY>
+struct LinearSink : RolloutSink<KIND> {
+    using Base = RolloutSink<KIND>;
+    float (&seen)[bgym::Env<KIND>::D];
+    double &ret;     // 0.0 + the rewards up to the first episode end, in step order
+    int32_t &len;    // steps up to and including the first episode end
+    bool &ended;
+    template <int D, typename I>
+    __device__ __forceinline__ void obs(I i, const float (&v)[D]) const {
+        if constexpr (SUMMARY) {
+            if (this->last) store_row<D>(this->last, i, v);
+        } else {
+            Base::template obs<D>(i, v);
+        }
+#pragma unroll
+        for (int k = 0; k < D; k++) seen[k] = v[k];
+    }
+    template <typename I>
+    __device__ __forceinline__ void scalars(I i, double reward, uint8_t term, uint8_t trunc) const {
+        if constexpr (SUMMARY) {
+            if (!ended) {
+                ret = ret + reward;
+                len += 1;
+                ended = (term | trunc) != 0;
+            }
+        } else {
+            Base::scalars(i, reward, term, trunc);
+        }
+    }
+    template <int D, typename I>
+    __device__ __forceinline__ void final_obs(I i, const float (&v)[D]) const {
+        if constexpr (!SUMMARY) Base::template final_obs<D>(i, v);
+    }
+    __device__ __forceinline__ void next(int64_t n) {
+        if constexpr (!SUMMARY) Base::next(n);
+    }
+};
+
+// The parameters and summary outputs of a b200gym_rollout_linear launch.  Env i's policy is weight + i * w_stride
+// (K * D floats) and bias + i * b_stride (K floats); strides 0: one policy shared by every env
+struct LinearPolicyArgs {
+    const float *weight, *bias;
+    int64_t w_stride, b_stride;
+    double *returns;    // [n], SUMMARY only
+    int32_t *lengths;
+    uint8_t *ended;
+};
+
+// T steps of env i under its linear policy (rollout_linear_kernel): rollout_env's loop with LinearActions and
+// LinearSink.  (Routing rollout_env itself through one loop shared with this driver changes the code the compiler
+// makes for the Pendulum and Acrobot rollout kernels, so the loop is kept twice.)  Step 0's input is observe() of the
+// state just loaded: for the classic kinds the observation the env last returned is that function of its state, and
+// the state, unlike the double-buffered observation rows, is where a CUDA graph replay finds the current one.  The
+// parameters are loaded once.  SUMMARY: no per-step outputs, the episode summary stored once at the end
+template <int KIND, bool SUMMARY>
+__device__ __forceinline__ void rollout_linear_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                   const LinearPolicyArgs &p) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    using Src = LinearActions<KIND, SUMMARY>;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D];
+    E::observe(s, o);
+    Src src{{}, {}, o};
+    const float *w = p.weight + i * p.w_stride, *b = p.bias + i * p.b_stride;
+#pragma unroll
+    for (int k = 0; k < Src::K * E::D; k++) src.w[k] = __ldg(w + k);
+#pragma unroll
+    for (int j = 0; j < Src::K; j++) src.b[j] = __ldg(b + j);
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, SUMMARY> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                   o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+    if constexpr (SUMMARY) {
+        p.returns[i] = ret;
+        p.lengths[i] = len;
+        p.ended[i] = ended ? 1 : 0;
+    }
 }
 
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the

@@ -639,9 +639,84 @@ class B200VectorEnv:
         self._sample_end(bit_generator, state, actions.numel(), captured)
         return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
 
+    def rollout_linear(self, weight, bias, T, *, summary=False):
+        """T steps of a linear policy in closed loop: bit for bit what
+        ``for t in range(T): a = policy(obs); obs, r, te, tr, info = self.step(a)`` returns, stacked, with ``obs``
+        starting at the observation the env last returned, and the env left where that loop leaves it.
+
+        With K = ``single_action_space.n`` (Discrete) or ``act_dim`` (Box) and D = ``obs_dim``, ``weight`` (K, D) and
+        ``bias`` (K,) are one policy for every env, or ``weight`` (N, K, D) and ``bias`` (N, K) one per env: float32,
+        contiguous, on the env's device.  The logits are ``z[j] = bias[j]``, then ``z[j] = z[j] + weight[j, k] * o[k]``
+        for k = 0 .. D-1, every float32 product and sum rounded (no fused multiply-add).  The action is ``np.argmax(z)``
+        (the first NaN, else the first maximum) for Discrete kinds and ``z`` itself, unclipped, for Box kinds.
+
+        ``summary=False`` -> ``(actions, obs, rewards, terminateds, truncateds, infos)`` as ``rollout_sampled()``
+        returns them.  ``summary=True`` -> ``(returns, lengths, ended)``, each (N,), over env i's first episode end
+        within the call (t_end; T - 1 if none): float64 ``0.0 + rewards[0] + ... + rewards[t_end]`` in step order,
+        int32 ``t_end + 1``, and bool; the env still takes all T steps, and no per-step tensor is allocated.
+
+        The classic-control kinds run the T steps in one launch, the policy next to each env's state, and start from
+        the observation of the current state (after ``set_state()``, that is the first input).  They may be captured in
+        a CUDA graph: replays read the current contents of ``weight`` and ``bias``.  The Box2D kinds launch the policy
+        and the step once per step and cannot be captured (DESIGN.md §4.12)."""
+        captured = self._rollout_guards("rollout_linear")
+        per_env = self._linear_params(weight, bias)
+        if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
+            raise ValueError(f"rollout_linear(T) needs an integer 1 <= T < 2**31, got {T!r}")
+        T = int(T)
+        if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
+                         _lib.KIND_BIPEDALWALKER_HARDCORE):
+            refuse_capture("rollout_linear() of a Box2D env", "its step 0 reads the observation rows the env last "
+                           "returned, which alternate between two buffers from call to call, so a replay would read a "
+                           "stale set")
+        first = self._out[self._flip]["obs"]   # the observations the env last returned, before the flip below
+        torch = _torch()
+        n, dev, vp = self.num_envs, self.device, ctypes.c_void_p
+        if summary:
+            returns = torch.empty(n, dtype=torch.float64, device=dev)
+            lengths = torch.empty(n, dtype=torch.int32, device=dev)
+            ended = torch.empty(n, dtype=torch.bool, device=dev)
+            self._flip ^= 1
+            last = self._out[self._flip]["obs"]
+            outs = [None] * 6 + [vp(returns.data_ptr()), vp(lengths.data_ptr()), vp(ended.data_ptr())]
+        else:
+            actions = torch.empty((T, n) if self.discrete else (T, n, self.act_dim),
+                                  dtype=torch.int64 if self.discrete else torch.float32, device=dev)
+            obs, reward, term, trunc, final_obs, last = self._rollout_outputs(T)
+            outs = [vp(actions.data_ptr()), vp(obs.data_ptr()), vp(reward.data_ptr()), vp(term.data_ptr()),
+                    vp(trunc.data_ptr()), vp(final_obs.data_ptr()) if self.autoreset else None, None, None, None]
+        _lib.check(self._lib.b200gym_rollout_linear(
+            self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env), T, *outs, vp(last.data_ptr()),
+            vp(first.data_ptr()), self._stream()), self._handle)
+        if summary:
+            return returns, lengths, ended
+        return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
+
+    def _linear_params(self, weight, bias):
+        """Check rollout_linear()'s parameters without a CUDA call -> whether they are per env."""
+        torch = _torch()
+        K = self.single_action_space.n if self.discrete else self.act_dim
+        K, D, n = int(K), self.obs_dim, self.num_envs
+        for name, x in (("weight", weight), ("bias", bias)):
+            if not isinstance(x, torch.Tensor):
+                raise ValueError(f"rollout_linear() needs {name} as a torch tensor, got {type(x).__name__}")
+            if x.dtype != torch.float32:
+                raise ValueError(f"rollout_linear() needs float32 {name}, got {x.dtype}")
+            if x.device != self.device:
+                raise ValueError(f"rollout_linear() needs {name} on {self.device}, got {x.device}")
+            if not x.is_contiguous():
+                raise ValueError(f"rollout_linear() needs a contiguous {name}")
+        shared = tuple(weight.shape) == (K, D) and tuple(bias.shape) == (K,)
+        per_env = tuple(weight.shape) == (n, K, D) and tuple(bias.shape) == (n, K)
+        if not (shared or per_env):
+            raise ValueError(f"rollout_linear() needs weight ({K}, {D}) and bias ({K},) for one policy, or weight "
+                             f"({n}, {K}, {D}) and bias ({n}, {K}) for one per env; got {tuple(weight.shape)} and "
+                             f"{tuple(bias.shape)}")
+        return per_env
+
     def _rollout_guards(self, what):
-        """The refusals of rollout() / rollout_sampled(), all raised before any CUDA call -> whether a CUDA graph is
-        being captured."""
+        """The refusals of rollout() / rollout_sampled() / rollout_linear(), all raised before any CUDA call -> whether
+        a CUDA graph is being captured."""
         self._assert_open(what)
         if self.backend == "numpy":
             raise error.Error(f"{what}() needs backend='torch': backend='numpy' steps through host buffers")

@@ -198,6 +198,40 @@ int b200gym_rollout_sampled(b200gym_t *h, uint64_t *record_dev, const uint64_t o
                             float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
                             float *final_obs_dev, float *last_obs_dev, void *stream);
 
+/*
+ * b200gym_rollout of a linear policy in closed loop: T times `actions = policy(obs); obs, ... = step(actions)`, where
+ * obs starts at the observation the env last returned.  With K = num_actions (Discrete kinds) or act_dim (Box kinds),
+ * D = obs_dim and o the float32 observation, the logits are
+ *     z[j] = bias[j];  for k in 0 .. D-1: z[j] = z[j] + weight[j][k] * o[k]
+ * in float32 with every product and every sum rounded (no fused multiply-add).  Discrete: the action is the index of
+ * the first NaN logit if there is one, else of the first maximum (np.argmax).  Box: the action is z, unclipped.
+ * Every slice is bit for bit what T pairs of that policy and b200gym_step write, and the handle is left where they
+ * leave it.
+ *   weight_dev, bias_dev  float32 on the handle's device, contiguous: [K][D] and [K] (per_env = 0, one policy for
+ *                  every env) or [n][K][D] and [n][K] (per_env = 1, env i uses row i); read by the launch, so a
+ *                  captured call reads their current contents at every replay
+ *   T              >= 1
+ * Per-step outputs (returns_dev NULL): actions_out_dev receives the actions, [T][n] int64 (Discrete) or
+ *                  [T][n][act_dim] float32 (Box); obs_dev ... final_obs_dev as b200gym_rollout; lengths_dev and
+ *                  ended_dev NULL.
+ * Summary (returns_dev non-NULL): actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev and final_obs_dev
+ *                  are NULL, and with t_end the first step at which terminated | truncated (T - 1 if none):
+ *   returns_dev    [n] float64: 0.0 + reward[0] + ... + reward[t_end], added in step order
+ *   lengths_dev    [n] int32: t_end + 1
+ *   ended_dev      [n] uint8: 1 if the episode ended within the T steps
+ *   last_obs_dev   [n][obs_dim] float32: receives the observations of step T - 1, in both modes
+ *   first_obs_dev  [n][obs_dim] float32: the observations the env last returned, step 0's input for the Box2D kinds;
+ *                  ignored (may be NULL) for the classic-control kinds, whose step 0 starts from the state
+ * Classic-control kinds: ONE launch; step 0's input is the observation of the env's current state (the observation
+ * every step and reset returns), each later step's the observation the step before produced, held in registers with
+ * the policy.  Box2D kinds: per step, one policy launch and the b200gym_step sequence; the summary mode steps through
+ * one scratch slice.  Offsets are 64-bit.
+ */
+int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env, int32_t T,
+                           void *actions_out_dev, float *obs_dev, double *reward_dev, uint8_t *terminated_dev,
+                           uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
+                           uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
