@@ -2162,6 +2162,20 @@ extern "C" int b200gym_selftest_trig(const double *x_dev, int64_t n, double *sin
     return 0;
 }
 
+// b2probe.cu: the probe kernel, in a module of its own so that this module's kernels compile as they did without it
+cudaError_t b2probe_launch(int op, const float *in_dev, int64_t n, float *out_dev, cudaStream_t stream);
+int b2probe_num_ops();
+
+extern "C" int b200gym_selftest_box2d(int op, const float *in_dev, int64_t n, float *out_dev, void *stream) {
+    if (op < 0 || op >= b2probe_num_ops() || !in_dev || !out_dev || n <= 0)
+        return fail(nullptr, "b200gym_selftest_box2d: bad argument");
+    const int dev = device_of(in_dev);
+    if (dev < 0 || device_of(out_dev) != dev) return fail(nullptr, "b200gym_selftest_box2d: buffers are not on one device");
+    DeviceGuard guard(dev);
+    CK(nullptr, b2probe_launch(op, in_dev, n, out_dev, (cudaStream_t)stream));
+    return 0;
+}
+
 extern "C" int b200gym_box2d_overflows(b200gym_t *h, void *stream, int64_t *count_out) {
     if (!h || !count_out) return fail(h, "b200gym_box2d_overflows: null argument");
     if (!h->is_lunar && !h->is_walker) return fail(h, "b200gym_box2d_overflows: not a Box2D-task handle");

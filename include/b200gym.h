@@ -615,6 +615,13 @@ int b200gym_selftest(int device, int64_t samples, uint64_t seed, int64_t *mismat
  * sq_dev may be NULL.  Asynchronous.
  */
 int b200gym_selftest_trig(const double *x_dev, int64_t n, double *sin_dev, double *cos_dev, double *sq_dev, void *stream);
+/*
+ * Device self-test of the Box2D building blocks (csrc/b2probe.cuh): one thread per record runs `op` on in_dev[n][16]
+ * float32 and writes out_dev[n][16].  op: 0 rot_of, 1 edge-polygon manifold, 2 box-polygon manifold, 3 edge ray cast,
+ * 4 box ray cast, 5 GJK distance, 6 time of impact, 7 solve22, 8 solve33; the record layouts are listed in
+ * b2probe.cuh.  Loads the task polygons into constant memory as b200gym_create does, then launches asynchronously.
+ */
+int b200gym_selftest_box2d(int op, const float *in_dev, int64_t n, float *out_dev, void *stream);
 
 #ifdef __cplusplus
 }

@@ -16,6 +16,7 @@
 #include "../../gym_b200/csrc/rng.cuh"
 #include "../../gym_b200/csrc/envs.cuh"
 #include "../../gym_b200/csrc/box2d_consts.h"
+#include "../../gym_b200/csrc/b2probe.cuh"
 #include "../../gym_b200/csrc/per_env.cuh"
 
 using bgym::Pcg64;
@@ -385,6 +386,12 @@ int hs_toi_probe(int shape, const float *c0, float a0, const float *c1, float a1
     xf1.p = b2l::sub(sB.c, b2l::rmul(xf1.q, sh.localCenter));
     *cannot_touch = b2l::toi_cannot_touch(sh, xf1, sB, pA) ? 1 : 0;
     return b2l::time_of_impact(*t_out, pA, sA, pB, sB, 1.0f);
+}
+
+// b200gym_selftest_box2d's per-record dispatch (csrc/b2probe.cuh) over in[n][16] -> out[n][16]
+void hs_box2d_probe(int op, const float *in, int64_t n, float *out) {
+    ensure_consts();
+    for (int64_t i = 0; i < n; i++) b2probe::probe_case(op, in + i * b2probe::kProbeWords, out + i * b2probe::kProbeWords);
 }
 
 // The task polygon `shape` as the device constants hold it: vertices (x, y pairs) into out, local centre into lc;

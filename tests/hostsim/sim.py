@@ -19,7 +19,8 @@ _LIB_SMALLCAP = os.path.join(_BUILD, "libhostsim_smallcap.so")
 SMALLCAP = {"lunar": 1, "walker": 2}
 _SRCS = [os.path.join(_HERE, "hostsim.cpp"), os.path.join(_HERE, "cuda_shim.h")] + [
     os.path.join(_ROOT, "gym_b200", "csrc", f) for f in ("rng.cuh", "envs.cuh", "glibc_trig.cuh", "b2lite.cuh", "b2lite_toi.cuh", "lunar.cuh",
-                                                         "walker.cuh", "per_env.cuh", "box2d_consts.h")]
+                                                         "walker.cuh", "per_env.cuh", "box2d_consts.h",
+                                                         "b2probe.cuh")]
 
 KIND = {"LunarLander": 5, "BipedalWalker": 6, "LunarLanderContinuous": 7, "BipedalWalkerHardcore": 8}
 _lib = None
@@ -70,6 +71,7 @@ def lib(smallcap=False):
         fp, f32 = ctypes.POINTER(ctypes.c_float), ctypes.c_float
         L.hs_toi_probe.restype = i32
         L.hs_toi_probe.argtypes = [i32, fp, f32, fp, f32, fp, fp, fp, fp, ctypes.POINTER(i32)]
+        L.hs_box2d_probe.argtypes = [i32, vp, i64, vp]
         if smallcap:
             _libs["small"] = L
             return L
@@ -262,3 +264,11 @@ def toi_probe(shape, c0, a0, c1, a1, edge=None, box=None):
                             ctypes.byref(t), ctypes.byref(ct))
     return int(st), float(t.value), bool(ct.value)
 
+
+
+def box2d_probe(op, records):
+    """csrc/b2probe.cuh on the CPU: op on float32 records (n, 16) -> (n, 16), what b200gym_selftest_box2d computes."""
+    rec = np.ascontiguousarray(records, dtype=np.float32).reshape(-1, 16)
+    out = np.zeros_like(rec)
+    lib().hs_box2d_probe(int(op), rec.ctypes.data, rec.shape[0], out.ctypes.data)
+    return out

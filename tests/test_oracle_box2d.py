@@ -525,20 +525,7 @@ def test_gjk_distance_matches_brute_force_geometry():
     termination) against an independent computation: the distance between a convex polygon and a segment is the
     minimum over (polygon vertex, segment) and (segment endpoint, polygon edge) point-to-segment distances when they
     do not overlap, and 0 when they do.  3 000 random poses of the lander's hexagon and of a thin leg box."""
-    def seg_dist(p, a, b):
-        ab, ap = b - a, p - a
-        t = np.clip(np.dot(ap, ab) / np.dot(ab, ab), 0.0, 1.0)
-        return float(np.linalg.norm(ap - t * ab))
-
-    def intersects(p1, p2, q1, q2):
-        def orient(a, b, c):
-            return (b[0] - a[0]) * (c[1] - a[1]) - (b[1] - a[1]) * (c[0] - a[0])
-        return (orient(p1, p2, q1) * orient(p1, p2, q2) < 0) and (orient(q1, q2, p1) * orient(q1, q2, p2) < 0)
-
-    def inside(poly, p):
-        n = len(poly)
-        return all(((poly[(i + 1) % n][0] - poly[i][0]) * (p[1] - poly[i][1]) - (poly[(i + 1) % n][1] - poly[i][1]) * (p[0] - poly[i][0])) >= 0
-                   for i in range(n))
+    from box2d_geometry import inside, intersects, seg_dist
 
     # both counter-clockwise, as b2PolygonShape::Set leaves them
     hexagon = np.array([(-17, -10), (17, -10), (17, 0), (14, 17), (-14, 17), (-17, 0)], dtype=np.float64) / 30.0
