@@ -374,6 +374,66 @@ __global__ void __launch_bounds__(kThreads) linear_policy_kernel(const float *ob
     }
 }
 
+// The CTA's shared copy of the `count` floats of one MLP policy shared by every env.  It is read from device memory at
+// every launch, so a replayed CUDA graph uses the current contents of the parameters.  Every thread of the CTA calls it
+__device__ __forceinline__ const float *mlp_stage(const float *params, int64_t count) {
+    extern __shared__ float4 mlp_shared[];
+    float *s = reinterpret_cast<float *>(mlp_shared);
+    for (int64_t q = threadIdx.x; q < count; q += blockDim.x) s[q] = __ldg(params + q);
+    __syncthreads();
+    return s;
+}
+
+// ... with the actions computed by each env's MLP policy from the observation of the step before (rollout_mlp_env):
+// PER_ENV, env i's row of parameters read from device memory at every step; otherwise one policy, staged in shared
+// memory once per CTA.  SUMMARY: no per-step outputs, one episode summary per env.  Held to 128 registers (two CTAs
+// per SM), ptxas spills the per-env Pendulum kernels, so the per-env kernels ask for one CTA per SM instead
+template <int KIND, bool SUMMARY, bool PER_ENV>
+__global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2) rollout_mlp_kernel(const StepArgs a, const int32_t T, float *last_obs,
+                                                               const MlpPolicyArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (PER_ENV) {
+        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, true>(a, i, T, last_obs, p.params + i * p.stride, p);
+    } else {
+        using Src = MlpActions<KIND, SUMMARY, false>;
+        const float *w = mlp_stage(p.params, mlp_param_count<Src::K, Src::D>(p.h1, p.h2));
+        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, false>(a, i, T, last_obs, w, p);
+    }
+}
+
+// One step's actions of a Box2D MLP-policy rollout, before that step's launches: linear_policy_kernel with env i's
+// MLP (mlp_outputs; PER_ENV as rollout_mlp_kernel) in place of its linear policy
+template <int K, int D, bool DISCRETE, bool PER_ENV>
+__global__ void __launch_bounds__(kThreads) mlp_policy_kernel(const float *obs, void *actions, const MlpPolicyArgs p,
+                                                              const double *reward, const uint8_t *term,
+                                                              const uint8_t *trunc, int64_t n, int32_t t_prev, int act,
+                                                              int init) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float *w = nullptr;
+    if (act) w = PER_ENV ? p.params + i * p.stride : mlp_stage(p.params, mlp_param_count<K, D>(p.h1, p.h2));
+    if (i >= n) return;
+    if (init) {
+        p.returns[i] = 0.0;
+        p.lengths[i] = 0;
+        p.ended[i] = 0;
+    } else if (t_prev >= 0 && !p.ended[i]) {   // step t_prev is the first episode end or before it
+        p.returns[i] = p.returns[i] + reward[i];
+        p.lengths[i] = t_prev + 1;
+        p.ended[i] = (term[i] | trunc[i]) != 0;
+    }
+    if (!act) return;
+    float o[D], z[K];
+#pragma unroll
+    for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
+    mlp_outputs<K, D, PER_ENV>(w, p.h1, p.h2, p.vec != 0, o, z);
+    if constexpr (DISCRETE) {
+        static_cast<long long *>(actions)[i] = argmax_first<K>(z);
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; j++) static_cast<float *>(actions)[i * K + j] = z[j];
+    }
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -2602,21 +2662,18 @@ static int launch_rollout_linear_kind(b200gym *h, const StepArgs &a, int32_t T, 
     return 0;
 }
 
-// A Box2D linear-policy rollout: per step, one linear_policy_kernel launch from the observation rows of the step
-// before (first_obs for step 0), then launch_step_box2d into slice t.  Summary mode: every step runs in one scratch
-// slice, and the policy launch of step t + 1 (or one last launch) folds step t into the summary
-static int launch_rollout_linear_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
-                                       const float *first_obs, const LinearPolicyArgs &p, bool summary,
-                                       cudaStream_t st) {
+// A Box2D closed-loop rollout: per step, one launch of `policy` (linear_policy_kernel, mlp_policy_kernel) from the
+// observation rows of the step before (first_obs for step 0), with `smem` bytes of dynamic shared memory, then
+// launch_step_box2d into slice t.  Summary mode: every step runs in one scratch slice, and the policy launch of step
+// t + 1 (or one last launch) folds step t into the summary.  kernel / entry: names for the error messages
+template <typename Args>
+static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                       const float *first_obs, const Args &p,
+                                       void (*policy)(const float *, void *, const Args, const double *,
+                                                      const uint8_t *, const uint8_t *, int64_t, int32_t, int, int),
+                                       size_t smem, bool summary, cudaStream_t st, const char *kernel,
+                                       const char *entry) {
     const int64_t n = h->n, D = h->D, cols = std::max(h->A, 1);
-    using Policy = void (*)(const float *, void *, const LinearPolicyArgs, const double *, const uint8_t *,
-                            const uint8_t *, int64_t, int32_t, int, int);
-    Policy policy;
-    switch (h->cfg.kind) {
-    case B200GYM_LUNARLANDER: policy = linear_policy_kernel<4, 8, true>; break;
-    case B200GYM_LUNARLANDER_CONT: policy = linear_policy_kernel<2, 8, false>; break;
-    default: policy = linear_policy_kernel<4, 24, false>; break;   // BipedalWalker(Hardcore)
-    }
     const size_t act_row = (size_t)n * cols * (h->A == 0 ? sizeof(long long) : sizeof(float));
     const int action_dtype = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
     StepArgs s = a;
@@ -2645,19 +2702,34 @@ static int launch_rollout_linear_box2d(b200gym *h, const StepArgs &a, int32_t T,
             s.truncated = a.truncated + t * n;
             s.final_obs = a.final_obs ? a.final_obs + t * n * D : nullptr;
         }
-        policy<<<blocks, kThreads, 0, st>>>(obs_in, const_cast<void *>(s.actions), p, s.reward, s.terminated,
-                                            s.truncated, n, summary ? t - 1 : -1, 1, summary && t == 0);
-        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "linear_policy_kernel: launch failed");
+        policy<<<blocks, kThreads, smem, st>>>(obs_in, const_cast<void *>(s.actions), p, s.reward, s.terminated,
+                                               s.truncated, n, summary ? t - 1 : -1, 1, summary && t == 0);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: launch failed", kernel);
         else rc = launch_step_box2d(h, s, action_dtype, st);
     }
     if (!rc && summary) {
-        policy<<<blocks, kThreads, 0, st>>>(s.obs, nullptr, p, s.reward, s.terminated, s.truncated, n, T - 1, 0, 0);
-        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "linear_policy_kernel: launch failed");
+        policy<<<blocks, kThreads, smem, st>>>(s.obs, nullptr, p, s.reward, s.terminated, s.truncated, n, T - 1, 0,
+                                               0);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: launch failed", kernel);
     }
     if (!rc && cudaMemcpyAsync(last_obs, s.obs, (size_t)n * D * sizeof(float), cudaMemcpyDeviceToDevice, st))
-        rc = fail(h, "b200gym_rollout_linear: copy of the last observations failed");
+        rc = fail(h, "%s: copy of the last observations failed", entry);
     if (scratch) cudaFreeAsync(scratch, st);
     return rc;
+}
+
+static int launch_rollout_linear_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                       const float *first_obs, const LinearPolicyArgs &p, bool summary,
+                                       cudaStream_t st) {
+    void (*policy)(const float *, void *, const LinearPolicyArgs, const double *, const uint8_t *, const uint8_t *,
+                   int64_t, int32_t, int, int);
+    switch (h->cfg.kind) {
+    case B200GYM_LUNARLANDER: policy = linear_policy_kernel<4, 8, true>; break;
+    case B200GYM_LUNARLANDER_CONT: policy = linear_policy_kernel<2, 8, false>; break;
+    default: policy = linear_policy_kernel<4, 24, false>; break;   // BipedalWalker(Hardcore)
+    }
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, p, policy, 0, summary, st, "linear_policy_kernel",
+                                       "b200gym_rollout_linear");
 }
 
 extern "C" int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env,
@@ -2695,6 +2767,85 @@ extern "C" int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, con
     case B200GYM_BIPEDALWALKER:
     case B200GYM_BIPEDALWALKER_HARDCORE:
         return launch_rollout_linear_box2d(h, a, T, last_obs_dev, first_obs_dev, p, summary, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+// ---- closed-loop rollouts of a ReLU MLP policy (b200gym_rollout_mlp) ----
+template <int KIND>
+static int launch_rollout_mlp_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const MlpPolicyArgs &p,
+                                   bool per_env, size_t smem, bool summary, cudaStream_t st) {
+    const unsigned blocks = blocks_for(h->n);
+    if (per_env) {
+        if (summary) rollout_mlp_kernel<KIND, true, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+        else rollout_mlp_kernel<KIND, false, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+    } else {
+        if (summary) rollout_mlp_kernel<KIND, true, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+        else rollout_mlp_kernel<KIND, false, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+template <int K, int D, bool DISCRETE>
+static int launch_rollout_mlp_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
+                                    const MlpPolicyArgs &p, bool per_env, size_t smem, bool summary, cudaStream_t st) {
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, p,
+                                       per_env ? mlp_policy_kernel<K, D, DISCRETE, true>
+                                               : mlp_policy_kernel<K, D, DISCRETE, false>,
+                                       per_env ? 0 : smem, summary, st, "mlp_policy_kernel", "b200gym_rollout_mlp");
+}
+
+extern "C" int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                                   int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                   uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                   double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev, float *last_obs_dev,
+                                   const float *first_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout_mlp: null handle");
+    if (n_layers != 1 && n_layers != 2)
+        return fail(h, "b200gym_rollout_mlp: n_layers must be 1 or 2 (got %d)", n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "b200gym_rollout_mlp: hidden widths must be 1 .. %d (got %d, %d)", kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "b200gym_rollout_mlp: T must be at least 1 (got %d)", T);
+    if (!params_dev || !last_obs_dev) return fail(h, "b200gym_rollout_mlp: null buffer");
+    const bool summary = returns_dev != nullptr;
+    if (summary ? (!lengths_dev || !ended_dev || actions_out_dev || obs_dev || reward_dev || terminated_dev ||
+                   truncated_dev || final_obs_dev)
+                : (!actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || lengths_dev ||
+                   ended_dev))
+        return fail(h, "b200gym_rollout_mlp: give either the per-step outputs or returns, lengths and ended");
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "b200gym_rollout_mlp: a Box2D env needs first_obs_dev");
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    // 16-byte rows of the second layer: h1 % 4 == 0 puts every row of it at a multiple of 4 floats from the policy's
+    // start; a per-env policy's start must itself be 16-byte aligned, the shared copy always is
+    const bool vec = h1 % 4 == 0 && (!per_env || (P % 4 == 0 && reinterpret_cast<uintptr_t>(params_dev) % 16 == 0));
+    const MlpPolicyArgs p{params_dev, per_env ? P : 0, h1, h2, vec ? 1 : 0, returns_dev, lengths_dev, ended_dev};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;   // at most 24.1 KB (BipedalWalker at (64, 64)): no opt-in needed
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool pe = per_env != 0;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_box2d<4, 8, true>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_box2d<2, 8, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_box2d<4, 24, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
     }
     return fail(h, "bad kind %d", h->cfg.kind);
 }

@@ -530,6 +530,171 @@ __device__ __forceinline__ void rollout_linear_env(const StepArgs &a, int64_t i,
     }
 }
 
+// ---- closed-loop rollouts of a ReLU MLP policy (b200gym_rollout_mlp) ----------------------------------------------
+
+constexpr int kMlpMaxWidth = 64;   // the widest hidden layer b200gym_rollout_mlp takes
+
+// The hidden layers' activation: z if z > 0 or z is NaN, else +0.0 (so NaN propagates and -0.0 becomes +0.0)
+__device__ __forceinline__ float mlp_relu(float z) { return (z > 0.0f || z != z) ? z : 0.0f; }
+
+// A parameter of the MLP: from device memory through the read-only path (GLOBAL, each env's own row), or from the
+// CTA's shared copy
+template <bool GLOBAL>
+__device__ __forceinline__ float mlp_ld(const float *p) {
+    if constexpr (GLOBAL) return __ldg(p);
+    else return *p;
+}
+template <bool GLOBAL>
+__device__ __forceinline__ float4 mlp_ld4(const float *p) {
+    if constexpr (GLOBAL) return __ldg(reinterpret_cast<const float4 *>(p));
+    else return *reinterpret_cast<const float4 *>(p);
+}
+
+// The K outputs z of the MLP D -> h1 (-> h2) -> K (h2 = 0: one hidden layer) whose packed parameters start at w: layer
+// by layer the weight (out, in) row-major, then the bias (out,).  Every unit starts at its bias and adds
+// weight[j, k] * x[k] for k = 0 .. in-1 in that order, every product and sum rounded to float32 (the library is built
+// with -fmad=false and the host build with -ffp-contract=off), as linear_logits; a hidden unit then goes through
+// mlp_relu.  The first hidden layer is held in a register array of kMlpMaxWidth under guarded, fully unrolled loops.
+// The last hidden layer is not stored: each of its units is added into the K outputs as soon as it is computed, in
+// ascending order, which is the same sum as adding them afterwards.  vec: every row of the second layer's weight starts
+// 16 bytes aligned and h1 % 4 == 0, so those rows (the bulk of the parameters) are read 16 bytes at a time
+template <int K, int D, bool GLOBAL>
+__device__ __forceinline__ void mlp_outputs(const float *w, int h1, int h2, bool vec, const float (&o)[D],
+                                            float (&z)[K]) {
+    const float *b1 = w + h1 * D, *w2 = b1 + h1;
+    if (h2 == 0) {
+        const float *b2 = w2 + K * h1;
+#pragma unroll
+        for (int k = 0; k < K; k++) z[k] = mlp_ld<GLOBAL>(b2 + k);
+        for (int j = 0; j < h1; j++) {
+            float u = mlp_ld<GLOBAL>(b1 + j);
+#pragma unroll
+            for (int k = 0; k < D; k++) u = u + mlp_ld<GLOBAL>(w + j * D + k) * o[k];
+            u = mlp_relu(u);
+#pragma unroll
+            for (int k = 0; k < K; k++) z[k] = z[k] + mlp_ld<GLOBAL>(w2 + k * h1 + j) * u;
+        }
+        return;
+    }
+    float x[kMlpMaxWidth];
+#pragma unroll
+    for (int j = 0; j < kMlpMaxWidth; j++) {
+        x[j] = 0.0f;
+        if (j < h1) {
+            float u = mlp_ld<GLOBAL>(b1 + j);
+#pragma unroll
+            for (int k = 0; k < D; k++) u = u + mlp_ld<GLOBAL>(w + j * D + k) * o[k];
+            x[j] = mlp_relu(u);
+        }
+    }
+    const float *b2 = w2 + h2 * h1, *w3 = b2 + h2, *b3 = w3 + K * h2;
+#pragma unroll
+    for (int k = 0; k < K; k++) z[k] = mlp_ld<GLOBAL>(b3 + k);
+    for (int j = 0; j < h2; j++) {
+        const float *row = w2 + j * h1;
+        float u = mlp_ld<GLOBAL>(b2 + j);
+        if (vec) {
+#pragma unroll
+            for (int m = 0; m < kMlpMaxWidth; m += 4) {
+                if (m < h1) {
+                    const float4 q = mlp_ld4<GLOBAL>(row + m);
+                    u = u + q.x * x[m];
+                    u = u + q.y * x[m + 1];
+                    u = u + q.z * x[m + 2];
+                    u = u + q.w * x[m + 3];
+                }
+            }
+        } else {
+#pragma unroll
+            for (int m = 0; m < kMlpMaxWidth; m++)
+                if (m < h1) u = u + mlp_ld<GLOBAL>(row + m) * x[m];
+        }
+        u = mlp_relu(u);
+#pragma unroll
+        for (int k = 0; k < K; k++) z[k] = z[k] + mlp_ld<GLOBAL>(w3 + k * h2 + j) * u;
+    }
+}
+
+// P, the number of floats of one MLP policy D -> h1 (-> h2) -> K: the sum over layers of out * in + out
+template <int K, int D>
+__host__ __device__ __forceinline__ int64_t mlp_param_count(int64_t h1, int64_t h2) {
+    return h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + h2 * h1 + h2 + K * h2 + K;
+}
+
+// The parameters and summary outputs of a b200gym_rollout_mlp launch.  Env i's policy is the P floats at
+// params + i * stride; stride 0: one policy shared by every env, which each CTA first copies to shared memory
+struct MlpPolicyArgs {
+    const float *params;
+    int64_t stride;
+    int32_t h1, h2;     // hidden widths, h2 = 0 for one hidden layer
+    int32_t vec;        // as mlp_outputs
+    double *returns;    // [n], SUMMARY only
+    int32_t *lengths;
+    uint8_t *ended;
+};
+
+// MlpActions: LinearActions with the MLP's outputs in place of the logits.  w: the env's parameters, in device memory
+// (GLOBAL) or the CTA's shared copy
+template <int KIND, bool SUMMARY, bool GLOBAL>
+struct MlpActions {
+    static constexpr int K = linear_logit_count<KIND>(), D = bgym::Env<KIND>::D;
+    const float *w;
+    int h1, h2;
+    bool vec;
+    const float (&o)[D];
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
+        float z[K];
+        mlp_outputs<K, D, GLOBAL>(w, h1, h2, vec, o, z);
+        ActT v;
+        if constexpr (bgym::Env<KIND>::A == 0) v = (ActT)argmax_first<K>(z);
+        else v = z[0];
+        if constexpr (!SUMMARY) store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+};
+
+// T steps of env i under its MLP policy at w (rollout_mlp_kernel): rollout_linear_env's loop, written out again so
+// that no pre-existing kernel changes, with MlpActions in place of LinearActions.  The parameters are read at every
+// step, from w: a per-env row in device memory (GLOBAL), too large for registers, or the CTA's shared copy
+template <int KIND, bool SUMMARY, bool GLOBAL>
+__device__ __forceinline__ void rollout_mlp_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                const float *w, const MlpPolicyArgs &p) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D];
+    E::observe(s, o);
+    const MlpActions<KIND, SUMMARY, GLOBAL> src{w, p.h1, p.h2, p.vec != 0, o};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, SUMMARY> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                   o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+    if constexpr (SUMMARY) {
+        p.returns[i] = ret;
+        p.lengths[i] = len;
+        p.ended[i] = ended ? 1 : 0;
+    }
+}
+
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the
 // observation row.  References as in lunar_reset_env.
 template <int KIND>

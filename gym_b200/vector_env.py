@@ -661,12 +661,42 @@ class B200VectorEnv:
         and the step once per step and cannot be captured (DESIGN.md §4.12)."""
         captured = self._rollout_guards("rollout_linear")
         per_env = self._linear_params(weight, bias)
+        vp = ctypes.c_void_p
+        return self._policy_rollout("rollout_linear", T, summary, captured, lambda T, outs, last, first: (
+            self._lib.b200gym_rollout_linear(self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env), T,
+                                             *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+
+    def rollout_mlp(self, params, hidden, T, *, summary=False):
+        """T steps of a ReLU MLP policy in closed loop: ``rollout_linear()`` with the policy
+        D -> hidden[0] (-> hidden[1]) -> K, ReLU after every hidden layer and nothing after the last.
+
+        ``hidden`` is a tuple of one or two widths, each 1 .. 64.  ``params`` packs one policy as P float32 values,
+        layer by layer the weight (out, in) row-major and then the bias (out,): exactly
+        ``torch.nn.utils.parameters_to_vector(nn.Sequential(nn.Linear(D, H1), nn.ReLU(), ..., nn.Linear(H_last, K)))``.
+        Shape (P,) is one policy for every env, (N, P) one per env: float32, contiguous, on the env's device.
+
+        Every unit is ``z[j] = bias[j]``, then ``z[j] = z[j] + W[j, k] * x[k]`` for k = 0 .. in-1, every float32
+        product and sum rounded (no fused multiply-add).  A hidden unit's activation is ``z`` if ``z > 0`` or ``z`` is
+        NaN, else +0.0 (NaN propagates, -0.0 becomes +0.0).  The action is taken from the K outputs as
+        ``rollout_linear()`` takes it from its logits.  Returns, guards, capture and the start from the current state
+        are ``rollout_linear()``'s (DESIGN.md §4.13)."""
+        captured = self._rollout_guards("rollout_mlp")
+        h1, h2, per_env = self._mlp_params(params, hidden)
+        vp = ctypes.c_void_p
+        return self._policy_rollout("rollout_mlp", T, summary, captured, lambda T, outs, last, first: (
+            self._lib.b200gym_rollout_mlp(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T,
+                                          *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+
+    def _policy_rollout(self, what, T, summary, captured, launch):
+        """The checks after the parameters', the outputs, and the call of rollout_linear() / rollout_mlp(), whose
+        entry point ``launch(T, outs, last, first)`` calls with the output pointers, the buffer that receives the last
+        observations and the observations the env last returned."""
         if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
-            raise ValueError(f"rollout_linear(T) needs an integer 1 <= T < 2**31, got {T!r}")
+            raise ValueError(f"{what}(T) needs an integer 1 <= T < 2**31, got {T!r}")
         T = int(T)
         if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
                          _lib.KIND_BIPEDALWALKER_HARDCORE):
-            refuse_capture("rollout_linear() of a Box2D env", "its step 0 reads the observation rows the env last "
+            refuse_capture(f"{what}() of a Box2D env", "its step 0 reads the observation rows the env last "
                            "returned, which alternate between two buffers from call to call, so a replay would read a "
                            "stale set")
         first = self._out[self._flip]["obs"]   # the observations the env last returned, before the flip below
@@ -685,9 +715,7 @@ class B200VectorEnv:
             obs, reward, term, trunc, final_obs, last = self._rollout_outputs(T)
             outs = [vp(actions.data_ptr()), vp(obs.data_ptr()), vp(reward.data_ptr()), vp(term.data_ptr()),
                     vp(trunc.data_ptr()), vp(final_obs.data_ptr()) if self.autoreset else None, None, None, None]
-        _lib.check(self._lib.b200gym_rollout_linear(
-            self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env), T, *outs, vp(last.data_ptr()),
-            vp(first.data_ptr()), self._stream()), self._handle)
+        _lib.check(launch(T, outs, last, first), self._handle)
         if summary:
             return returns, lengths, ended
         return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
@@ -714,9 +742,34 @@ class B200VectorEnv:
                              f"{tuple(bias.shape)}")
         return per_env
 
+    def _mlp_params(self, params, hidden):
+        """Check rollout_mlp()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden layer), per_env)."""
+        torch = _torch()
+        if not isinstance(hidden, (tuple, list)) or not 1 <= len(hidden) <= 2 or any(
+                isinstance(h, (bool, np.bool_)) or not isinstance(h, (int, np.integer)) or not 1 <= int(h) <= 64
+                for h in hidden):
+            raise ValueError(f"rollout_mlp() needs hidden as a tuple of one or two widths, each 1 .. 64, got {hidden!r}")
+        widths = [int(h) for h in hidden]
+        K = self.single_action_space.n if self.discrete else self.act_dim
+        sizes = [self.obs_dim] + widths + [int(K)]
+        P = sum(o * i + o for i, o in zip(sizes[:-1], sizes[1:]))
+        if not isinstance(params, torch.Tensor):
+            raise ValueError(f"rollout_mlp() needs params as a torch tensor, got {type(params).__name__}")
+        if params.dtype != torch.float32:
+            raise ValueError(f"rollout_mlp() needs float32 params, got {params.dtype}")
+        if params.device != self.device:
+            raise ValueError(f"rollout_mlp() needs params on {self.device}, got {params.device}")
+        if not params.is_contiguous():
+            raise ValueError("rollout_mlp() needs contiguous params")
+        per_env = tuple(params.shape) == (self.num_envs, P)
+        if not (per_env or tuple(params.shape) == (P,)):
+            raise ValueError(f"rollout_mlp() with hidden {tuple(widths)} needs params ({P},) for one policy or "
+                             f"({self.num_envs}, {P}) for one per env; got {tuple(params.shape)}")
+        return widths[0], widths[1] if len(widths) == 2 else 0, per_env
+
     def _rollout_guards(self, what):
-        """The refusals of rollout() / rollout_sampled() / rollout_linear(), all raised before any CUDA call -> whether
-        a CUDA graph is being captured."""
+        """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp(), all raised before any CUDA
+        call -> whether a CUDA graph is being captured."""
         self._assert_open(what)
         if self.backend == "numpy":
             raise error.Error(f"{what}() needs backend='torch': backend='numpy' steps through host buffers")

@@ -232,6 +232,27 @@ int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, const float *b
                            uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
                            uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
 
+/*
+ * b200gym_rollout_linear with a ReLU MLP policy: layers D -> h1 (-> h2) -> K, K and D as there.  One policy is P floats,
+ * P = sum over layers of out * in + out, packed layer by layer as the weight [out][in] row-major, then the bias [out]
+ * (torch.nn.utils.parameters_to_vector of nn.Sequential(nn.Linear(D, h1), nn.ReLU(), ..., nn.Linear(h_last, K))).
+ * Every unit, x being the layer's float32 input, is
+ *     z[j] = bias[j];  for k in 0 .. in-1: z[j] = z[j] + weight[j][k] * x[k]
+ * with every product and every sum rounded (no fused multiply-add); a hidden unit is then z[j] if z[j] > 0 or z[j] is
+ * NaN, else +0.0.  The action is taken from the K outputs as b200gym_rollout_linear takes it from its logits.
+ *   params_dev     float32 on the handle's device, contiguous: [P] (per_env = 0, one policy for every env) or [n][P]
+ *                  (per_env = 1, env i uses row i); read by the launch, so a captured call reads its current contents
+ *                  at every replay
+ *   n_layers       1 or 2 hidden layers; h1, h2 their widths, 1 .. 64 (h2 ignored for one layer)
+ *   T ... first_obs_dev  as b200gym_rollout_linear
+ * Classic-control kinds: ONE launch; a shared policy is staged in each CTA's shared memory, a per-env row is read from
+ * device memory at every step.  Box2D kinds: per step, one policy launch and the b200gym_step sequence.
+ */
+int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2, int32_t T,
+                        void *actions_out_dev, float *obs_dev, double *reward_dev, uint8_t *terminated_dev,
+                        uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
+                        uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
