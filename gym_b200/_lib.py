@@ -138,6 +138,8 @@ SIGNATURES = {
                                       _vp]),
     "b200gym_rollout_mlp": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                    _vp, _vp, _vp, _vp]),
+    "b200gym_rollout_mlp_noisy": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp]),
     "b200gym_invalid_actions": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_invalid_seen": (_i32, [_vp]),
     "b200gym_host_buffers": (_i32, [_vp, ctypes.POINTER(HostIO)]),

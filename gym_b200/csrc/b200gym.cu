@@ -434,6 +434,45 @@ __global__ void __launch_bounds__(kThreads) mlp_policy_kernel(const float *obs, 
     }
 }
 
+// ... with the actions computed by each env's MLP policy plus the caller's noise (rollout_mlp_noisy_env); PER_ENV and
+// the launch bounds as rollout_mlp_kernel
+template <int KIND, bool PER_ENV>
+__global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2)
+    rollout_mlp_noisy_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpNoisyArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (PER_ENV) {
+        if (i < a.n) rollout_mlp_noisy_env<KIND, true>(a, i, T, last_obs, p.mlp.params + i * p.mlp.stride, p);
+    } else {
+        using Src = MlpNoisyActions<KIND, false>;
+        const float *w = mlp_stage(p.mlp.params, mlp_param_count<Src::K, Src::D>(p.mlp.h1, p.mlp.h2));
+        if (i < a.n) rollout_mlp_noisy_env<KIND, false>(a, i, T, last_obs, w, p);
+    }
+}
+
+// One step's actions of a Box2D noisy MLP-policy rollout: mlp_policy_kernel with the step's noise slice added to the
+// outputs (noisy_outputs), which go to the step's outputs slice.  The launch passes p.noise and p.outputs at that
+// step's slice.  No summary mode: reward, term, trunc, t_prev, act and init are the launcher's and unused here
+template <int K, int D, bool DISCRETE, bool PER_ENV>
+__global__ void __launch_bounds__(kThreads) mlp_noisy_policy_kernel(const float *obs, void *actions,
+                                                                    const MlpNoisyArgs p, const double *, const uint8_t *,
+                                                                    const uint8_t *, int64_t n, int32_t, int, int) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float *w = PER_ENV ? p.mlp.params + i * p.mlp.stride
+                             : mlp_stage(p.mlp.params, mlp_param_count<K, D>(p.mlp.h1, p.mlp.h2));
+    if (i >= n) return;
+    float o[D], z[K], y[K];
+#pragma unroll
+    for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
+    mlp_outputs<K, D, PER_ENV>(w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, z);
+    noisy_outputs<K>(z, p.noise + i * K, p.outputs + i * K, y);
+    if constexpr (DISCRETE) {
+        static_cast<long long *>(actions)[i] = argmax_first<K>(y);
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; j++) static_cast<float *>(actions)[i * K + j] = y[j];
+    }
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -2662,13 +2701,14 @@ static int launch_rollout_linear_kind(b200gym *h, const StepArgs &a, int32_t T, 
     return 0;
 }
 
-// A Box2D closed-loop rollout: per step, one launch of `policy` (linear_policy_kernel, mlp_policy_kernel) from the
-// observation rows of the step before (first_obs for step 0), with `smem` bytes of dynamic shared memory, then
-// launch_step_box2d into slice t.  Summary mode: every step runs in one scratch slice, and the policy launch of step
-// t + 1 (or one last launch) folds step t into the summary.  kernel / entry: names for the error messages
-template <typename Args>
+// A Box2D closed-loop rollout: per step, one launch of `policy` (linear_policy_kernel, mlp_policy_kernel,
+// mlp_noisy_policy_kernel) with the arguments args_at(t) from the observation rows of the step before (first_obs for
+// step 0), with `smem` bytes of dynamic shared memory, then launch_step_box2d into slice t.  Summary mode: every step
+// runs in one scratch slice, and the policy launch of step t + 1 (or one last launch, with args_at(T - 1)) folds step t
+// into the summary.  kernel / entry: names for the error messages
+template <typename Args, typename ArgsAt>
 static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
-                                       const float *first_obs, const Args &p,
+                                       const float *first_obs, const ArgsAt &args_at,
                                        void (*policy)(const float *, void *, const Args, const double *,
                                                       const uint8_t *, const uint8_t *, int64_t, int32_t, int, int),
                                        size_t smem, bool summary, cudaStream_t st, const char *kernel,
@@ -2702,14 +2742,15 @@ static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T,
             s.truncated = a.truncated + t * n;
             s.final_obs = a.final_obs ? a.final_obs + t * n * D : nullptr;
         }
-        policy<<<blocks, kThreads, smem, st>>>(obs_in, const_cast<void *>(s.actions), p, s.reward, s.terminated,
-                                               s.truncated, n, summary ? t - 1 : -1, 1, summary && t == 0);
+        policy<<<blocks, kThreads, smem, st>>>(obs_in, const_cast<void *>(s.actions), args_at(t), s.reward,
+                                               s.terminated, s.truncated, n, summary ? t - 1 : -1, 1,
+                                               summary && t == 0);
         if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: launch failed", kernel);
         else rc = launch_step_box2d(h, s, action_dtype, st);
     }
     if (!rc && summary) {
-        policy<<<blocks, kThreads, smem, st>>>(s.obs, nullptr, p, s.reward, s.terminated, s.truncated, n, T - 1, 0,
-                                               0);
+        policy<<<blocks, kThreads, smem, st>>>(s.obs, nullptr, args_at(T - 1), s.reward, s.terminated, s.truncated,
+                                               n, T - 1, 0, 0);
         if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: launch failed", kernel);
     }
     if (!rc && cudaMemcpyAsync(last_obs, s.obs, (size_t)n * D * sizeof(float), cudaMemcpyDeviceToDevice, st))
@@ -2728,8 +2769,8 @@ static int launch_rollout_linear_box2d(b200gym *h, const StepArgs &a, int32_t T,
     case B200GYM_LUNARLANDER_CONT: policy = linear_policy_kernel<2, 8, false>; break;
     default: policy = linear_policy_kernel<4, 24, false>; break;   // BipedalWalker(Hardcore)
     }
-    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, p, policy, 0, summary, st, "linear_policy_kernel",
-                                       "b200gym_rollout_linear");
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, [&](int32_t) { return p; }, policy, 0, summary,
+                                       st, "linear_policy_kernel", "b200gym_rollout_linear");
 }
 
 extern "C" int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env,
@@ -2790,7 +2831,7 @@ static int launch_rollout_mlp_kind(b200gym *h, const StepArgs &a, int32_t T, flo
 template <int K, int D, bool DISCRETE>
 static int launch_rollout_mlp_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
                                     const MlpPolicyArgs &p, bool per_env, size_t smem, bool summary, cudaStream_t st) {
-    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, p,
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, [&](int32_t) { return p; },
                                        per_env ? mlp_policy_kernel<K, D, DISCRETE, true>
                                                : mlp_policy_kernel<K, D, DISCRETE, false>,
                                        per_env ? 0 : smem, summary, st, "mlp_policy_kernel", "b200gym_rollout_mlp");
@@ -2846,6 +2887,86 @@ extern "C" int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int pe
     case B200GYM_BIPEDALWALKER:
     case B200GYM_BIPEDALWALKER_HARDCORE:
         return launch_rollout_mlp_box2d<4, 24, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+// ---- stochastic rollouts of a ReLU MLP policy (b200gym_rollout_mlp_noisy) ----
+template <int KIND>
+static int launch_rollout_mlp_noisy_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                         const MlpNoisyArgs &p, bool per_env, size_t smem, cudaStream_t st) {
+    const unsigned blocks = blocks_for(h->n);
+    if (per_env) rollout_mlp_noisy_kernel<KIND, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+    else rollout_mlp_noisy_kernel<KIND, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// The policy launch of step t reads noise slice t and writes outputs slice t
+template <int K, int D, bool DISCRETE>
+static int launch_rollout_mlp_noisy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                          const float *first_obs, const MlpNoisyArgs &p, bool per_env, size_t smem,
+                                          cudaStream_t st) {
+    const int64_t slice = h->n * K;
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs,
+                                       [&](int32_t t) {
+                                           MlpNoisyArgs q = p;
+                                           q.noise = p.noise + t * slice;
+                                           q.outputs = p.outputs + t * slice;
+                                           return q;
+                                       },
+                                       per_env ? mlp_noisy_policy_kernel<K, D, DISCRETE, true>
+                                               : mlp_noisy_policy_kernel<K, D, DISCRETE, false>,
+                                       per_env ? 0 : smem, false, st, "mlp_noisy_policy_kernel",
+                                       "b200gym_rollout_mlp_noisy");
+}
+
+extern "C" int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                         int h2, int32_t T, const float *noise_dev, float *outputs_dev,
+                                         void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                         uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                         float *last_obs_dev, const float *first_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout_mlp_noisy: null handle");
+    if (n_layers != 1 && n_layers != 2)
+        return fail(h, "b200gym_rollout_mlp_noisy: n_layers must be 1 or 2 (got %d)", n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "b200gym_rollout_mlp_noisy: hidden widths must be 1 .. %d (got %d, %d)", kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "b200gym_rollout_mlp_noisy: T must be at least 1 (got %d)", T);
+    if (!params_dev || !noise_dev || !outputs_dev || !actions_out_dev || !obs_dev || !reward_dev || !terminated_dev ||
+        !truncated_dev || !last_obs_dev)
+        return fail(h, "b200gym_rollout_mlp_noisy: null buffer");
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "b200gym_rollout_mlp_noisy: a Box2D env needs first_obs_dev");
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    // as b200gym_rollout_mlp
+    const bool vec = h1 % 4 == 0 && (!per_env || (P % 4 == 0 && reinterpret_cast<uintptr_t>(params_dev) % 16 == 0));
+    const MlpNoisyArgs p{{params_dev, per_env ? P : 0, h1, h2, vec ? 1 : 0, nullptr, nullptr, nullptr}, noise_dev,
+                         outputs_dev};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool pe = per_env != 0;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_noisy_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, p, pe, smem, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, p, pe, smem, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, p, pe, smem, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_noisy_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, p, pe, smem, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_noisy_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, p, pe, smem, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_noisy_box2d<4, 8, true>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_noisy_box2d<2, 8, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_noisy_box2d<4, 24, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
     }
     return fail(h, "bad kind %d", h->cfg.kind);
 }

@@ -695,6 +695,107 @@ __device__ __forceinline__ void rollout_mlp_env(const StepArgs &a, int64_t i, in
     }
 }
 
+// ---- stochastic rollouts of a ReLU MLP policy (b200gym_rollout_mlp_noisy) -----------------------------------------
+
+// A load of an input the rollout reads once and never again: evict-first on the device, where T steps of noise are far
+// larger than L2; a plain load in the host build
+template <typename T>
+__device__ __forceinline__ T load_once(const T *p) {
+#ifdef __CUDA_ARCH__
+    return __ldcs(p);
+#else
+    return *p;
+#endif
+}
+
+// The arguments of a b200gym_rollout_mlp_noisy launch: the policy (mlp; no summary, so its returns, lengths and ended
+// are null) and slice 0 of the [T][n][K] noise it reads and of the [T][n][K] outputs it writes
+struct MlpNoisyArgs {
+    MlpPolicyArgs mlp;
+    const float *noise;
+    float *outputs;
+};
+
+// y = z + noise[k] for the K outputs z of an MLP, one rounded float32 add each (IEEE: a NaN or infinite term follows
+// the sum), with z stored to out[0 .. K-1].  `noise` and `out` point at env i's row
+template <int K>
+__device__ __forceinline__ void noisy_outputs(const float (&z)[K], const float *noise, float *out, float (&y)[K]) {
+    float e[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) e[k] = load_once(noise + k);
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+        store_once(out + k, z[k]);
+        y[k] = z[k] + e[k];
+    }
+}
+
+// MlpNoisyActions: MlpActions with the caller's noise added to the outputs before the action is taken from them.  The
+// outputs z go to `outputs` and the action to the row of actions, both written once; noise and outputs point at row
+// t of their [T][n][K] arrays and move on by one row per step (next)
+template <int KIND, bool GLOBAL>
+struct MlpNoisyActions {
+    static constexpr int K = linear_logit_count<KIND>(), D = bgym::Env<KIND>::D;
+    const float *w;
+    int h1, h2;
+    bool vec;
+    const float (&o)[D];
+    const float *noise;
+    float *outputs;
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
+        float z[K], y[K];
+        mlp_outputs<K, D, GLOBAL>(w, h1, h2, vec, o, z);
+        noisy_outputs<K>(z, noise + i * K, outputs + i * K, y);
+        ActT v;
+        if constexpr (bgym::Env<KIND>::A == 0) v = (ActT)argmax_first<K>(y);
+        else v = y[0];
+        store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+    __device__ __forceinline__ void next(int64_t n) {
+        noise += n * K;
+        outputs += n * K;
+    }
+};
+
+// T steps of env i under its MLP policy at w with the caller's noise (rollout_mlp_noisy_kernel): rollout_mlp_env's
+// loop without the summary mode, written out again so that no pre-existing kernel changes, with MlpNoisyActions in
+// place of MlpActions
+template <int KIND, bool GLOBAL>
+__device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                      const float *w, const MlpNoisyArgs &p) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D];
+    E::observe(s, o);
+    MlpNoisyActions<KIND, GLOBAL> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, p.noise, p.outputs};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, false> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                 o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        src.next(n);
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the
 // observation row.  References as in lunar_reset_env.
 template <int KIND>

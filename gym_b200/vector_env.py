@@ -687,18 +687,84 @@ class B200VectorEnv:
             self._lib.b200gym_rollout_mlp(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T,
                                           *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
 
-    def _policy_rollout(self, what, T, summary, captured, launch):
-        """The checks after the parameters', the outputs, and the call of rollout_linear() / rollout_mlp(), whose
-        entry point ``launch(T, outs, last, first)`` calls with the output pointers, the buffer that receives the last
-        observations and the observations the env last returned."""
-        if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
-            raise ValueError(f"{what}(T) needs an integer 1 <= T < 2**31, got {T!r}")
-        T = int(T)
+    def rollout_mlp_noisy(self, params, hidden, noise):
+        """T steps of a stochastic ReLU MLP policy in closed loop, T = ``noise.shape[0]`` -> ``(actions, outputs, obs,
+        rewards, terminateds, truncateds, infos)``: bit for bit what
+        ``for t in range(T): z = mlp(obs); a = rule(z + noise[t]); obs, r, te, tr, info = self.step(a)`` returns,
+        stacked, with ``obs`` starting at the observation the env last returned, and the env left where that loop
+        leaves it.
+
+        ``params`` and ``hidden`` are ``rollout_mlp()``'s, and z is its K outputs.  ``noise`` is float32 (T, N, K),
+        contiguous, on the env's device, 1 <= T < 2**31, with K = ``single_action_space.n`` (Discrete) or ``act_dim``
+        (Box).  Each ``z[k] + noise[t, i, k]`` is one rounded float32 add, IEEE NaN and infinity included; ``rule`` is
+        ``np.argmax`` (the first NaN, else the first maximum) for Discrete kinds and the identity, unclipped, for Box
+        kinds.  ``outputs`` is float32 (T, N, K), z before the noise; the other six are ``rollout_mlp()``'s.
+
+        The sampling distribution is the noise's.  Gumbel noise makes the Discrete action an exact sample of
+        ``softmax(outputs)``, so the log-probabilities of the actions come from ``outputs`` afterwards::
+
+            u = torch.rand(T, N, K, device=dev).clamp_(min=torch.finfo(torch.float32).tiny)
+            g = -torch.log(-torch.log(u))
+            a, logits, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), g)
+            logp = torch.distributions.Categorical(logits=logits).log_prob(a)
+
+        and scaled normal noise makes the Box action a sample of N(outputs, std**2)::
+
+            std = log_std.exp()
+            eps = torch.randn(T, N, K, device=dev)
+            a, mean, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), std * eps)
+            logp = torch.distributions.Normal(mean, std).log_prob(a).sum(-1)
+
+        Noise of -0.0 everywhere gives ``rollout_mlp()``'s actions (+0.0 would turn a -0.0 Box output into +0.0).
+        Guards and the start from the current state are ``rollout_linear()``'s.  The classic-control kinds may be
+        captured in a CUDA graph, and replays read the current contents of ``params`` and ``noise``, so filling the
+        noise and rolling out can be one graph; the Box2D kinds cannot (DESIGN.md §4.14)."""
+        captured = self._rollout_guards("rollout_mlp_noisy")
+        h1, h2, per_env = self._mlp_params(params, hidden, "rollout_mlp_noisy")
+        T = self._noise_steps(noise)
+        self._refuse_box2d_capture("rollout_mlp_noisy")
+        outputs = _torch().empty_like(noise)
+        vp = ctypes.c_void_p
+        actions, obs, reward, term, trunc, infos = self._policy_rollout(
+            "rollout_mlp_noisy", T, False, captured, lambda T, outs, last, first: (
+                self._lib.b200gym_rollout_mlp_noisy(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1,
+                                                    h2, T, vp(noise.data_ptr()), vp(outputs.data_ptr()), *outs[:6],
+                                                    vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+        return actions, outputs, obs, reward, term, trunc, infos
+
+    def _noise_steps(self, noise):
+        """Check rollout_mlp_noisy()'s noise without a CUDA call -> T."""
+        torch = _torch()
+        K = int(self.single_action_space.n if self.discrete else self.act_dim)
+        if not isinstance(noise, torch.Tensor):
+            raise ValueError(f"rollout_mlp_noisy() needs noise as a torch tensor, got {type(noise).__name__}")
+        if noise.dtype != torch.float32:
+            raise ValueError(f"rollout_mlp_noisy() needs float32 noise, got {noise.dtype}")
+        if noise.device != self.device:
+            raise ValueError(f"rollout_mlp_noisy() needs noise on {self.device}, got {noise.device}")
+        if not noise.is_contiguous():
+            raise ValueError("rollout_mlp_noisy() needs contiguous noise")
+        if noise.dim() != 3 or tuple(noise.shape[1:]) != (self.num_envs, K) or not 1 <= noise.shape[0] <= 2 ** 31 - 1:
+            raise ValueError(f"rollout_mlp_noisy() needs noise (T, {self.num_envs}, {K}) with 1 <= T < 2**31, got "
+                             f"{tuple(noise.shape)}")
+        return int(noise.shape[0])
+
+    def _refuse_box2d_capture(self, what):
+        """Raise if a Box2D env's policy rollout is being captured."""
         if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
                          _lib.KIND_BIPEDALWALKER_HARDCORE):
             refuse_capture(f"{what}() of a Box2D env", "its step 0 reads the observation rows the env last "
                            "returned, which alternate between two buffers from call to call, so a replay would read a "
                            "stale set")
+
+    def _policy_rollout(self, what, T, summary, captured, launch):
+        """The checks after the parameters', the outputs, and the call of rollout_linear() / rollout_mlp() /
+        rollout_mlp_noisy(), whose entry point ``launch(T, outs, last, first)`` calls with the output pointers, the
+        buffer that receives the last observations and the observations the env last returned."""
+        if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
+            raise ValueError(f"{what}(T) needs an integer 1 <= T < 2**31, got {T!r}")
+        T = int(T)
+        self._refuse_box2d_capture(what)
         first = self._out[self._flip]["obs"]   # the observations the env last returned, before the flip below
         torch = _torch()
         n, dev, vp = self.num_envs, self.device, ctypes.c_void_p
@@ -742,34 +808,35 @@ class B200VectorEnv:
                              f"{tuple(bias.shape)}")
         return per_env
 
-    def _mlp_params(self, params, hidden):
-        """Check rollout_mlp()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden layer), per_env)."""
+    def _mlp_params(self, params, hidden, what="rollout_mlp"):
+        """Check rollout_mlp()'s or rollout_mlp_noisy()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden
+        layer), per_env)."""
         torch = _torch()
         if not isinstance(hidden, (tuple, list)) or not 1 <= len(hidden) <= 2 or any(
                 isinstance(h, (bool, np.bool_)) or not isinstance(h, (int, np.integer)) or not 1 <= int(h) <= 64
                 for h in hidden):
-            raise ValueError(f"rollout_mlp() needs hidden as a tuple of one or two widths, each 1 .. 64, got {hidden!r}")
+            raise ValueError(f"{what}() needs hidden as a tuple of one or two widths, each 1 .. 64, got {hidden!r}")
         widths = [int(h) for h in hidden]
         K = self.single_action_space.n if self.discrete else self.act_dim
         sizes = [self.obs_dim] + widths + [int(K)]
         P = sum(o * i + o for i, o in zip(sizes[:-1], sizes[1:]))
         if not isinstance(params, torch.Tensor):
-            raise ValueError(f"rollout_mlp() needs params as a torch tensor, got {type(params).__name__}")
+            raise ValueError(f"{what}() needs params as a torch tensor, got {type(params).__name__}")
         if params.dtype != torch.float32:
-            raise ValueError(f"rollout_mlp() needs float32 params, got {params.dtype}")
+            raise ValueError(f"{what}() needs float32 params, got {params.dtype}")
         if params.device != self.device:
-            raise ValueError(f"rollout_mlp() needs params on {self.device}, got {params.device}")
+            raise ValueError(f"{what}() needs params on {self.device}, got {params.device}")
         if not params.is_contiguous():
-            raise ValueError("rollout_mlp() needs contiguous params")
+            raise ValueError(f"{what}() needs contiguous params")
         per_env = tuple(params.shape) == (self.num_envs, P)
         if not (per_env or tuple(params.shape) == (P,)):
-            raise ValueError(f"rollout_mlp() with hidden {tuple(widths)} needs params ({P},) for one policy or "
+            raise ValueError(f"{what}() with hidden {tuple(widths)} needs params ({P},) for one policy or "
                              f"({self.num_envs}, {P}) for one per env; got {tuple(params.shape)}")
         return widths[0], widths[1] if len(widths) == 2 else 0, per_env
 
     def _rollout_guards(self, what):
-        """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp(), all raised before any CUDA
-        call -> whether a CUDA graph is being captured."""
+        """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp() / rollout_mlp_noisy(), all
+        raised before any CUDA call -> whether a CUDA graph is being captured."""
         self._assert_open(what)
         if self.backend == "numpy":
             raise error.Error(f"{what}() needs backend='torch': backend='numpy' steps through host buffers")

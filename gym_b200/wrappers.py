@@ -76,6 +76,13 @@ class VectorWrapper:
                           "fused rollout of the wrapped env would skip it; call step() with the policy's actions T "
                           "times instead")
 
+    def rollout_mlp_noisy(self, params, hidden, noise):
+        """Refused, as rollout(): step the wrapper with the policy's actions instead."""
+        from gym_b200 import error
+        raise error.Error(f"{type(self).__name__} does not support rollout_mlp_noisy(): it acts after every step, and "
+                          "a fused rollout of the wrapped env would skip it; call step() with the policy's actions T "
+                          "times instead")
+
     def close(self, **kwargs):
         return self.env.close(**kwargs)
 

@@ -253,6 +253,26 @@ int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int per_env, int 
                         uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
                         uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
 
+/*
+ * b200gym_rollout_mlp with the caller's noise added to the MLP's outputs before the action is taken from them: at step
+ * t env i's outputs z[0 .. K-1] (b200gym_rollout_mlp's arithmetic) become y[k] = z[k] + noise[t][i][k], one rounded
+ * float32 add each, and the action is the first index of a NaN, else of the first maximum, of y (Discrete kinds) or y
+ * itself, unclipped (Box kinds).  Noise -log(-log(U)) makes the Discrete action an exact sample of softmax(z)
+ * (Gumbel-max); noise std * N(0, 1) makes the Box action a sample of N(z, std^2).
+ *   params_dev ... h2  as b200gym_rollout_mlp
+ *   T                  number of steps, >= 1
+ *   noise_dev          float32 [T][n][K] on the handle's device, read by the launch (a captured call reads its current
+ *                      contents at every replay)
+ *   outputs_dev        float32 [T][n][K]: receives z of every step, before the noise
+ *   actions_out_dev ... first_obs_dev  as b200gym_rollout_mlp without the summary mode: the per-step outputs are
+ *                      required
+ * Classic-control kinds: ONE launch.  Box2D kinds: per step, one policy launch and the b200gym_step sequence.
+ */
+int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                              int32_t T, const float *noise_dev, float *outputs_dev, void *actions_out_dev,
+                              float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                              float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
