@@ -207,8 +207,8 @@ struct StagedSink {
 };
 
 // kernel B: every row that the tile's bulk stores cover is written into the tile's stage -- the new state and
-// TimeLimit counter in place over the inputs, so that a row nobody writes (an invalid action, an env left for the
-// deferred reset) goes back to HBM unchanged.  The final observation is only handed back (`fin`, a register array
+// TimeLimit counter in place over the inputs, so that a row nobody writes (an invalid action) goes back to HBM
+// unchanged.  The final observation is only handed back (`fin`, a register array
 // of the calling thread): the kernel stores it after the warp has released the stage, so that no global store is
 // outstanding at the warp's proxy fence
 struct InPlaceSink {
@@ -498,14 +498,10 @@ __device__ __forceinline__ void st_bulk(void *gmem_dst, const void *smem_src, ui
 }
 __device__ __forceinline__ void st_bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void st_bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// ... until every bulk group of this thread but the most recent one is COMPLETE
-__device__ __forceinline__ void st_bulk_wait_prev() { asm volatile("cp.async.bulk.wait_group 1;" ::: "memory"); }
 // ... until the bulk copies of this thread are COMPLETE (their writes performed), not just their source read
 __device__ __forceinline__ void st_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // generic-proxy writes to shared memory -> visible to the async proxy that executes the bulk copy
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// completed bulk-copy writes to global memory -> ordered before the generic-proxy stores that follow
-__device__ __forceinline__ void fence_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // mbarrier in shared memory: `count` arrivals plus the transaction bytes announced by expect_tx complete a phase
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
@@ -656,43 +652,40 @@ __global__ void __launch_bounds__(kThreads, Tuning<KIND>::kMinCtas) step_kernel_
 // stage's output block: InPlaceSink), fence the writes to the async proxy and arrive on the stage's `done`
 // mbarrier; the copy thread then pushes the whole tile out with S + 5 bulk stores and, once they have read the
 // stage, refills it with the tile kBulkStages rounds ahead.  So the compute warps execute only shared-memory loads and
-// stores on the common path.  Dense warps reset inline (through the stage).  The other finishing envs are reset with
-// direct stores, which must land after the tile's bulk store of the same rows.  When a CTA walks few tiles (the
-// 2^20-env step), each thread resets its env two tiles later: after issuing a tile's refill the copy thread waits
-// until the previous tile's bulk stores have COMPLETED and releases its rows on the stage's `stored` mbarrier, and the
-// compute warps do the reset while the next stage may still be in flight.  Otherwise, as in kernel P, the envs go onto
-// the CTA's list, drained once after every bulk store of the CTA has completed; so are the last two tiles' in-loop
-// resets.  The drain after the loop is a fixed cost per launch (about 10 us for ~90 resets a CTA at 2^20 on H100):
-// that is what the in-loop resets take off the short launches.
+// stores on the common path.  Every finishing env is reset inside the stage, before the warp's `done` arrive, so a
+// CTA is finished with a tile once its bulk stores have been issued.  The reset's one global load is the env's
+// 32-byte PCG64 record.  Where the kind can tell from a tile's inputs which envs will finish (will_reset: CartPole),
+// the record is requested into L2 as soon as the warp has read its inputs, so that it arrives while the float64 step
+// runs.  An env that resets without having been predicted loads its record then; correctness never depends on the
+// prediction.
 // Whole tiles only, every row 16-byte aligned (launch_step_typed checks), 32-bit env indices.
 constexpr int kBulkStages = 3;   // 2 stages at 5 CTAs/SM measured slower (DESIGN §4.1)
-constexpr int kBulkResetCap = 2 * kThreads;   // >= the in-loop mode's 2 deferred resets per compute thread; list mode:
-                                              // ~11 finishing envs per tile, so ~45 tiles before the list is full
-constexpr int kBulkInLoopResetTiles = 16;     // CartPole, H100: in-loop resets faster at 8 tiles per CTA (2^20 envs),
-                                              // the list at 62 (2^23 envs)
 
 // Phase clocks of kernel B (-DB200_PHASE_CLOCKS, scripts/cartpole_phases.py; the default build compiles none of it).
 // Lane 0 of every compute warp and the copy thread add clock() cycles per phase into g_phase_cycles; every CTA
-// stamps %globaltimer at its start, when its last compute warp leaves the loop, and at the start and end of the reset
-// drain.  b200gym_phase_clocks reads (and clears) both.
+// stamps %globaltimer at its start, when its last compute warp leaves the loop, and when its copy thread exits.
+// b200gym_phase_clocks reads (and clears) both.
 #ifdef B200_PHASE_CLOCKS
 enum PhaseBucket {
-    kPhFull, kPhAdvance, kPhReset, kPhArrive, kPhComputeLoop, kPhComputeTiles,   // compute warps (lane 0)
-    kPhDone, kPhStore, kPhWaitRead, kPhLoad, kPhWaitAll, kPhCopyLoop, kPhWaitPrev,   // copy thread
-    kPhStoredWait,                                                              // compute warps (part of kPhReset)
+    kPhFull, kPhAdvance, kPhRecord, kPhReset, kPhArrive, kPhComputeLoop, kPhComputeTiles,   // compute warps (lane 0)
+    kPhDone, kPhStore, kPhWaitRead, kPhLoad, kPhFinalWait, kPhCopyLoop,                         // copy thread
     kPhBuckets
 };
 constexpr int kPhMaxCtas = 4096;
 __device__ unsigned long long g_phase_cycles[kPhBuckets];
-__device__ unsigned long long g_phase_ns[kPhMaxCtas][4];   // start, loop end, drain start, drain end
+__device__ unsigned long long g_phase_ns[kPhMaxCtas][3];   // start, loop end, exit
 // 32-bit clocks (differences are exact modulo 2^32) and per-warp sums in shared memory: the instrumented loop
 // keeps no extra 64-bit registers live, so it runs with the registers of the default build
 #define PH_CLOCK(t) const unsigned t = (unsigned)clock()
 #define PH_DECL()                                                                              \
     __shared__ unsigned ph_s[kThreads / 32 + 1][kPhBuckets];                                  \
+    __shared__ unsigned ph_zero;                                                               \
     for (int b_ = threadIdx.x; b_ < (kThreads / 32 + 1) * kPhBuckets; b_ += blockDim.x) (&ph_s[0][0])[b_] = 0u
 #define PH_ACC(b, t0, t1) \
     do { if ((threadIdx.x & 31) == 0) ph_s[threadIdx.x >> 5][b] += (t1) - (t0); } while (0)
+// an instruction that reads v, so that a clock read after it comes after v's load has completed
+#define PH_USE(v) \
+    do { if ((v) == 0ull) ph_zero = 1u; } while (0)
 #define PH_FLUSH()                                                                             \
     do {                                                                                       \
         if (threadIdx.x < kPhBuckets) {                                                        \
@@ -711,7 +704,7 @@ extern "C" int b200gym_phase_clocks(unsigned long long *cycles, unsigned long lo
     if (cudaMemcpyFromSymbol(ns, g_phase_ns, sizeof g_phase_ns) != cudaSuccess) return 1;
     if (clear) {
         static const unsigned long long zc[kPhBuckets] = {};
-        static unsigned long long zn[kPhMaxCtas][4] = {};
+        static unsigned long long zn[kPhMaxCtas][3] = {};
         if (cudaMemcpyToSymbol(g_phase_cycles, zc, sizeof zc) != cudaSuccess) return 1;
         if (cudaMemcpyToSymbol(g_phase_ns, zn, sizeof zn) != cudaSuccess) return 1;
     }
@@ -721,6 +714,7 @@ extern "C" int b200gym_phase_clocks(unsigned long long *cycles, unsigned long lo
 #define PH_CLOCK(t)
 #define PH_DECL()
 #define PH_ACC(b, t0, t1)
+#define PH_USE(v)
 #define PH_FLUSH()
 #define PH_STAMP(slot)
 #define PH_STAMP_MAX(slot)
@@ -748,30 +742,20 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
     using E = Env<KIND>;
     using L = BulkLayout<KIND, ActT>;
     extern __shared__ __align__(128) unsigned char stage_mem[];   // [kBulkStages][L::kBytes]
-    // per stage: full = its inputs have landed, done = the compute warps are through with it, stored = the bulk
-    // stores of the tile it last held have COMPLETED (direct stores to that tile's rows may follow)
-    __shared__ __align__(8) uint64_t full[kBulkStages], done[kBulkStages], stored[kBulkStages];
-    __shared__ int reset_list[kBulkResetCap];
-    __shared__ int reset_count;
+    // per stage: full = its inputs have landed, done = the compute warps are through with it
+    __shared__ __align__(8) uint64_t full[kBulkStages], done[kBulkStages];
     const int tid = threadIdx.x;
     PH_DECL();
     if (tid == 0) {
         PH_STAMP(0);
-        reset_count = 0;
         for (int q = 0; q < kBulkStages; q++) {
             acp::mbar_init(&full[q], 1);
             acp::mbar_init(&done[q], kThreads / 32);
-            acp::mbar_init(&stored[q], 1);
         }
         acp::fence_mbar_init();
     }
     __syncthreads();
     const uint32_t first = (uint32_t)a.first, n = (uint32_t)a.n;
-    const DirectSinkT<false> direct{a};
-    // where the autoresets of non-dense warps go (DESIGN §4.1): a CTA that walks few tiles resets them inside the
-    // loop, two tiles later, so that its drain after the loop is short; one that walks many tiles lists them and
-    // drains the list once, after the loop, where its cost is spread over all its tiles
-    const bool in_loop_resets = (num_tiles + (int)gridDim.x - 1) / (int)gridDim.x <= kBulkInLoopResetTiles;
 
     if (tid >= kThreads) {
         if (tid == kThreads) {   // the copy thread
@@ -802,7 +786,6 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
             for (int t = blockIdx.x; q < kBulkStages && t < num_tiles; t += gridDim.x) load(t, q++);
             q = 0;
             uint32_t parity = 0;
-            int prev_q = -1;
             PH_CLOCK(c_begin);
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 PH_CLOCK(c0);
@@ -812,18 +795,6 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
                 PH_CLOCK(c2);
                 PH_ACC(kPhDone, c0, c1);
                 PH_ACC(kPhStore, c1, c2);
-                if (in_loop_resets && prev_q >= 0) {
-                    // the previous tile's stores were issued a tile ago and have normally completed: release its rows
-                    // to the deferred resets.  Released before the refill below is issued, so that no compute warp
-                    // can reach a `stored` wait while the barrier's previous phase is still open (a parity wait
-                    // would then pass at once)
-                    PH_CLOCK(c5);
-                    acp::st_bulk_wait_prev();
-                    acp::fence_async_global();
-                    acp::mbar_arrive(&stored[prev_q]);
-                    PH_CLOCK(c6);
-                    PH_ACC(kPhWaitPrev, c5, c6);
-                }
                 const int next = tile + kBulkStages * (int)gridDim.x;
                 if (next < num_tiles) {
                     // the stage is free once the stores have READ it (a few hundred ns); waiting right away keeps
@@ -835,50 +806,31 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
                     PH_ACC(kPhWaitRead, c2, c3);
                     PH_ACC(kPhLoad, c3, c4);
                 }
-                prev_q = q;
                 if (++q == kBulkStages) { q = 0; parity ^= 1u; }
             }
             PH_CLOCK(c_end);
-            acp::st_bulk_wait_all();     // the drain below overwrites rows of these stores
-            acp::fence_async_global();
+            acp::st_bulk_wait_read();    // the stages must outlive the stores that read them
             PH_CLOCK(c_drained);
             PH_ACC(kPhCopyLoop, c_begin, c_end);
-            PH_ACC(kPhWaitAll, c_end, c_drained);
+            PH_ACC(kPhFinalWait, c_end, c_drained);
         }
     } else {
         const int lane = tid & 31;
         int q = 0;
         uint32_t parity = 0;
-        // in-loop resets: this thread's env in the tile before last / the last tile, if it waits for its reset (offset
-        // from `first`, else -1)
-        int pend2 = -1, pend1 = -1;
         PH_CLOCK(w_begin);
-        for (int tile = blockIdx.x, walked = 0; tile < num_tiles; tile += gridDim.x, walked++) {
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             PH_CLOCK(w0);
-            // the resets deferred two tiles ago, while the next stage may still be in flight: that tile's bulk
-            // stores have completed once the copy thread has released its stage's `stored` phase
-            if (__any_sync(0xffffffffu, pend2 >= 0)) {
-                const int u = walked - 2;
-                PH_CLOCK(s0);
-                acp::mbar_wait(&stored[u % kBulkStages], (uint32_t)(u / kBulkStages) & 1u);
-                PH_CLOCK(s1);
-                PH_ACC(kPhStoredWait, s0, s1);
-                if (pend2 >= 0) reset_env<KIND>(a, direct, first + (uint32_t)pend2);
-            }
-            pend2 = pend1;
-            pend1 = -1;
             unsigned char *b = stage_mem + q * L::kBytes;
-            const uint32_t j = (uint32_t)tile * kThreads + tid;
-            const uint32_t i = first + j;
+            const uint32_t i = first + (uint32_t)tile * kThreads + tid;
+            uint64_t *const rec = a.rng + 4 * (size_t)i;
             float fin[E::D];
             const InPlaceSink sink{reinterpret_cast<double *>(b + L::kStateOff), reinterpret_cast<int32_t *>(b + L::kElapsedOff),
                                    reinterpret_cast<float *>(b + L::kObsOff), reinterpret_cast<double *>(b + L::kRewardOff),
                                    b + L::kTermOff, b + L::kTruncOff, i - tid, fin};
-            PH_CLOCK(wd);
-            PH_ACC(kPhReset, w0, wd);
             acp::mbar_wait(&full[q], parity);
             PH_CLOCK(w1);
-            PH_ACC(kPhFull, wd, w1);
+            PH_ACC(kPhFull, w0, w1);
             double s[E::S];
 #pragma unroll
             for (int k = 0; k < E::S; k++) s[k] = sink.s_state[k * kThreads + tid];
@@ -887,52 +839,41 @@ __global__ void __launch_bounds__(kThreads + 32, Tuning<KIND>::kBulkMinCtas)
             long long action_int = 0;
             float a0 = 0.0f;
             decode_action<KIND>(av, action_int, a0);
+            if (will_reset<KIND>(a, s, elapsed, action_int)) asm volatile("prefetch.global.L2 [%0];" ::"l"(rec));
             const bool need = advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0);
-            const unsigned m = __ballot_sync(0xffffffffu, need);
             PH_CLOCK(w2);
             PH_ACC(kPhAdvance, w1, w2);
-            bool deferred = false;
+            // the reset through the stage; the record's write-back, like the final observation, waits until the
+            // stage is released, so that no global store is outstanding at the proxy fence
+            bgym::Pcg64 g;
             if (need) {
-                bool inline_reset = __popc(m) >= 12;   // dense enough: reset right here, through the stage
-                if (!inline_reset) {
-                    if (in_loop_resets) pend1 = (int)j;
-                    else {
-                        const int slot = atomicAdd(&reset_count, 1);
-                        if (slot < kBulkResetCap) reset_list[slot] = (int)j;
-                        else inline_reset = true;   // list full (whole batch truncating at once)
-                    }
-                    deferred = !inline_reset;
-                }
-                if (inline_reset) reset_env<KIND>(a, sink, i);
+                g = bgym::pcg64_load(rec);
+                PH_USE((uint64_t)g.state);
             }
             PH_CLOCK(w3);
-            PH_ACC(kPhReset, w2, w3);
+            PH_ACC(kPhRecord, w2, w3);
+            if (need) reset_env_from<KIND>(sink, i, g);
+            PH_CLOCK(w4);
+            PH_ACC(kPhReset, w3, w4);
             acp::fence_async_smem();
             __syncwarp();
             if (lane == 0) acp::mbar_arrive(&done[q]);
-            PH_CLOCK(w4);
-            // the lanes' global traffic comes after the stage is released: the final observation, and the PCG64
-            // record that the deferred reset starts with, fetched into L2 by then
-            if (need && a.final_obs) store_row<E::D>(a.final_obs, i, fin);
-            if (deferred) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.rng + 4 * (size_t)i));
-            PH_ACC(kPhArrive, w3, w4);
+            if (need) {
+                if (a.final_obs) store_row<E::D>(a.final_obs, i, fin);
+                bgym::pcg64_store(rec, g);
+            }
+            PH_CLOCK(w5);
+            PH_ACC(kPhArrive, w4, w5);
             PH_ACC(kPhComputeTiles, 0, 1);
             if (++q == kBulkStages) { q = 0; parity ^= 1u; }
         }
         PH_CLOCK(w_end);
         PH_ACC(kPhComputeLoop, w_begin, w_end);
         if (lane == 0) PH_STAMP_MAX(1);
-        // the last two tiles' in-loop resets wait for every bulk store of the CTA to complete, with the list's
-        if (pend2 >= 0) reset_list[atomicAdd(&reset_count, 1)] = pend2;
-        if (pend1 >= 0) reset_list[atomicAdd(&reset_count, 1)] = pend1;
     }
-    __syncthreads();
-    if (tid == 0) PH_STAMP(2);
-    const int cnt = min(reset_count, kBulkResetCap);
-    for (int q = tid; q < cnt; q += kThreads + 32) reset_env<KIND>(a, direct, first + (uint32_t)reset_list[q]);
 #ifdef B200_PHASE_CLOCKS
     __syncthreads();
-    if (tid == 0) PH_STAMP(3);
+    if (tid == 0) PH_STAMP(2);
     PH_FLUSH();
 #endif
 }

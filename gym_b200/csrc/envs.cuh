@@ -139,6 +139,24 @@ struct Env<B200GYM_CARTPOLE> {
         for (int k = 0; k < 4; k++) obs[k] = (float)s[k];
     }
 
+    // x and theta after one Euler step (cartpole.py:150, :152) and the termination test on them (:162-167).  Neither
+    // depends on the action, so whether a state terminates on its next step is known before the step runs
+    // (will_terminate); step() computes `terminated` through the same two functions, so the two always agree
+    __device__ static void next_x_theta(const double (&s)[S], double &x, double &theta) {
+        const double tau = kCartPole[6];
+        x = s[0] + tau * s[1];
+        theta = s[2] + tau * s[3];
+    }
+    __device__ static bool out_of_bounds(double x, double theta) {
+        const double theta_threshold = kCartPole[7], x_threshold = kCartPole[8];
+        return (x < -x_threshold) || (x > x_threshold) || (theta < -theta_threshold) || (theta > theta_threshold);
+    }
+    __device__ static bool will_terminate(const double (&s)[S]) {
+        double x, theta;
+        next_x_theta(s, x, theta);
+        return out_of_bounds(x, theta);
+    }
+
     // cartpole.py:130-188, "euler" integrator (:149-153)
     __device__ static void step(double (&s)[S], bool /*fresh*/, int action, float /*a0*/,
                                 double /*param0*/, float (&obs)[D], double &reward, bool &terminated) {
@@ -147,10 +165,8 @@ struct Env<B200GYM_CARTPOLE> {
         const double length = kCartPole[3];                                  // :94
         const double polemass_length = kCartPole[4];                         // :95  masspole * length
         const double force_mag = kCartPole[5], tau = kCartPole[6];           // :96-97
-        const double theta_threshold = kCartPole[7];                         // :101 12 * 2 * pi / 360
-        const double x_threshold = kCartPole[8];                             // :102
 
-        double x = s[0], x_dot = s[1], theta = s[2], theta_dot = s[3];
+        double x_dot = s[1], theta = s[2], theta_dot = s[3];
         const double force = (action == 1) ? force_mag : -force_mag;         // :135
         double sintheta, costheta;
         sincos_small(theta, sintheta, costheta);                             // :136-137
@@ -163,13 +179,12 @@ struct Env<B200GYM_CARTPOLE> {
                                                 inv_total_mass)));                         // :144-146
         const double xacc = temp - div_by_const(polemass_length * thetaacc * costheta, total_mass,
                                                 inv_total_mass);                           // :147
-        x = x + tau * x_dot;                                                 // :150
+        double x;
+        next_x_theta(s, x, theta);                                           // :150, :152
         x_dot = x_dot + tau * xacc;                                          // :151
-        theta = theta + tau * theta_dot;                                     // :152
         theta_dot = theta_dot + tau * thetaacc;                              // :153
         s[0] = x; s[1] = x_dot; s[2] = theta; s[3] = theta_dot;              // :160
-        terminated = (x < -x_threshold) || (x > x_threshold) ||
-                     (theta < -theta_threshold) || (theta > theta_threshold);  // :162-167
+        terminated = out_of_bounds(x, theta);                                // :162-167
         reward = 1.0;                                                        // :169-174
         obs[0] = (float)x; obs[1] = (float)x_dot; obs[2] = (float)theta; obs[3] = (float)theta_dot;  // :188
     }

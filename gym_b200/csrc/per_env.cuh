@@ -204,21 +204,42 @@ __device__ __forceinline__ bool advance_env(const StepArgs &a, const Sink &sink,
     return needs_reset;
 }
 
+// Whether advance_env will return true for these inputs, known before it runs: kernel B uses it to fetch the PCG64
+// records of a tile's finishing envs early.  Only CartPole's termination can be seen ahead (Env::will_terminate); the
+// other kinds answer false.  A kernel must not depend on the answer for correctness
+template <int KIND>
+__device__ __forceinline__ bool will_reset(const StepArgs &a, const double (&s)[bgym::Env<KIND>::S], int32_t elapsed,
+                                           long long action_int) {
+    using E = bgym::Env<KIND>;
+    if constexpr (KIND == B200GYM_CARTPOLE) {
+        if (!a.autoreset || action_int < 0 || action_int >= E::NACT) return false;
+        return ((a.max_steps > 0) && (elapsed + 1 >= a.max_steps)) || E::will_terminate(s);
+    } else {
+        return false;
+    }
+}
+
 // Phase 2: the unseeded env.reset() of the autoreset (sync_vector_env.py:154) for env i, by
-// whichever thread picked it off the CTA's compacted list.
+// whichever thread picked it off the CTA's compacted list.  reset_env_from: the same with env i's PCG64 record
+// loaded and written back by the caller
 template <int KIND, typename Sink, typename I>
-__device__ __forceinline__ void reset_env(const StepArgs &a, const Sink &sink, I i) {
+__device__ __forceinline__ void reset_env_from(const Sink &sink, I i, bgym::Pcg64 &g) {
     using E = bgym::Env<KIND>;
     double s[E::S];
     float obs[E::D];
-    bgym::Pcg64 g = bgym::pcg64_load(a.rng + 4 * (size_t)i);
     double lo, hi;
     E::default_bounds(lo, hi);
     E::reset(s, g, lo, hi, obs);
-    bgym::pcg64_store(a.rng + 4 * (size_t)i, g);
     sink.template state<E::S>(i, s);
     sink.elapsed(i, 0);                                                  // time_limit.py:67
     sink.template obs<E::D>(i, obs);
+}
+
+template <int KIND, typename Sink, typename I>
+__device__ __forceinline__ void reset_env(const StepArgs &a, const Sink &sink, I i) {
+    bgym::Pcg64 g = bgym::pcg64_load(a.rng + 4 * (size_t)i);
+    reset_env_from<KIND>(sink, i, g);
+    bgym::pcg64_store(a.rng + 4 * (size_t)i, g);
 }
 
 // ---- rollouts (b200gym_rollout) ---------------------------------------------------------------------------------

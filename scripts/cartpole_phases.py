@@ -1,14 +1,14 @@
 """Where kernel B's time per tile goes: the CartPole step kernel (step_kernel_persistent_bulk) built with
 -DB200_PHASE_CLOCKS, which adds up clock() cycles per phase.
 
-Compute warps (lane 0 of each): waiting on the stage's `full` barrier, advance_env (inputs from the stage, dynamics,
-TimeLimit, results into the stage), reset handling (inline resets, list pushes, and the in-loop resets of the tile
-before last, including `stored_wait` for that tile's bulk stores to complete), and the proxy fence + `done` arrive.
-The copy thread: waiting on `done`, issuing the tile's bulk stores, waiting until they have read the stage, issuing
-the refill's bulk loads, waiting for the previous tile's stores to complete (in-loop resets only), and the final wait
-for every store to complete.  Every CTA also stamps %globaltimer when its last compute warp leaves the loop, and at
-the start and end of the reset drain, relative to the CTA's start.  The instrumented build of one action width's
-kernel spills 4 bytes; the default build spills none.
+Compute warps (lane 0 of each): waiting on the stage's `full` barrier, advance_env (inputs from the stage, the
+lookahead's record prefetch, dynamics, TimeLimit, results into the stage), waiting for the PCG64 records of the
+finishing envs (`record_wait`), the resets through the stage (`reset`), and the proxy fence + `done` arrive with the
+final-observation and record stores after it.  The copy thread: waiting on `done`,
+issuing the tile's bulk stores, waiting until they have read the stage, issuing the refill's bulk loads, and the final
+wait until the last stores have read their stage.  Every CTA also stamps %globaltimer when its last compute warp
+leaves the loop and when the CTA exits, relative to the CTA's start.  The instrumented build spills 8 to 16 bytes;
+the default build spills none.
 
 Builds the variant into a temporary directory (or takes --lib) and loads it through B200GYM_LIB.  Prints one JSON
 line per shape: bench.py's (2^20 envs, L2 flushed before every step, median over steps) and 2^23 envs stepped back to
@@ -26,9 +26,10 @@ sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
 
-COMPUTE = ["full_wait", "advance_env", "reset", "fence_arrive"]
-COPY = ["done_wait", "store_issue", "wait_read", "load_issue", "final_wait_all"]
-N_BUCKETS = 14   # enum PhaseBucket in csrc/b200gym.cu
+COMPUTE = ["full_wait", "advance_env", "record_wait", "reset", "fence_arrive"]
+COPY = ["done_wait", "store_issue", "wait_read", "load_issue", "final_wait_read"]
+N_BUCKETS = 13   # enum PhaseBucket in csrc/b200gym.cu
+N_STAMPS = 3     # g_phase_ns: CTA start, loop end, exit
 MAX_CTAS = 4096
 
 
@@ -36,35 +37,33 @@ def build_variant(out_dir):
     from gym_b200 import build
     lib = os.path.join(out_dir, "libb200gym_phases.so")
     cmd = ([build._nvcc()] + build.NVCC_FLAGS + ["-DB200_PHASE_CLOCKS", "-o", lib] +
-           [os.path.join(build.CSRC, "b200gym.cu")])
+           [f for f in build.sources() if f.endswith(".cu")])
     subprocess.run(cmd, check=True)
     return lib
 
 
 def read_clocks(lib, clear):
     cyc = (ctypes.c_ulonglong * N_BUCKETS)()
-    ns = (ctypes.c_ulonglong * (MAX_CTAS * 4))()
+    ns = (ctypes.c_ulonglong * (MAX_CTAS * N_STAMPS))()
     if lib.b200gym_phase_clocks(cyc, ns, int(clear)) != 0:
         raise RuntimeError("b200gym_phase_clocks failed")
     c = np.array(cyc[:], dtype=np.float64)
-    t = np.array(ns[:], dtype=np.float64).reshape(MAX_CTAS, 4)
+    t = np.array(ns[:], dtype=np.float64).reshape(MAX_CTAS, N_STAMPS)
     return c, t[t[:, 0] > 0]
 
 
 def summarise(c, t):
     """one launch's (or a sum of launches') counters -> shares, cycles per tile and CTA time stamps"""
-    tiles = max(c[5], 1.0)
+    tiles = max(c[6], 1.0)
     comp = {k: c[b] for b, k in enumerate(COMPUTE)}
-    comp["stored_wait"] = c[13]   # part of "reset": waiting until a tile's bulk stores have completed
-    copy = {k: c[6 + b] for b, k in enumerate(COPY)}
-    copy["wait_prev_stored"] = c[12]   # kernels that release each tile's rows to in-loop resets
-    comp_loop, copy_loop = max(c[4], 1.0), max(c[11], 1.0)
+    copy = {k: c[7 + b] for b, k in enumerate(COPY)}
+    comp_loop, copy_loop = max(c[5], 1.0), max(c[12], 1.0)
     out = {
         "compute_share": {k: v / comp_loop for k, v in comp.items()},
         "compute_cycles_per_warp_tile": {k: v / tiles for k, v in comp.items()},
         "compute_loop_cycles_per_warp_tile": comp_loop / tiles,
         # the copy thread handles one tile per 8 compute warp-tiles
-        "copy_share": {k: v / copy_loop for k, v in copy.items() if k != "final_wait_all"},
+        "copy_share": {k: v / copy_loop for k, v in copy.items() if k != "final_wait_read"},
         "copy_cycles_per_tile": {k: v / (tiles / 8) for k, v in copy.items()},
     }
     if len(t):
@@ -73,8 +72,7 @@ def summarise(c, t):
         out["cta_us"] = {
             "start_spread_max": float(start_spread.max()) / 1e3,
             "loop_end_mean": float(rel[:, 0].mean()) / 1e3, "loop_end_max": float(rel[:, 0].max()) / 1e3,
-            "drain_start_mean": float(rel[:, 1].mean()) / 1e3, "drain_start_max": float(rel[:, 1].max()) / 1e3,
-            "drain_end_mean": float(rel[:, 2].mean()) / 1e3, "drain_end_max": float(rel[:, 2].max()) / 1e3,
+            "exit_mean": float(rel[:, 1].mean()) / 1e3, "exit_max": float(rel[:, 1].max()) / 1e3,
         }
     return out
 
@@ -115,7 +113,7 @@ def run(lib, torch, gym_b200, log2n, steps, warmup, flushed):
             env.step(pool[k % 16])
         torch.cuda.synchronize()
         c, _ = read_clocks(lib, True)
-        res = summarise(c / steps, np.zeros((0, 4)))
+        res = summarise(c / steps, np.zeros((0, N_STAMPS)))
     env.close()
     res.update({"log2_envs": log2n, "steps": steps, "l2_flushed": flushed})
     return res
