@@ -31,6 +31,9 @@ LUNAR_ENABLE_WIND = 1
 # enum b200gym_action_dtype
 ACT_I64, ACT_I32, ACT_U8, ACT_F32 = 0, 1, 2, 3
 
+# enum b200gym_mlp_activation, by the name rollout_mlp(activation=) takes
+MLP_ACTIVATIONS = {"relu": 0, "tanh": 1}
+
 
 class Config(ctypes.Structure):
     """struct b200gym_config"""
@@ -140,6 +143,10 @@ SIGNATURES = {
                                    _vp, _vp, _vp, _vp]),
     "b200gym_rollout_mlp_noisy": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                          _vp, _vp, _vp, _vp]),
+    "b200gym_rollout_mlp_act": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                       _vp, _vp, _vp, _vp, _vp, _i32]),
+    "b200gym_rollout_mlp_noisy_act": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                             _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200gym_invalid_actions": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_invalid_seen": (_i32, [_vp]),
     "b200gym_host_buffers": (_i32, [_vp, ctypes.POINTER(HostIO)]),
@@ -180,6 +187,7 @@ SIGNATURES = {
     "b200gym_box2d_overflows": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_box2d_list_counts": (_i32, [_vp, _vp, _i32, _vp, _vp]),
     "b200gym_selftest_trig": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp]),
+    "b200gym_selftest_tanh": (_i32, [_vp, _i64, _vp, _vp]),
     "b200gym_selftest_box2d": (_i32, [_i32, _vp, _i64, _vp, _vp]),
     "b200gym_selftest": (_i32, [_i32, _i64, ctypes.c_uint64, ctypes.POINTER(_i64)]),
 }

@@ -386,24 +386,25 @@ __device__ __forceinline__ const float *mlp_stage(const float *params, int64_t c
 
 // ... with the actions computed by each env's MLP policy from the observation of the step before (rollout_mlp_env):
 // PER_ENV, env i's row of parameters read from device memory at every step; otherwise one policy, staged in shared
-// memory once per CTA.  SUMMARY: no per-step outputs, one episode summary per env.  Held to 128 registers (two CTAs
-// per SM), ptxas spills the per-env Pendulum kernels, so the per-env kernels ask for one CTA per SM instead
-template <int KIND, bool SUMMARY, bool PER_ENV>
+// memory once per CTA.  SUMMARY: no per-step outputs, one episode summary per env.  ACT: the hidden layers' activation
+// (mlp_act).  Held to 128 registers (two CTAs per SM), ptxas spills the per-env Pendulum kernels, so the per-env
+// kernels ask for one CTA per SM instead
+template <int KIND, bool SUMMARY, bool PER_ENV, int ACT>
 __global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2) rollout_mlp_kernel(const StepArgs a, const int32_t T, float *last_obs,
                                                                const MlpPolicyArgs p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if constexpr (PER_ENV) {
-        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, true>(a, i, T, last_obs, p.params + i * p.stride, p);
+        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, true, ACT>(a, i, T, last_obs, p.params + i * p.stride, p);
     } else {
-        using Src = MlpActions<KIND, SUMMARY, false>;
+        using Src = MlpActions<KIND, SUMMARY, false, ACT>;
         const float *w = mlp_stage(p.params, mlp_param_count<Src::K, Src::D>(p.h1, p.h2));
-        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, false>(a, i, T, last_obs, w, p);
+        if (i < a.n) rollout_mlp_env<KIND, SUMMARY, false, ACT>(a, i, T, last_obs, w, p);
     }
 }
 
 // One step's actions of a Box2D MLP-policy rollout, before that step's launches: linear_policy_kernel with env i's
-// MLP (mlp_outputs; PER_ENV as rollout_mlp_kernel) in place of its linear policy
-template <int K, int D, bool DISCRETE, bool PER_ENV>
+// MLP (mlp_outputs; PER_ENV and ACT as rollout_mlp_kernel) in place of its linear policy
+template <int K, int D, bool DISCRETE, bool PER_ENV, int ACT>
 __global__ void __launch_bounds__(kThreads) mlp_policy_kernel(const float *obs, void *actions, const MlpPolicyArgs p,
                                                               const double *reward, const uint8_t *term,
                                                               const uint8_t *trunc, int64_t n, int32_t t_prev, int act,
@@ -425,7 +426,7 @@ __global__ void __launch_bounds__(kThreads) mlp_policy_kernel(const float *obs, 
     float o[D], z[K];
 #pragma unroll
     for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
-    mlp_outputs<K, D, PER_ENV>(w, p.h1, p.h2, p.vec != 0, o, z);
+    mlp_outputs<K, D, PER_ENV, ACT>(w, p.h1, p.h2, p.vec != 0, o, z);
     if constexpr (DISCRETE) {
         static_cast<long long *>(actions)[i] = argmax_first<K>(z);
     } else {
@@ -434,25 +435,25 @@ __global__ void __launch_bounds__(kThreads) mlp_policy_kernel(const float *obs, 
     }
 }
 
-// ... with the actions computed by each env's MLP policy plus the caller's noise (rollout_mlp_noisy_env); PER_ENV and
-// the launch bounds as rollout_mlp_kernel
-template <int KIND, bool PER_ENV>
+// ... with the actions computed by each env's MLP policy plus the caller's noise (rollout_mlp_noisy_env); PER_ENV, ACT
+// and the launch bounds as rollout_mlp_kernel
+template <int KIND, bool PER_ENV, int ACT>
 __global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2)
     rollout_mlp_noisy_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpNoisyArgs p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if constexpr (PER_ENV) {
-        if (i < a.n) rollout_mlp_noisy_env<KIND, true>(a, i, T, last_obs, p.mlp.params + i * p.mlp.stride, p);
+        if (i < a.n) rollout_mlp_noisy_env<KIND, true, ACT>(a, i, T, last_obs, p.mlp.params + i * p.mlp.stride, p);
     } else {
-        using Src = MlpNoisyActions<KIND, false>;
+        using Src = MlpNoisyActions<KIND, false, ACT>;
         const float *w = mlp_stage(p.mlp.params, mlp_param_count<Src::K, Src::D>(p.mlp.h1, p.mlp.h2));
-        if (i < a.n) rollout_mlp_noisy_env<KIND, false>(a, i, T, last_obs, w, p);
+        if (i < a.n) rollout_mlp_noisy_env<KIND, false, ACT>(a, i, T, last_obs, w, p);
     }
 }
 
 // One step's actions of a Box2D noisy MLP-policy rollout: mlp_policy_kernel with the step's noise slice added to the
 // outputs (noisy_outputs), which go to the step's outputs slice.  The launch passes p.noise and p.outputs at that
 // step's slice.  No summary mode: reward, term, trunc, t_prev, act and init are the launcher's and unused here
-template <int K, int D, bool DISCRETE, bool PER_ENV>
+template <int K, int D, bool DISCRETE, bool PER_ENV, int ACT>
 __global__ void __launch_bounds__(kThreads) mlp_noisy_policy_kernel(const float *obs, void *actions,
                                                                     const MlpNoisyArgs p, const double *, const uint8_t *,
                                                                     const uint8_t *, int64_t n, int32_t, int, int) {
@@ -463,7 +464,7 @@ __global__ void __launch_bounds__(kThreads) mlp_noisy_policy_kernel(const float 
     float o[D], z[K], y[K];
 #pragma unroll
     for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
-    mlp_outputs<K, D, PER_ENV>(w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, z);
+    mlp_outputs<K, D, PER_ENV, ACT>(w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, z);
     noisy_outputs<K>(z, p.noise + i * K, p.outputs + i * K, y);
     if constexpr (DISCRETE) {
         static_cast<long long *>(actions)[i] = argmax_first<K>(y);
@@ -1560,6 +1561,14 @@ __global__ void __launch_bounds__(kThreads) selftest_trig_kernel(const double *x
     if (sq) sq[i] = gt::sq(x[i]);
 }
 
+// device self-test: the tanh activation of the MLP policies (mlp_tanh) evaluated on caller-supplied arguments (the
+// caller compares with torch.tanh on the same device)
+__global__ void __launch_bounds__(kThreads) selftest_tanh_kernel(const float *x, int64_t n, float *y) {
+    const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    y[i] = mlp_tanh(x[i]);
+}
+
 static inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 // ---------------------------------------------------------------------------
@@ -2202,6 +2211,16 @@ extern "C" int b200gym_selftest_trig(const double *x_dev, int64_t n, double *sin
     return 0;
 }
 
+extern "C" int b200gym_selftest_tanh(const float *x_dev, int64_t n, float *y_dev, void *stream) {
+    if (!x_dev || !y_dev || n <= 0) return fail(nullptr, "b200gym_selftest_tanh: bad argument");
+    const int dev = device_of(x_dev);
+    if (dev < 0) return fail(nullptr, "b200gym_selftest_tanh: x is not a device pointer");
+    DeviceGuard guard(dev);
+    selftest_tanh_kernel<<<blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, n, y_dev);
+    CK(nullptr, cudaGetLastError());
+    return 0;
+}
+
 // b2probe.cu: the probe kernel, in a module of its own so that this module's kernels compile as they did without it
 cudaError_t b2probe_launch(int op, const float *in_dev, int64_t n, float *out_dev, cudaStream_t stream);
 int b2probe_num_ops();
@@ -2753,29 +2772,54 @@ extern "C" int b200gym_rollout_linear(b200gym_t *h, const float *weight_dev, con
     return fail(h, "bad kind %d", h->cfg.kind);
 }
 
-// ---- closed-loop rollouts of a ReLU MLP policy (b200gym_rollout_mlp) ----
-template <int KIND>
+// ---- closed-loop rollouts of an MLP policy (b200gym_rollout_mlp) ----
+template <int KIND, int ACT>
 static int launch_rollout_mlp_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const MlpPolicyArgs &p,
                                    bool per_env, size_t smem, bool summary, cudaStream_t st) {
     const unsigned blocks = blocks_for(h->n);
     if (per_env) {
-        if (summary) rollout_mlp_kernel<KIND, true, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
-        else rollout_mlp_kernel<KIND, false, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+        if (summary) rollout_mlp_kernel<KIND, true, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+        else rollout_mlp_kernel<KIND, false, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
     } else {
-        if (summary) rollout_mlp_kernel<KIND, true, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
-        else rollout_mlp_kernel<KIND, false, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+        if (summary) rollout_mlp_kernel<KIND, true, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+        else rollout_mlp_kernel<KIND, false, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
     }
     CK(h, cudaGetLastError());
     return 0;
 }
 
-template <int K, int D, bool DISCRETE>
+template <int K, int D, bool DISCRETE, int ACT>
 static int launch_rollout_mlp_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
                                     const MlpPolicyArgs &p, bool per_env, size_t smem, bool summary, cudaStream_t st) {
     return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, [&](int32_t) { return p; },
-                                       per_env ? mlp_policy_kernel<K, D, DISCRETE, true>
-                                               : mlp_policy_kernel<K, D, DISCRETE, false>,
+                                       per_env ? mlp_policy_kernel<K, D, DISCRETE, true, ACT>
+                                               : mlp_policy_kernel<K, D, DISCRETE, false, ACT>,
                                        per_env ? 0 : smem, summary, st, "mlp_policy_kernel", "b200gym_rollout_mlp");
+}
+
+template <int ACT>
+static int launch_rollout_mlp(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
+                              const MlpPolicyArgs &p, bool pe, size_t smem, bool summary, cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, pe, smem, summary, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, pe, smem, summary, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, pe, smem, summary, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, summary, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, summary, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, summary, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
 }
 
 extern "C" int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
@@ -2783,7 +2827,20 @@ extern "C" int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int pe
                                    uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
                                    double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev, float *last_obs_dev,
                                    const float *first_obs_dev, void *stream) {
+    return b200gym_rollout_mlp_act(h, params_dev, per_env, n_layers, h1, h2, T, actions_out_dev, obs_dev, reward_dev,
+                                   terminated_dev, truncated_dev, final_obs_dev, returns_dev, lengths_dev, ended_dev,
+                                   last_obs_dev, first_obs_dev, stream, B200GYM_MLP_RELU);
+}
+
+extern "C" int b200gym_rollout_mlp_act(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                       int h2, int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                       uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                       double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev,
+                                       float *last_obs_dev, const float *first_obs_dev, void *stream, int activation) {
     if (!h) return fail(h, "b200gym_rollout_mlp: null handle");
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "b200gym_rollout_mlp_act: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)",
+                    activation);
     if (n_layers != 1 && n_layers != 2)
         return fail(h, "b200gym_rollout_mlp: n_layers must be 1 or 2 (got %d)", n_layers);
     if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
@@ -2810,41 +2867,24 @@ extern "C" int b200gym_rollout_mlp(b200gym_t *h, const float *params_dev, int pe
     const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
     cudaStream_t st = (cudaStream_t)stream;
     const bool pe = per_env != 0;
-    switch (h->cfg.kind) {
-    case B200GYM_CARTPOLE:
-        return launch_rollout_mlp_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_MOUNTAINCAR:
-        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_MOUNTAINCAR_CONT:
-        return launch_rollout_mlp_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_PENDULUM:
-        return launch_rollout_mlp_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_ACROBOT:
-        return launch_rollout_mlp_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_LUNARLANDER:
-        return launch_rollout_mlp_box2d<4, 8, true>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_LUNARLANDER_CONT:
-        return launch_rollout_mlp_box2d<2, 8, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
-    case B200GYM_BIPEDALWALKER:
-    case B200GYM_BIPEDALWALKER_HARDCORE:
-        return launch_rollout_mlp_box2d<4, 24, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
-    }
-    return fail(h, "bad kind %d", h->cfg.kind);
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_mlp<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
+    return launch_rollout_mlp<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, st);
 }
 
-// ---- stochastic rollouts of a ReLU MLP policy (b200gym_rollout_mlp_noisy) ----
-template <int KIND>
+// ---- stochastic rollouts of an MLP policy (b200gym_rollout_mlp_noisy) ----
+template <int KIND, int ACT>
 static int launch_rollout_mlp_noisy_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
                                          const MlpNoisyArgs &p, bool per_env, size_t smem, cudaStream_t st) {
     const unsigned blocks = blocks_for(h->n);
-    if (per_env) rollout_mlp_noisy_kernel<KIND, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
-    else rollout_mlp_noisy_kernel<KIND, false><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+    if (per_env) rollout_mlp_noisy_kernel<KIND, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+    else rollout_mlp_noisy_kernel<KIND, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
     CK(h, cudaGetLastError());
     return 0;
 }
 
 // The policy launch of step t reads noise slice t and writes outputs slice t
-template <int K, int D, bool DISCRETE>
+template <int K, int D, bool DISCRETE, int ACT>
 static int launch_rollout_mlp_noisy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
                                           const float *first_obs, const MlpNoisyArgs &p, bool per_env, size_t smem,
                                           cudaStream_t st) {
@@ -2856,10 +2896,35 @@ static int launch_rollout_mlp_noisy_box2d(b200gym *h, const StepArgs &a, int32_t
                                            q.outputs = p.outputs + t * slice;
                                            return q;
                                        },
-                                       per_env ? mlp_noisy_policy_kernel<K, D, DISCRETE, true>
-                                               : mlp_noisy_policy_kernel<K, D, DISCRETE, false>,
+                                       per_env ? mlp_noisy_policy_kernel<K, D, DISCRETE, true, ACT>
+                                               : mlp_noisy_policy_kernel<K, D, DISCRETE, false, ACT>,
                                        per_env ? 0 : smem, false, st, "mlp_noisy_policy_kernel",
                                        "b200gym_rollout_mlp_noisy");
+}
+
+template <int ACT>
+static int launch_rollout_mlp_noisy(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
+                                    const MlpNoisyArgs &p, bool pe, size_t smem, cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_noisy_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, pe, smem, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, pe, smem, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, pe, smem, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_noisy_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, pe, smem, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_noisy_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, pe, smem, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_noisy_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_noisy_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_noisy_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, pe, smem, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
 }
 
 extern "C" int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
@@ -2867,7 +2932,22 @@ extern "C" int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, 
                                          void *actions_out_dev, float *obs_dev, double *reward_dev,
                                          uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
                                          float *last_obs_dev, const float *first_obs_dev, void *stream) {
+    return b200gym_rollout_mlp_noisy_act(h, params_dev, per_env, n_layers, h1, h2, T, noise_dev, outputs_dev,
+                                         actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev,
+                                         final_obs_dev, last_obs_dev, first_obs_dev, stream, B200GYM_MLP_RELU);
+}
+
+extern "C" int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                             int h2, int32_t T, const float *noise_dev, float *outputs_dev,
+                                             void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                             uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                             float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                             int activation) {
     if (!h) return fail(h, "b200gym_rollout_mlp_noisy: null handle");
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h,
+                    "b200gym_rollout_mlp_noisy_act: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)",
+                    activation);
     if (n_layers != 1 && n_layers != 2)
         return fail(h, "b200gym_rollout_mlp_noisy: n_layers must be 1 or 2 (got %d)", n_layers);
     if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
@@ -2890,26 +2970,9 @@ extern "C" int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, 
     const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
     cudaStream_t st = (cudaStream_t)stream;
     const bool pe = per_env != 0;
-    switch (h->cfg.kind) {
-    case B200GYM_CARTPOLE:
-        return launch_rollout_mlp_noisy_kind<B200GYM_CARTPOLE>(h, a, T, last_obs_dev, p, pe, smem, st);
-    case B200GYM_MOUNTAINCAR:
-        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR>(h, a, T, last_obs_dev, p, pe, smem, st);
-    case B200GYM_MOUNTAINCAR_CONT:
-        return launch_rollout_mlp_noisy_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last_obs_dev, p, pe, smem, st);
-    case B200GYM_PENDULUM:
-        return launch_rollout_mlp_noisy_kind<B200GYM_PENDULUM>(h, a, T, last_obs_dev, p, pe, smem, st);
-    case B200GYM_ACROBOT:
-        return launch_rollout_mlp_noisy_kind<B200GYM_ACROBOT>(h, a, T, last_obs_dev, p, pe, smem, st);
-    case B200GYM_LUNARLANDER:
-        return launch_rollout_mlp_noisy_box2d<4, 8, true>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
-    case B200GYM_LUNARLANDER_CONT:
-        return launch_rollout_mlp_noisy_box2d<2, 8, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
-    case B200GYM_BIPEDALWALKER:
-    case B200GYM_BIPEDALWALKER_HARDCORE:
-        return launch_rollout_mlp_noisy_box2d<4, 24, false>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
-    }
-    return fail(h, "bad kind %d", h->cfg.kind);
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_mlp_noisy<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
+    return launch_rollout_mlp_noisy<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------

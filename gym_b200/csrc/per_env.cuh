@@ -551,12 +551,24 @@ __device__ __forceinline__ void rollout_linear_env(const StepArgs &a, int64_t i,
     }
 }
 
-// ---- closed-loop rollouts of a ReLU MLP policy (b200gym_rollout_mlp) ----------------------------------------------
+// ---- closed-loop rollouts of an MLP policy (b200gym_rollout_mlp) --------------------------------------------------
 
 constexpr int kMlpMaxWidth = 64;   // the widest hidden layer b200gym_rollout_mlp takes
 
 // The hidden layers' activation: z if z > 0 or z is NaN, else +0.0 (so NaN propagates and -0.0 becomes +0.0)
 __device__ __forceinline__ float mlp_relu(float z) { return (z > 0.0f || z != z) ? z : 0.0f; }
+
+// The tanh activation: CUDA's tanhf on the device, which compiles to the instruction sequence of torch.tanh's float32
+// CUDA kernel (DESIGN.md §4.15), and the C library's tanhf in the host build.  b200gym_selftest_tanh evaluates it
+__host__ __device__ __forceinline__ float mlp_tanh(float z) { return tanhf(z); }
+
+// The activation ACT (B200GYM_MLP_RELU or B200GYM_MLP_TANH) of a hidden unit, chosen at compile time
+template <int ACT>
+__device__ __forceinline__ float mlp_act(float z) {
+    static_assert(ACT == B200GYM_MLP_RELU || ACT == B200GYM_MLP_TANH, "unknown MLP activation");
+    if constexpr (ACT == B200GYM_MLP_TANH) return mlp_tanh(z);
+    else return mlp_relu(z);
+}
 
 // A parameter of the MLP: from device memory through the read-only path (GLOBAL, each env's own row), or from the
 // CTA's shared copy
@@ -575,11 +587,11 @@ __device__ __forceinline__ float4 mlp_ld4(const float *p) {
 // by layer the weight (out, in) row-major, then the bias (out,).  Every unit starts at its bias and adds
 // weight[j, k] * x[k] for k = 0 .. in-1 in that order, every product and sum rounded to float32 (the library is built
 // with -fmad=false and the host build with -ffp-contract=off), as linear_logits; a hidden unit then goes through
-// mlp_relu.  The first hidden layer is held in a register array of kMlpMaxWidth under guarded, fully unrolled loops.
-// The last hidden layer is not stored: each of its units is added into the K outputs as soon as it is computed, in
+// mlp_act<ACT>.  The first hidden layer is held in a register array of kMlpMaxWidth under guarded, fully unrolled
+// loops.  The last hidden layer is not stored: each of its units is added into the K outputs as soon as it is computed, in
 // ascending order, which is the same sum as adding them afterwards.  vec: every row of the second layer's weight starts
 // 16 bytes aligned and h1 % 4 == 0, so those rows (the bulk of the parameters) are read 16 bytes at a time
-template <int K, int D, bool GLOBAL>
+template <int K, int D, bool GLOBAL, int ACT>
 __device__ __forceinline__ void mlp_outputs(const float *w, int h1, int h2, bool vec, const float (&o)[D],
                                             float (&z)[K]) {
     const float *b1 = w + h1 * D, *w2 = b1 + h1;
@@ -591,7 +603,7 @@ __device__ __forceinline__ void mlp_outputs(const float *w, int h1, int h2, bool
             float u = mlp_ld<GLOBAL>(b1 + j);
 #pragma unroll
             for (int k = 0; k < D; k++) u = u + mlp_ld<GLOBAL>(w + j * D + k) * o[k];
-            u = mlp_relu(u);
+            u = mlp_act<ACT>(u);
 #pragma unroll
             for (int k = 0; k < K; k++) z[k] = z[k] + mlp_ld<GLOBAL>(w2 + k * h1 + j) * u;
         }
@@ -605,7 +617,7 @@ __device__ __forceinline__ void mlp_outputs(const float *w, int h1, int h2, bool
             float u = mlp_ld<GLOBAL>(b1 + j);
 #pragma unroll
             for (int k = 0; k < D; k++) u = u + mlp_ld<GLOBAL>(w + j * D + k) * o[k];
-            x[j] = mlp_relu(u);
+            x[j] = mlp_act<ACT>(u);
         }
     }
     const float *b2 = w2 + h2 * h1, *w3 = b2 + h2, *b3 = w3 + K * h2;
@@ -630,7 +642,7 @@ __device__ __forceinline__ void mlp_outputs(const float *w, int h1, int h2, bool
             for (int m = 0; m < kMlpMaxWidth; m++)
                 if (m < h1) u = u + mlp_ld<GLOBAL>(row + m) * x[m];
         }
-        u = mlp_relu(u);
+        u = mlp_act<ACT>(u);
 #pragma unroll
         for (int k = 0; k < K; k++) z[k] = z[k] + mlp_ld<GLOBAL>(w3 + k * h2 + j) * u;
     }
@@ -655,8 +667,8 @@ struct MlpPolicyArgs {
 };
 
 // MlpActions: LinearActions with the MLP's outputs in place of the logits.  w: the env's parameters, in device memory
-// (GLOBAL) or the CTA's shared copy
-template <int KIND, bool SUMMARY, bool GLOBAL>
+// (GLOBAL) or the CTA's shared copy; ACT: the hidden layers' activation (mlp_act)
+template <int KIND, bool SUMMARY, bool GLOBAL, int ACT>
 struct MlpActions {
     static constexpr int K = linear_logit_count<KIND>(), D = bgym::Env<KIND>::D;
     const float *w;
@@ -666,7 +678,7 @@ struct MlpActions {
     template <typename ActT>
     __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
         float z[K];
-        mlp_outputs<K, D, GLOBAL>(w, h1, h2, vec, o, z);
+        mlp_outputs<K, D, GLOBAL, ACT>(w, h1, h2, vec, o, z);
         ActT v;
         if constexpr (bgym::Env<KIND>::A == 0) v = (ActT)argmax_first<K>(z);
         else v = z[0];
@@ -677,8 +689,9 @@ struct MlpActions {
 
 // T steps of env i under its MLP policy at w (rollout_mlp_kernel): rollout_linear_env's loop, written out again so
 // that no pre-existing kernel changes, with MlpActions in place of LinearActions.  The parameters are read at every
-// step, from w: a per-env row in device memory (GLOBAL), too large for registers, or the CTA's shared copy
-template <int KIND, bool SUMMARY, bool GLOBAL>
+// step, from w: a per-env row in device memory (GLOBAL), too large for registers, or the CTA's shared copy.  ACT as
+// MlpActions, ReLU when not given
+template <int KIND, bool SUMMARY, bool GLOBAL, int ACT = B200GYM_MLP_RELU>
 __device__ __forceinline__ void rollout_mlp_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
                                                 const float *w, const MlpPolicyArgs &p) {
     using E = bgym::Env<KIND>;
@@ -690,7 +703,7 @@ __device__ __forceinline__ void rollout_mlp_env(const StepArgs &a, int64_t i, in
     int32_t elapsed = a.elapsed[i];
     float o[E::D];
     E::observe(s, o);
-    const MlpActions<KIND, SUMMARY, GLOBAL> src{w, p.h1, p.h2, p.vec != 0, o};
+    const MlpActions<KIND, SUMMARY, GLOBAL, ACT> src{w, p.h1, p.h2, p.vec != 0, o};
     double ret = 0.0;
     int32_t len = 0;
     bool ended = false;
@@ -716,7 +729,7 @@ __device__ __forceinline__ void rollout_mlp_env(const StepArgs &a, int64_t i, in
     }
 }
 
-// ---- stochastic rollouts of a ReLU MLP policy (b200gym_rollout_mlp_noisy) -----------------------------------------
+// ---- stochastic rollouts of an MLP policy (b200gym_rollout_mlp_noisy) ---------------------------------------------
 
 // A load of an input the rollout reads once and never again: evict-first on the device, where T steps of noise are far
 // larger than L2; a plain load in the host build
@@ -754,7 +767,7 @@ __device__ __forceinline__ void noisy_outputs(const float (&z)[K], const float *
 // MlpNoisyActions: MlpActions with the caller's noise added to the outputs before the action is taken from them.  The
 // outputs z go to `outputs` and the action to the row of actions, both written once; noise and outputs point at row
 // t of their [T][n][K] arrays and move on by one row per step (next)
-template <int KIND, bool GLOBAL>
+template <int KIND, bool GLOBAL, int ACT>
 struct MlpNoisyActions {
     static constexpr int K = linear_logit_count<KIND>(), D = bgym::Env<KIND>::D;
     const float *w;
@@ -766,7 +779,7 @@ struct MlpNoisyActions {
     template <typename ActT>
     __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
         float z[K], y[K];
-        mlp_outputs<K, D, GLOBAL>(w, h1, h2, vec, o, z);
+        mlp_outputs<K, D, GLOBAL, ACT>(w, h1, h2, vec, o, z);
         noisy_outputs<K>(z, noise + i * K, outputs + i * K, y);
         ActT v;
         if constexpr (bgym::Env<KIND>::A == 0) v = (ActT)argmax_first<K>(y);
@@ -782,8 +795,8 @@ struct MlpNoisyActions {
 
 // T steps of env i under its MLP policy at w with the caller's noise (rollout_mlp_noisy_kernel): rollout_mlp_env's
 // loop without the summary mode, written out again so that no pre-existing kernel changes, with MlpNoisyActions in
-// place of MlpActions
-template <int KIND, bool GLOBAL>
+// place of MlpActions; ACT as rollout_mlp_env
+template <int KIND, bool GLOBAL, int ACT = B200GYM_MLP_RELU>
 __device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
                                                       const float *w, const MlpNoisyArgs &p) {
     using E = bgym::Env<KIND>;
@@ -795,7 +808,7 @@ __device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t
     int32_t elapsed = a.elapsed[i];
     float o[E::D];
     E::observe(s, o);
-    MlpNoisyActions<KIND, GLOBAL> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, p.noise, p.outputs};
+    MlpNoisyActions<KIND, GLOBAL, ACT> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, p.noise, p.outputs};
     double ret = 0.0;
     int32_t len = 0;
     bool ended = false;

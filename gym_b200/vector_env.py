@@ -666,9 +666,9 @@ class B200VectorEnv:
             self._lib.b200gym_rollout_linear(self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env), T,
                                              *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
 
-    def rollout_mlp(self, params, hidden, T, *, summary=False):
-        """T steps of a ReLU MLP policy in closed loop: ``rollout_linear()`` with the policy
-        D -> hidden[0] (-> hidden[1]) -> K, ReLU after every hidden layer and nothing after the last.
+    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu"):
+        """T steps of an MLP policy in closed loop: ``rollout_linear()`` with the policy
+        D -> hidden[0] (-> hidden[1]) -> K, the activation after every hidden layer and nothing after the last.
 
         ``hidden`` is a tuple of one or two widths, each 1 .. 64.  ``params`` packs one policy as P float32 values,
         layer by layer the weight (out, in) row-major and then the bias (out,): exactly
@@ -676,27 +676,35 @@ class B200VectorEnv:
         Shape (P,) is one policy for every env, (N, P) one per env: float32, contiguous, on the env's device.
 
         Every unit is ``z[j] = bias[j]``, then ``z[j] = z[j] + W[j, k] * x[k]`` for k = 0 .. in-1, every float32
-        product and sum rounded (no fused multiply-add).  A hidden unit's activation is ``z`` if ``z > 0`` or ``z`` is
-        NaN, else +0.0 (NaN propagates, -0.0 becomes +0.0).  The action is taken from the K outputs as
-        ``rollout_linear()`` takes it from its logits.  Returns, guards, capture and the start from the current state
-        are ``rollout_linear()``'s (DESIGN.md §4.13)."""
+        product and sum rounded (no fused multiply-add).  ``activation`` (keyword only) is ``"relu"`` or ``"tanh"``:
+
+        * ``"relu"``: a hidden unit's activation is ``z`` if ``z > 0`` or ``z`` is NaN, else +0.0 (NaN propagates,
+          -0.0 becomes +0.0), so ``nn.ReLU`` gives the same bits;
+        * ``"tanh"``: it is ``tanhf(z)`` of CUDA's math library, for the policies of CleanRL's PPO and
+          Stable-Baselines3's ``MlpPolicy`` (``nn.Tanh``).  ``torch.tanh`` / ``nn.Tanh`` on the device gives the same
+          bits: the two compile to the same instructions, and the tests check every float32 input against the torch
+          build they run with.  Another torch or CUDA build is not covered by that check (DESIGN.md §4.15).
+
+        The action is taken from the K outputs as ``rollout_linear()`` takes it from its logits.  Returns, guards,
+        capture and the start from the current state are ``rollout_linear()``'s (DESIGN.md §4.13)."""
         captured = self._rollout_guards("rollout_mlp")
-        h1, h2, per_env = self._mlp_params(params, hidden)
+        h1, h2, per_env, act = self._mlp_params(params, hidden, activation)
         vp = ctypes.c_void_p
         return self._policy_rollout("rollout_mlp", T, summary, captured, lambda T, outs, last, first: (
-            self._lib.b200gym_rollout_mlp(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T,
-                                          *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+            self._lib.b200gym_rollout_mlp_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2,
+                                              T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(),
+                                              act)))
 
-    def rollout_mlp_noisy(self, params, hidden, noise):
-        """T steps of a stochastic ReLU MLP policy in closed loop, T = ``noise.shape[0]`` -> ``(actions, outputs, obs,
+    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu"):
+        """T steps of a stochastic MLP policy in closed loop, T = ``noise.shape[0]`` -> ``(actions, outputs, obs,
         rewards, terminateds, truncateds, infos)``: bit for bit what
         ``for t in range(T): z = mlp(obs); a = rule(z + noise[t]); obs, r, te, tr, info = self.step(a)`` returns,
         stacked, with ``obs`` starting at the observation the env last returned, and the env left where that loop
         leaves it.
 
-        ``params`` and ``hidden`` are ``rollout_mlp()``'s, and z is its K outputs.  ``noise`` is float32 (T, N, K),
-        contiguous, on the env's device, 1 <= T < 2**31, with K = ``single_action_space.n`` (Discrete) or ``act_dim``
-        (Box).  Each ``z[k] + noise[t, i, k]`` is one rounded float32 add, IEEE NaN and infinity included; ``rule`` is
+        ``params``, ``hidden`` and ``activation`` are ``rollout_mlp()``'s, and z is its K outputs.  ``noise`` is
+        float32 (T, N, K), contiguous, on the env's device, 1 <= T < 2**31, with K = ``single_action_space.n``
+        (Discrete) or ``act_dim`` (Box).  Each ``z[k] + noise[t, i, k]`` is one rounded float32 add, IEEE NaN and infinity included; ``rule`` is
         ``np.argmax`` (the first NaN, else the first maximum) for Discrete kinds and the identity, unclipped, for Box
         kinds.  ``outputs`` is float32 (T, N, K), z before the noise; the other six are ``rollout_mlp()``'s.
 
@@ -715,21 +723,30 @@ class B200VectorEnv:
             a, mean, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), std * eps)
             logp = torch.distributions.Normal(mean, std).log_prob(a).sum(-1)
 
+        A CleanRL-shaped tanh actor runs as it is, packed with ``parameters_to_vector``::
+
+            actor = nn.Sequential(nn.Linear(D, 64), nn.Tanh(), nn.Linear(64, 64), nn.Tanh(), nn.Linear(64, K)).cuda()
+            params = torch.nn.utils.parameters_to_vector(actor.parameters()).detach()
+            a, logits, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), g, activation="tanh")
+
+        with ``g`` the Gumbel noise above (Discrete kinds), or ``std * eps`` in its place (Box kinds).
+
         Noise of -0.0 everywhere gives ``rollout_mlp()``'s actions (+0.0 would turn a -0.0 Box output into +0.0).
         Guards and the start from the current state are ``rollout_linear()``'s.  The classic-control kinds may be
         captured in a CUDA graph, and replays read the current contents of ``params`` and ``noise``, so filling the
         noise and rolling out can be one graph; the Box2D kinds cannot (DESIGN.md §4.14)."""
         captured = self._rollout_guards("rollout_mlp_noisy")
-        h1, h2, per_env = self._mlp_params(params, hidden, "rollout_mlp_noisy")
+        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, "rollout_mlp_noisy")
         T = self._noise_steps(noise)
         self._refuse_box2d_capture("rollout_mlp_noisy")
         outputs = _torch().empty_like(noise)
         vp = ctypes.c_void_p
         actions, obs, reward, term, trunc, infos = self._policy_rollout(
             "rollout_mlp_noisy", T, False, captured, lambda T, outs, last, first: (
-                self._lib.b200gym_rollout_mlp_noisy(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1,
-                                                    h2, T, vp(noise.data_ptr()), vp(outputs.data_ptr()), *outs[:6],
-                                                    vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+                self._lib.b200gym_rollout_mlp_noisy_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden),
+                                                        h1, h2, T, vp(noise.data_ptr()), vp(outputs.data_ptr()),
+                                                        *outs[:6], vp(last.data_ptr()), vp(first.data_ptr()),
+                                                        self._stream(), act)))
         return actions, outputs, obs, reward, term, trunc, infos
 
     def _noise_steps(self, noise):
@@ -808,10 +825,12 @@ class B200VectorEnv:
                              f"{tuple(bias.shape)}")
         return per_env
 
-    def _mlp_params(self, params, hidden, what="rollout_mlp"):
+    def _mlp_params(self, params, hidden, activation, what="rollout_mlp"):
         """Check rollout_mlp()'s or rollout_mlp_noisy()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden
-        layer), per_env)."""
+        layer), per_env, the b200gym_mlp_activation code)."""
         torch = _torch()
+        if not isinstance(activation, str) or activation not in _lib.MLP_ACTIVATIONS:
+            raise ValueError(f"{what}() needs activation 'relu' or 'tanh', got {activation!r}")
         if not isinstance(hidden, (tuple, list)) or not 1 <= len(hidden) <= 2 or any(
                 isinstance(h, (bool, np.bool_)) or not isinstance(h, (int, np.integer)) or not 1 <= int(h) <= 64
                 for h in hidden):
@@ -832,7 +851,7 @@ class B200VectorEnv:
         if not (per_env or tuple(params.shape) == (P,)):
             raise ValueError(f"{what}() with hidden {tuple(widths)} needs params ({P},) for one policy or "
                              f"({self.num_envs}, {P}) for one per env; got {tuple(params.shape)}")
-        return widths[0], widths[1] if len(widths) == 2 else 0, per_env
+        return widths[0], widths[1] if len(widths) == 2 else 0, per_env, _lib.MLP_ACTIVATIONS[activation]
 
     def _rollout_guards(self, what):
         """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp() / rollout_mlp_noisy(), all

@@ -273,6 +273,30 @@ int b200gym_rollout_mlp_noisy(b200gym_t *h, const float *params_dev, int per_env
                               float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
                               float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream);
 
+/* The hidden layers' activation of b200gym_rollout_mlp_act / b200gym_rollout_mlp_noisy_act. */
+enum b200gym_mlp_activation {
+    B200GYM_MLP_RELU = 0, /* z if z > 0 or z is NaN, else +0.0 (b200gym_rollout_mlp) */
+    B200GYM_MLP_TANH = 1  /* tanhf(z) of CUDA's math library: on an H100 the bits of torch.tanh on a float32 CUDA
+                             tensor (checked for every input against the torch build of the tests; see
+                             b200gym_selftest_tanh) */
+};
+
+/*
+ * b200gym_rollout_mlp and b200gym_rollout_mlp_noisy with the hidden layers' activation `activation`, a
+ * b200gym_mlp_activation; any other value fails.  Every unit's sum is as there, and the output layer stays linear.
+ * b200gym_rollout_mlp(...) is b200gym_rollout_mlp_act(..., B200GYM_MLP_RELU), and likewise for the noisy one.
+ */
+int b200gym_rollout_mlp_act(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                            int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                            uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev,
+                            int32_t *lengths_dev, uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev,
+                            void *stream, int activation);
+int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                                  int32_t T, const float *noise_dev, float *outputs_dev, void *actions_out_dev,
+                                  float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                  float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                  int activation);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
@@ -656,6 +680,12 @@ int b200gym_selftest(int device, int64_t samples, uint64_t seed, int64_t *mismat
  * sq_dev may be NULL.  Asynchronous.
  */
 int b200gym_selftest_trig(const double *x_dev, int64_t n, double *sin_dev, double *cos_dev, double *sq_dev, void *stream);
+/*
+ * Device self-test of the tanh activation of the MLP policies (B200GYM_MLP_TANH): y_dev[k] = the activation of
+ * x_dev[k] for k < n, float32, computed by the same device function the policy kernels inline (the caller compares
+ * with torch.tanh on the same device).  Asynchronous.
+ */
+int b200gym_selftest_tanh(const float *x_dev, int64_t n, float *y_dev, void *stream);
 /*
  * Device self-test of the Box2D building blocks (csrc/b2probe.cuh): one thread per record runs `op` on in_dev[n][16]
  * float32 and writes out_dev[n][16].  op: 0 rot_of, 1 edge-polygon manifold, 2 box-polygon manifold, 3 edge ray cast,
