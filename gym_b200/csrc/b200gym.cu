@@ -110,6 +110,7 @@ struct b200gym {
     unsigned long long *snap_bad = nullptr;       // page-locked, device-mapped word: an out-of-range snapshot index was met
     unsigned long long *snap_bad_dev = nullptr;   // device alias
     unsigned char *snap_scratch = nullptr;        // b200gym_clone: n rows
+    b200gym *from_batch = nullptr;                // b200gym_rollout_from, Box2D kinds: scratch batch (lazily created)
     // per-env wrapper chain (b200gym_subenv_set); the host-buffer path runs it inside its calls
     struct {
         bool on = false, out_f64 = false, episode = false;
@@ -2074,6 +2075,7 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     cudaFree(h->toi_mid);
     if (h->snap_bad) cudaFreeHost(h->snap_bad);
     cudaFree(h->snap_scratch);
+    if (h->from_batch) b200gym_destroy(h->from_batch);
     if (h->sub.final64) cudaFreeHost(h->sub.final64);
     if (h->sub.ep_r) cudaFreeHost(h->sub.ep_r);
     if (h->sub.ep_l) cudaFreeHost(h->sub.ep_l);
@@ -3514,10 +3516,12 @@ static int snap_save(b200gym *h, const int64_t *idx, int64_t m, void *snap, cuda
     return 0;
 }
 
+// bad: the index-error flag to raise (null: the handle's own)
 static int snap_load(b200gym *h, const void *snap, int64_t snap_rows, const int64_t *row, const int64_t *dst, int64_t m,
-                     cudaStream_t st) {
+                     cudaStream_t st, unsigned long long *bad = nullptr) {
     int T, R;
-    const SnapArgs a = snap_args(h, &T, &R);
+    SnapArgs a = snap_args(h, &T, &R);
+    if (bad) a.bad = bad;
     const unsigned grid = (unsigned)((m + T - 1) / T);
     snapshot_load_kernel<<<grid, kThreads, (size_t)T * R + 2 * T * 8 + 8, st>>>(a, (const unsigned char *)snap, snap_rows,
                                                                               row, dst, m);
@@ -3568,4 +3572,165 @@ extern "C" int b200gym_snapshot_index_error(b200gym_t *h) {
     if (!h->snap_bad || *(volatile unsigned long long *)h->snap_bad == 0ULL) return 0;
     *(volatile unsigned long long *)h->snap_bad = 0ULL;
     return 1;
+}
+
+// ---- rollouts from snapshot rows (b200gym_rollout_from) ----
+// Branch b's T steps from its row (rollout_from_env), one thread per branch.  The thread's byte of s_flags holds the
+// branch's copy of the row's flag byte, so that advance_env never touches the handle's flags
+template <int KIND, bool STATES>
+__global__ void __launch_bounds__(kThreads) rollout_from_kernel(const StepArgs a, const int32_t T,
+                                                                const RolloutFromArgs p) {
+    __shared__ uint8_t s_flags[kThreads];
+    using ActT = typename std::conditional<Env<KIND>::A == 0, long long, float>::type;
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.n) return;
+    StepArgs c = a;
+    c.flags = s_flags;
+    rollout_from_env<KIND, ActT, STATES>(c, b, (int)threadIdx.x, T, p);
+}
+
+// The Box2D path: fold step t's reward and flags into the summary of every branch (linear_policy_kernel's fold; step
+// 0 starts it at 0.0 + reward)
+__global__ void __launch_bounds__(kThreads) rollout_from_fold_kernel(const RolloutFromArgs p, int64_t B,
+                                                                     const double *reward, const uint8_t *term,
+                                                                     const uint8_t *trunc, int32_t t) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    if (t == 0) {
+        p.returns[b] = 0.0 + reward[b];
+        p.lengths[b] = 1;
+        p.ended[b] = (term[b] | trunc[b]) != 0;
+    } else if (!p.ended[b]) {
+        p.returns[b] = p.returns[b] + reward[b];
+        p.lengths[b] = t + 1;
+        p.ended[b] = (term[b] | trunc[b]) != 0;
+    }
+}
+
+// ... and, last, zero the outputs of the branches whose row index is out of range (the load skipped them and raised
+// the flag): R bytes of end row and D floats of end observation each, when given
+__global__ void __launch_bounds__(kThreads) rollout_from_skip_kernel(const RolloutFromArgs p, int64_t B, int R, int D) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int64_t row = p.row_idx[b];
+    if (row >= 0 && row < p.n_rows) return;
+    p.returns[b] = 0.0;
+    p.lengths[b] = 0;
+    p.ended[b] = 0;
+    if (!p.end_rows) return;
+    for (int c = 0; c < R / 16; c++) reinterpret_cast<uint4 *>(p.end_rows + b * R)[c] = make_uint4(0u, 0u, 0u, 0u);
+    for (int k = 0; k < D; k++) p.end_obs[b * D + k] = 0.0f;
+}
+
+template <int KIND>
+static int launch_rollout_from_kind(b200gym *h, const StepArgs &a, int32_t T, const RolloutFromArgs &p,
+                                    cudaStream_t st) {
+    if (snap_row_bytes(KIND) != classic_row_bytes<KIND>())
+        return fail(h, "b200gym_rollout_from: row layout mismatch for kind %d", KIND);
+    if (p.end_rows) rollout_from_kernel<KIND, true><<<blocks_for(a.n), kThreads, 0, st>>>(a, T, p);
+    else rollout_from_kernel<KIND, false><<<blocks_for(a.n), kThreads, 0, st>>>(a, T, p);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// A Box2D rollout from rows, composed of what the engine has: the rows loaded into a handle-owned scratch batch of at
+// least B envs (envs [0, B) used), the step sequence of launch_step_box2d per step into one slice of outputs, the fold
+// after each step, and with end states a save of the scratch batch.  Its steps take milliseconds, so fusing them would
+// save nothing measurable.  Invalid actions count in h's counter and bad row indices raise h's flag
+static int launch_rollout_from_box2d(b200gym *h, const RolloutFromArgs &p, int64_t B, const void *actions,
+                                     int action_dtype, int32_t T, cudaStream_t st) {
+    const char *who = "b200gym_rollout_from";
+    if (!h->from_batch || h->from_batch->n < B) {
+        if (h->from_batch) b200gym_destroy(h->from_batch);
+        h->from_batch = nullptr;
+        b200gym *s = nullptr;
+        if (b200gym_create(&h->cfg, B, h->device, &s))
+            return fail(h, "%s: cannot create the scratch batch: %s", who, b200gym_last_error(nullptr));
+        h->from_batch = s;
+        // the envs a bad row index leaves unloaded step from a valid state: seeded (a zero PCG64 record only ever
+        // draws zero, on which BipedalWalker's terrain draws never finish), then reset
+        const uint32_t seed[4] = {0u, 0u, 0u, 0u};
+        if (b200gym_seed_range(s, seed, 0, st) || launch_reset(s, nullptr, nullptr, nullptr, st))
+            return fail(h, "%s: %s", who, s->err.c_str());
+    }
+    b200gym *s = h->from_batch;
+    if (snap_prepare(s, who)) return fail(h, "%s", s->err.c_str());
+    if (snap_load(s, p.rows, p.n_rows, p.row_idx, nullptr, B, st, h->snap_bad_dev)) return fail(h, "%s", s->err.c_str());
+    const int64_t D = h->D;
+    const size_t obs_bytes = ((size_t)B * D * sizeof(float) + 15) / 16 * 16;
+    const size_t r_bytes = ((size_t)B * sizeof(double) + 15) / 16 * 16, f_bytes = ((size_t)B + 15) / 16 * 16;
+    void *scratch = nullptr;
+    CK(h, cudaMallocAsync(&scratch, obs_bytes + r_bytes + 2 * f_bytes, st));
+    unsigned char *base = static_cast<unsigned char *>(scratch);
+    float *obs = reinterpret_cast<float *>(base);
+    double *reward = reinterpret_cast<double *>(base + obs_bytes);
+    uint8_t *term = base + obs_bytes + r_bytes, *trunc = term + f_bytes;
+    StepArgs a = make_args(s, nullptr, obs, reward, term, trunc, nullptr);
+    a.count = B;
+    a.invalid = h->invalid;
+    a.invalid_seen = h->invalid_seen_dev;
+    const size_t act_row = (size_t)B * std::max(h->A, 1) * action_size(action_dtype);
+    const unsigned blocks = blocks_for(B);
+    int rc = 0;
+    for (int32_t t = 0; t < T && !rc; t++) {
+        a.actions = static_cast<const unsigned char *>(actions) + (size_t)t * act_row;
+        if (launch_step_box2d(s, a, action_dtype, st)) {
+            rc = fail(h, "%s", s->err.c_str());
+            break;
+        }
+        rollout_from_fold_kernel<<<blocks, kThreads, 0, st>>>(p, B, reward, term, trunc, t);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: rollout_from_fold_kernel launch failed", who);
+    }
+    if (!rc && p.end_rows) {
+        if (snap_save(s, nullptr, B, p.end_rows, st)) rc = fail(h, "%s", s->err.c_str());
+        else if (cudaMemcpyAsync(p.end_obs, obs, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToDevice, st))
+            rc = fail(h, "%s: copy of the end observations failed", who);
+    }
+    if (!rc && p.row_idx) {
+        rollout_from_skip_kernel<<<blocks, kThreads, 0, st>>>(p, B, snap_row_bytes(h->cfg.kind), (int)D);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: rollout_from_skip_kernel launch failed", who);
+    }
+    cudaFreeAsync(scratch, st);
+    return rc;
+}
+
+extern "C" int b200gym_rollout_from(b200gym_t *h, const void *snap_rows_dev, int64_t n_rows, const int64_t *row_idx_dev,
+                                    int64_t B, const void *actions_dev, int action_dtype, int32_t T,
+                                    double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev, void *end_rows_dev,
+                                    float *end_obs_dev, void *stream) {
+    if (!h) return fail(h, "b200gym_rollout_from: null handle");
+    if (B < 1) return fail(h, "b200gym_rollout_from: B must be at least 1 (got %lld)", (long long)B);
+    if (T < 1) return fail(h, "b200gym_rollout_from: T must be at least 1 (got %d)", T);
+    if (n_rows < 0 || (!row_idx_dev && n_rows < B))
+        return fail(h, "b200gym_rollout_from: %lld rows cannot start %lld branches without row indices",
+                    (long long)n_rows, (long long)B);
+    if (!actions_dev || !returns_dev || !lengths_dev || !ended_dev)
+        return fail(h, "b200gym_rollout_from: null buffer");
+    if (!end_rows_dev != !end_obs_dev)
+        return fail(h, "b200gym_rollout_from: give both end_rows_dev and end_obs_dev, or neither");
+    if (snap_check_ptr(h, snap_rows_dev, "b200gym_rollout_from")) return 1;
+    if (end_rows_dev && (uintptr_t)end_rows_dev % 128 != 0)
+        return fail(h, "b200gym_rollout_from: end_rows_dev must be 128-byte aligned");
+    const int want = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
+    if (action_dtype != want)
+        return fail(h, "b200gym_rollout_from: this env needs %s actions (got dtype code %d)",
+                    h->A == 0 ? "int64" : "float32", action_dtype);
+    DeviceGuard guard(h->device);
+    // the index-error flag only matters when row indices are given
+    if (row_idx_dev && snap_prepare(h, "b200gym_rollout_from")) return 1;
+    RolloutFromArgs p{static_cast<const unsigned char *>(snap_rows_dev), n_rows, row_idx_dev, returns_dev, lengths_dev,
+                      ended_dev, static_cast<unsigned char *>(end_rows_dev), end_obs_dev, h->snap_bad_dev};
+    cudaStream_t st = (cudaStream_t)stream;
+    if (h->is_lunar || h->is_walker) return launch_rollout_from_box2d(h, p, B, actions_dev, action_dtype, T, st);
+    StepArgs a = make_args(h, actions_dev, nullptr, nullptr, nullptr, nullptr, nullptr);
+    a.state = nullptr; a.elapsed = nullptr; a.flags = nullptr; a.rng = nullptr; a.lunar_rec = nullptr;   // not h's envs
+    a.n = B; a.count = B;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_from_kind<B200GYM_CARTPOLE>(h, a, T, p, st);
+    case B200GYM_MOUNTAINCAR: return launch_rollout_from_kind<B200GYM_MOUNTAINCAR>(h, a, T, p, st);
+    case B200GYM_MOUNTAINCAR_CONT: return launch_rollout_from_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, p, st);
+    case B200GYM_PENDULUM: return launch_rollout_from_kind<B200GYM_PENDULUM>(h, a, T, p, st);
+    case B200GYM_ACROBOT: return launch_rollout_from_kind<B200GYM_ACROBOT>(h, a, T, p, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
 }

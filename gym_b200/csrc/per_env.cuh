@@ -830,6 +830,105 @@ __device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t
     a.elapsed[i] = elapsed;
 }
 
+// ---- rollouts from snapshot rows (b200gym_rollout_from) ------------------------------------------------------------
+
+// The snapshot row of a classic kind (b200gym.cu, snapshot_save_kernel): the PCG64 record {state_hi, state_lo, inc_hi,
+// inc_lo} in bytes [0, 32), float64 state[S] from byte 32, then the TimeLimit counter, the flag byte in the low byte of
+// the next word, and zeros up to a multiple of 32 bytes
+template <int KIND>
+__host__ __device__ constexpr int classic_row_bytes() {
+    return (32 + 8 * bgym::Env<KIND>::S + 4 + 1 + 31) / 32 * 32;
+}
+
+// The arguments of a b200gym_rollout_from launch.  Branch b starts from row row_idx[b] (row_idx null: row b) of the
+// n_rows rows at `rows`; a row index out of range skips the branch: zero outputs, and `bad` raised.  end_rows and
+// end_obs: null, or [B] rows and observations of the end states (STATES)
+struct RolloutFromArgs {
+    const unsigned char *rows;
+    int64_t n_rows;
+    const int64_t *row_idx;
+    double *returns;
+    int32_t *lengths;
+    uint8_t *ended;
+    unsigned char *end_rows;
+    float *end_obs;
+    unsigned long long *bad;   // page-locked, device-mapped word (the handle's snapshot index-error flag)
+};
+
+// T steps of branch b (rollout_from_kernel): rollout_env's loop from a snapshot row instead of the handle's arrays,
+// written out again so that no pre-existing kernel changes.  The PCG64 stream of the autoresets, the state and the
+// TimeLimit counter are loaded from the row once and held in registers (reset_env_from, never reset_env: the handle's
+// records are not the branch's).  a.actions is the [T][B] array and a.n = B; a.flags[f] is the branch's own copy of
+// the row's flag byte, which advance_env reads and writes for CartPole without autoreset (the kernel gives each thread
+// a byte of shared memory; nothing else is indexed by f).  LinearSink<KIND, true> folds the rewards and flags into the
+// episode summary and keeps the last observation; nothing is stored per step.  STATES: the end row in the layout of
+// classic_row_bytes and the end observation are stored at the end
+template <int KIND, typename ActT, bool STATES, typename I>
+__device__ __forceinline__ void rollout_from_env(const StepArgs &a, int64_t b, I f, int32_t T,
+                                                 const RolloutFromArgs &p) {
+    using E = bgym::Env<KIND>;
+    constexpr int R = classic_row_bytes<KIND>(), C = R / 16;
+    const int64_t row = p.row_idx ? p.row_idx[b] : b;
+    if (row < 0 || row >= p.n_rows) {
+        *reinterpret_cast<volatile unsigned long long *>(p.bad) = 1ULL;
+        p.returns[b] = 0.0;
+        p.lengths[b] = 0;
+        p.ended[b] = 0;
+        if constexpr (STATES) {
+            ulonglong2 *out = reinterpret_cast<ulonglong2 *>(p.end_rows + b * R);
+#pragma unroll
+            for (int c = 0; c < C; c++) out[c] = make_ulonglong2(0ULL, 0ULL);
+#pragma unroll
+            for (int k = 0; k < E::D; k++) p.end_obs[b * E::D + k] = 0.0f;
+        }
+        return;
+    }
+    const ulonglong2 *in = reinterpret_cast<const ulonglong2 *>(p.rows + row * R);
+    bgym::Pcg64 g = bgym::pcg64_load(reinterpret_cast<const uint64_t *>(in));
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k += 2) {
+        const ulonglong2 v = __ldg(in + 2 + k / 2);
+        s[k] = __longlong_as_double((long long)v.x);
+        s[k + 1] = __longlong_as_double((long long)v.y);
+    }
+    const ulonglong2 tail = __ldg(in + 2 + E::S / 2);   // {elapsed | flags << 32, 0}
+    int32_t elapsed = (int32_t)(uint32_t)tail.x;
+    a.flags[f] = (uint8_t)(tail.x >> 32);
+    float o[E::D] = {};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, true> sink{{s, elapsed, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    const ReadActions src{};
+    for (int32_t t = 0; t < T; t++) {
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, b), action_int, a0);
+        if (advance_env<KIND>(a, sink, f, s, elapsed, action_int, a0)) reset_env_from<KIND>(sink, f, g);
+        act += a.n;
+    }
+    p.returns[b] = ret;
+    p.lengths[b] = len;
+    p.ended[b] = ended ? 1 : 0;
+    if constexpr (STATES) {
+        static_assert(E::S % 2 == 0 && 2 + E::S / 2 + 1 <= C, "row layout");
+        ulonglong2 *out = reinterpret_cast<ulonglong2 *>(p.end_rows + b * R);
+        out[0] = make_ulonglong2((unsigned long long)(uint64_t)(g.state >> 64), (unsigned long long)(uint64_t)g.state);
+        out[1] = make_ulonglong2((unsigned long long)(uint64_t)(g.inc >> 64), (unsigned long long)(uint64_t)g.inc);
+#pragma unroll
+        for (int k = 0; k < E::S; k += 2)
+            out[2 + k / 2] = make_ulonglong2((unsigned long long)__double_as_longlong(s[k]),
+                                             (unsigned long long)__double_as_longlong(s[k + 1]));
+        out[2 + E::S / 2] = make_ulonglong2((unsigned long long)(uint32_t)elapsed |
+                                                ((unsigned long long)a.flags[f] << 32), 0ULL);
+#pragma unroll
+        for (int c = 2 + E::S / 2 + 1; c < C; c++) out[c] = make_ulonglong2(0ULL, 0ULL);
+        store_row<E::D>(p.end_obs, b, o);
+    }
+}
+
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the
 // observation row.  References as in lunar_reset_env.
 template <int KIND>

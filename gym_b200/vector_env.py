@@ -420,11 +420,12 @@ class B200VectorEnv:
                            "an env with backend='torch'")
 
     # ------------------------------------------------------------------ step
-    def _device_actions(self, actions, captured=False, steps=False):
+    def _device_actions(self, actions, captured=False, steps=False, n=None, what=None):
         """Bring `actions` to a contiguous device tensor of a dtype the kernel reads directly.  steps=True: a leading
-        time axis of length >= 1, with the shape checked exactly (rollout)."""
+        time axis of length >= 1, with the shape checked exactly (rollout).  n: the batch size (default num_envs)."""
         torch = _torch()
-        what = "rollout()" if steps else "step()"
+        n = self.num_envs if n is None else n
+        what = what or ("rollout()" if steps else "step()")
         if captured and not (isinstance(actions, torch.Tensor) and actions.device == self.device):
             raise error.Error(f"{what} cannot be captured in a CUDA graph with actions that are not a CUDA tensor on "
                               f"{self.device}: the host-to-device copy cannot be replayed (got "
@@ -442,12 +443,12 @@ class B200VectorEnv:
                 actions, code = actions.to(torch.int32), _lib.ACT_I32
             else:
                 raise error.InvalidAction(f"Discrete actions must be integers, got {actions.dtype}")
-            shape = (self.num_envs,)
+            shape = (n,)
         else:
             if actions.dtype != torch.float32:
                 actions = actions.to(torch.float32)  # the Box dtype (e.g. pendulum.py:113-115)
             code = _lib.ACT_F32
-            shape = (self.num_envs, self.act_dim)
+            shape = (n, self.act_dim)
         if steps:
             if actions.dim() != len(shape) + 1 or tuple(actions.shape[1:]) != shape or actions.shape[0] < 1:
                 raise error.InvalidAction(f"expected actions of shape (T, {', '.join(map(str, shape))}) with T >= 1, "
@@ -749,6 +750,102 @@ class B200VectorEnv:
                                                         self._stream(), act)))
         return actions, outputs, obs, reward, term, trunc, infos
 
+    def rollout_from(self, snap, actions, *, rows=None, states=False):
+        """T steps of B branches, each from a snapshot row, without touching this env -> ``(returns, lengths, ended)``,
+        and with ``states=True`` also an ``EnvSnapshot`` of the B end states.
+
+        ``snap`` is an ``EnvSnapshot`` of this env or of any env of the same kind and construction config (anything
+        else raises ``error.Error``).  ``rows`` is None (branch b starts from row b, B = ``len(snap)``) or B row indices,
+        duplicates allowed: a CUDA tensor, whose out-of-range entries skip their branch (zero outputs, zero end row and
+        observation) and make the next call raise, as ``snapshot()`` / ``restore()`` do; or a host sequence, checked
+        here.  ``actions`` is (T, B) integers (Discrete) or (T, B, A) float32 (Box), as ``rollout()`` takes them.
+
+        Bit for bit, with ``twin`` a fresh env of the same id and config with B envs::
+
+            twin.restore(EnvSnapshot(snap.header, snap.rows[rows], snap.obs[rows]))
+            obs, r, te, tr, info = twin.rollout(actions)
+
+        the results are ``rollout_linear(summary=True)``'s fold of ``r``, ``te`` and ``tr`` over each branch's first
+        episode end t_end (T - 1 if none): float64 ``0.0 + r[0] + ... + r[t_end]`` in step order, int32 ``t_end + 1``
+        and bool; every branch takes all T steps.  The end states are ``twin.snapshot()``, with ``snap``'s header, and
+        go straight back into ``rollout_from``.  So the autoresets of K branches from one root draw the same reset
+        states, as K deep copies would; CartPole's ``autoreset=False`` flag comes from the row; an invalid Discrete
+        action gives a NaN reward and counts in this env's invalid-action counter.  This env's state, RNG records,
+        TimeLimit counters, observation buffers and action-space generator do not move, and it needs no ``reset()``.
+
+        MPPI, R roots of ``real`` with K sampled action sequences each (here CartPole, with a placeholder cost)::
+
+            snap = real.snapshot(roots)                                  # R rows
+            rows = torch.arange(R, device=dev).repeat_interleave(K)      # R * K branches
+            acts = torch.randint(0, 2, (T, R * K), device=dev)
+            returns, lengths, ended = real.rollout_from(snap, acts, rows=rows)   # real does not move
+            w = torch.softmax(returns.view(R, K) / temperature, dim=1)   # weights of the K sequences of each root
+
+        Tree expansion, the end states fed back in::
+
+            ret, _, _, leaves = real.rollout_from(snap, acts, rows=rows, states=True)
+            best = ret.topk(16).indices.repeat_interleave(K)              # K children of each of the 16 best leaves
+            ret2, _, _, deeper = real.rollout_from(leaves, acts2, rows=best, states=True)
+
+        Refused where ``rollout()`` is (``backend="numpy"``, ``wrappers=``, a pending async call), before any CUDA call.
+        The classic-control kinds run in one launch, one thread per branch, and may be captured in a CUDA graph: replays
+        read the current contents of ``snap.rows``, ``rows`` and ``actions`` (the first call with CUDA-tensor ``rows``
+        allocates the env's index-error flag, so make one outside the capture).  The Box2D kinds load the rows into a
+        scratch batch the env keeps and step it launch by launch; they cannot be captured (DESIGN.md §4.16)."""
+        captured = self._rollout_guards("rollout_from", reset_needed=False)
+        if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
+                         _lib.KIND_BIPEDALWALKER_HARDCORE):
+            refuse_capture("rollout_from() of a Box2D env", "it steps a scratch batch that is created on first use, "
+                           "through a scratch allocation per call")
+        if not isinstance(snap, EnvSnapshot):
+            raise error.Error(f"rollout_from() needs an EnvSnapshot, got {type(snap).__name__}")
+        R = self.snapshot_row_bytes
+        check_compatible(snap.header, self.kind, R, self._snapshot_config())
+        torch = _torch()
+        r = snap.rows
+        if not (isinstance(r, torch.Tensor) and r.dtype == torch.uint8 and r.device == self.device and r.dim() == 2
+                and r.shape[1] == R and r.is_contiguous()):
+            raise error.Error(f"rollout_from() needs the snapshot's rows as a contiguous uint8 (m, {R}) tensor on "
+                              f"{self.device}")
+        m = int(r.shape[0])
+        if rows is None:
+            idx, B = None, m
+        elif isinstance(rows, torch.Tensor) and rows.is_cuda:
+            if rows.dim() != 1 or rows.dtype.is_floating_point or rows.dtype == torch.bool or rows.device != self.device:
+                raise error.Error(f"rollout_from() rows must be a 1-D integer tensor on {self.device}, got {rows.dtype} "
+                                  f"of shape {tuple(rows.shape)} on {rows.device}")
+            idx, B = rows, int(rows.shape[0])
+        else:
+            if captured:
+                raise error.Error("rollout_from() cannot be captured in a CUDA graph with host rows: the host-to-device "
+                                  "copy cannot be replayed; pass a CUDA tensor")
+            idx = host_indices(rows.numpy() if isinstance(rows, torch.Tensor) else rows, m, "rollout_from rows")
+            B = int(idx.shape[0])
+        if B < 1:
+            raise error.Error("rollout_from() needs at least one branch, got B = 0")
+        act, code = self._device_actions(actions, captured, steps=True, n=B, what="rollout_from()")
+        T = int(act.shape[0])
+        if T > 2 ** 31 - 1:
+            raise error.Error(f"rollout_from() needs T < 2**31, got {T}")
+        if self.discrete and code != _lib.ACT_I64:
+            act, code = act.to(torch.int64), _lib.ACT_I64
+        if idx is not None:
+            idx = (torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx).to(self.device, torch.int64).contiguous()
+        dev, vp = self.device, ctypes.c_void_p
+        returns = torch.empty(B, dtype=torch.float64, device=dev)
+        lengths = torch.empty(B, dtype=torch.int32, device=dev)
+        ended = torch.empty(B, dtype=torch.bool, device=dev)
+        end_rows = torch.empty((B, R), dtype=torch.uint8, device=dev) if states else None
+        end_obs = torch.empty((B, self.obs_dim), dtype=torch.float32, device=dev) if states else None
+        _lib.check(self._lib.b200gym_rollout_from(
+            self._handle, vp(r.data_ptr()), m, None if idx is None else vp(idx.data_ptr()), B, vp(act.data_ptr()), code,
+            T, vp(returns.data_ptr()), vp(lengths.data_ptr()), vp(ended.data_ptr()),
+            vp(end_rows.data_ptr()) if states else None, vp(end_obs.data_ptr()) if states else None, self._stream()),
+            self._handle)
+        if states:
+            return returns, lengths, ended, EnvSnapshot(snap.header, end_rows, end_obs)
+        return returns, lengths, ended
+
     def _noise_steps(self, noise):
         """Check rollout_mlp_noisy()'s noise without a CUDA call -> T."""
         torch = _torch()
@@ -853,9 +950,10 @@ class B200VectorEnv:
                              f"({self.num_envs}, {P}) for one per env; got {tuple(params.shape)}")
         return widths[0], widths[1] if len(widths) == 2 else 0, per_env, _lib.MLP_ACTIVATIONS[activation]
 
-    def _rollout_guards(self, what):
-        """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp() / rollout_mlp_noisy(), all
-        raised before any CUDA call -> whether a CUDA graph is being captured."""
+    def _rollout_guards(self, what, reset_needed=True):
+        """The refusals of rollout() / rollout_sampled() / rollout_linear() / rollout_mlp() / rollout_mlp_noisy() /
+        rollout_from(), all raised before any CUDA call -> whether a CUDA graph is being captured.  rollout_from()
+        reads none of the env's state, so it passes reset_needed=False."""
         self._assert_open(what)
         if self.backend == "numpy":
             raise error.Error(f"{what}() needs backend='torch': backend='numpy' steps through host buffers")
@@ -865,7 +963,7 @@ class B200VectorEnv:
         if self._state != _STATE_DEFAULT:
             raise error.AlreadyPendingCallError(
                 f"Calling `{what}` while waiting for a pending call to `{self._state}` to complete.", self._state)
-        if not self._has_reset:
+        if reset_needed and not self._has_reset:
             raise error.ResetNeeded(f"Cannot call env.{what}() before calling env.reset()")
         captured = capturing()
         # the same poll as step_async: an invalid action of an earlier call raises here (not while capturing)

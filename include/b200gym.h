@@ -387,6 +387,32 @@ int b200gym_clone(b200gym_t *h, const int64_t *src_dev, void *stream);
 int b200gym_snapshot_index_error(b200gym_t *h);
 
 /*
+ * T steps of B branches, each from a snapshot row, touching none of the handle's envs.  Branch b is what a fresh
+ * handle of the same kind and configuration with B envs computes after loading row row_idx_dev[b] (row b if
+ * row_idx_dev is NULL) into env b and running b200gym_rollout with the branch's column of actions: its autoresets
+ * draw from its own copy of the row's PCG64 record, and CartPole's autoreset=False flag byte comes from the row.
+ *   snap_rows_dev  n_rows rows of b200gym_snapshot_row_bytes(kind) bytes, 128-byte aligned, from a handle of the same
+ *                  kind and configuration (the caller checks that; the rows carry no header)
+ *   row_idx_dev    NULL (then n_rows >= B), or [B] int64 row indices on the device; duplicates allowed.  An index out of
+ *                  [0, n_rows) skips its branch: zero outputs (end row and observation included), and the flag of
+ *                  b200gym_snapshot_index_error() raised
+ *   actions_dev    [T][B] int64 (Discrete kinds) or [T][B][act_dim] float32 (Box kinds); action_dtype says which.
+ *                  An invalid Discrete action gives a NaN reward and counts in this handle's invalid-action counter
+ *   T              >= 1; B >= 1
+ *   returns_dev, lengths_dev, ended_dev   [B] float64 / int32 / uint8: b200gym_rollout_linear's summary of each
+ *                  branch (first episode end t_end, or T - 1): 0.0 + reward[0] + ... + reward[t_end], t_end + 1, ended
+ *   end_rows_dev, end_obs_dev   both NULL, or [B] rows (128-byte aligned, the layout b200gym_snapshot_save writes,
+ *                  padding zero) and [B][obs_dim] float32 observations of the branches' end states
+ * Classic-control kinds: ONE launch, one thread per branch, the state, PCG64 stream and TimeLimit counter in registers;
+ * may be captured in a CUDA graph (the first call with row_idx_dev allocates the index-error flag: make it outside a
+ * capture).  Box2D kinds: the rows loaded into a handle-owned scratch batch of at least B envs (created on first use,
+ * recreated when B grows), the b200gym_step sequence per step, and a save of the scratch batch; not capturable.
+ */
+int b200gym_rollout_from(b200gym_t *h, const void *snap_rows_dev, int64_t n_rows, const int64_t *row_idx_dev, int64_t B,
+                         const void *actions_dev, int action_dtype, int32_t T, double *returns_dev, int32_t *lengths_dev,
+                         uint8_t *ended_dev, void *end_rows_dev, float *end_obs_dev, void *stream);
+
+/*
  * LunarLander only (state_dim is 0 for it; get/set_state handle the TimeLimit counters and RNG):
  * the three rigid bodies {lander, leg(-1), leg(+1)} of every env as float32 [n][18] =
  * 3 x {c.x, c.y, angle, v.x, v.y, omega} and int32 [n][6] = {game_over, leg0 contact, leg1 contact,
