@@ -475,6 +475,41 @@ __global__ void __launch_bounds__(kThreads) mlp_noisy_policy_kernel(const float 
     }
 }
 
+// The CTA's shared copies of two nets, mlp_stage's for each: the `na` floats at a, then, from the next 16-byte boundary,
+// the `nc` floats at c.  Returns the copy of c; the copy of a is at the start of the dynamic shared memory
+__device__ __forceinline__ const float *mlp_stage_pair(const float *a, int64_t na, const float *c, int64_t nc) {
+    extern __shared__ float4 mlp_shared[];
+    float *s = reinterpret_cast<float *>(mlp_shared), *sc = s + (na + 3) / 4 * 4;
+    for (int64_t q = threadIdx.x; q < na; q += blockDim.x) s[q] = __ldg(a + q);
+    for (int64_t q = threadIdx.x; q < nc; q += blockDim.x) sc[q] = __ldg(c + q);
+    __syncthreads();
+    return sc;
+}
+
+// ... with the noisy actor's actions and the critic's values (rollout_actor_critic_env).  Both nets are shared by every
+// env and staged in shared memory once per CTA, the actor first; launch bounds as the shared-policy noisy kernels
+template <int KIND, int ACT>
+__global__ void __launch_bounds__(kThreads, 2)
+    rollout_actor_critic_kernel(const StepArgs a, const int32_t T, float *last_obs, const ActorCriticArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    using Src = MlpNoisyActions<KIND, false, ACT>;
+    const int h1 = p.actor.mlp.h1, h2 = p.actor.mlp.h2;
+    const float *wc = mlp_stage_pair(p.actor.mlp.params, mlp_param_count<Src::K, Src::D>(h1, h2), p.critic,
+                                     mlp_param_count<1, Src::D>(h1, h2));
+    extern __shared__ float4 mlp_shared[];
+    if (i < a.n) rollout_actor_critic_env<KIND, ACT>(a, i, T, last_obs, reinterpret_cast<const float *>(mlp_shared),
+                                                     wc, p);
+}
+
+// The advantages of a b200gym_rollout_actor_critic call, one thread per env (gae_env), after the rollout: a launch of
+// its own for every kind, so the rollout kernel keeps its registers and the Box2D path shares it
+__global__ void __launch_bounds__(kThreads) gae_kernel(const double *reward, const uint8_t *term, const uint8_t *trunc,
+                                                       const float *values, float *adv, int64_t n, int32_t T, float g,
+                                                       float gl) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) gae_env(i, n, T, g, gl, reward, term, trunc, values, adv);
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -2667,14 +2702,20 @@ static int launch_rollout_linear_kind(b200gym *h, const StepArgs &a, int32_t T, 
 // mlp_noisy_policy_kernel) with the arguments args_at(t) from the observation rows of the step before (first_obs for
 // step 0), with `smem` bytes of dynamic shared memory, then launch_step_box2d into slice t.  Summary mode: every step
 // runs in one scratch slice, and the policy launch of step t + 1 (or one last launch, with args_at(T - 1)) folds step t
-// into the summary.  kernel / entry: names for the error messages
-template <typename Args, typename ArgsAt>
+// into the summary.  kernel / entry: names for the error messages.  hook(t, obs_in, s, after): launches of the
+// caller's own around step t, made before the policy launch (after false, obs_in the policy's input) and after the
+// step sequence (after true, s the step's outputs); non-zero fails the rollout
+struct NoStepHook {
+    int operator()(int32_t, const float *, const StepArgs &, bool) const { return 0; }
+};
+
+template <typename Args, typename ArgsAt, typename Hook = NoStepHook>
 static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
                                        const float *first_obs, const ArgsAt &args_at,
                                        void (*policy)(const float *, void *, const Args, const double *,
                                                       const uint8_t *, const uint8_t *, int64_t, int32_t, int, int),
                                        size_t smem, bool summary, cudaStream_t st, const char *kernel,
-                                       const char *entry) {
+                                       const char *entry, const Hook &hook = Hook{}) {
     const int64_t n = h->n, D = h->D, cols = std::max(h->A, 1);
     const size_t act_row = (size_t)n * cols * (h->A == 0 ? sizeof(long long) : sizeof(float));
     const int action_dtype = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
@@ -2704,11 +2745,13 @@ static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T,
             s.truncated = a.truncated + t * n;
             s.final_obs = a.final_obs ? a.final_obs + t * n * D : nullptr;
         }
+        if ((rc = hook(t, obs_in, s, false))) break;
         policy<<<blocks, kThreads, smem, st>>>(obs_in, const_cast<void *>(s.actions), args_at(t), s.reward,
                                                s.terminated, s.truncated, n, summary ? t - 1 : -1, 1,
                                                summary && t == 0);
         if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: launch failed", kernel);
         else rc = launch_step_box2d(h, s, action_dtype, st);
+        if (!rc) rc = hook(t, obs_in, s, true);
     }
     if (!rc && summary) {
         policy<<<blocks, kThreads, smem, st>>>(s.obs, nullptr, args_at(T - 1), s.reward, s.terminated, s.truncated,
@@ -2975,6 +3018,134 @@ extern "C" int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_d
     if (activation == B200GYM_MLP_TANH)
         return launch_rollout_mlp_noisy<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
     return launch_rollout_mlp_noisy<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
+}
+
+// ---- on-policy collection with a critic (b200gym_rollout_actor_critic) ----
+static int launch_gae(b200gym *h, const StepArgs &a, int32_t T, const ActorCriticArgs &p, float g, float gl,
+                      cudaStream_t st) {
+    gae_kernel<<<blocks_for(h->n), kThreads, 0, st>>>(a.reward, a.terminated, a.truncated, p.values, p.advantages, h->n,
+                                                      T, g, gl);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+template <int KIND, int ACT>
+static int launch_rollout_actor_critic_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                            const ActorCriticArgs &p, size_t smem, float g, float gl,
+                                            cudaStream_t st) {
+    rollout_actor_critic_kernel<KIND, ACT><<<blocks_for(h->n), kThreads, smem, st>>>(a, T, last_obs, p);
+    CK(h, cudaGetLastError());
+    return launch_gae(h, a, T, p, g, gl, st);
+}
+
+// Composed launch by launch: around the noisy policy launch and step sequence of step t, the critic (mlp_policy_kernel
+// with K = 1, whose Box "action" is V) on the step's input rows into values[t], and after it on the step's final
+// observation rows into advantages[t], the holding slot gae_kernel reads where the step truncated without terminating
+// (every row is evaluated, the others are overwritten unread).  Then the critic on the last observations into
+// values[T], and gae_kernel
+template <int K, int D, bool DISCRETE, int ACT>
+static int launch_rollout_actor_critic_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                             const float *first_obs, const ActorCriticArgs &p, size_t smem_actor,
+                                             size_t smem_critic, float g, float gl, cudaStream_t st) {
+    const int64_t n = h->n, slice = n * K;
+    const MlpPolicyArgs c{p.critic, 0, p.actor.mlp.h1, p.actor.mlp.h2, p.actor.mlp.vec, nullptr, nullptr, nullptr};
+    const unsigned blocks = blocks_for(n);
+    auto critic = [&](const float *obs, float *out) {
+        mlp_policy_kernel<1, D, false, false, ACT><<<blocks, kThreads, smem_critic, st>>>(obs, out, c, nullptr, nullptr,
+                                                                                        nullptr, n, -1, 1, 0);
+        return cudaGetLastError() != cudaSuccess ? fail(h, "mlp_policy_kernel (critic): launch failed") : 0;
+    };
+    int rc = launch_rollout_policy_box2d(
+        h, a, T, last_obs, first_obs,
+        [&](int32_t t) {
+            MlpNoisyArgs q = p.actor;
+            q.noise = p.actor.noise + t * slice;
+            q.outputs = p.actor.outputs + t * slice;
+            return q;
+        },
+        mlp_noisy_policy_kernel<K, D, DISCRETE, false, ACT>, smem_actor, false, st, "mlp_noisy_policy_kernel",
+        "b200gym_rollout_actor_critic", [&](int32_t t, const float *obs_in, const StepArgs &s, bool after) {
+            return after ? critic(s.final_obs, p.advantages + t * n) : critic(obs_in, p.values + t * n);
+        });
+    if (!rc) rc = critic(last_obs, p.values + (int64_t)T * n);
+    return rc ? rc : launch_gae(h, a, T, p, g, gl, st);
+}
+
+template <int ACT>
+static int launch_rollout_actor_critic(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                       const float *first_obs, const ActorCriticArgs &p, size_t smem_actor,
+                                       size_t smem_critic, float g, float gl, cudaStream_t st) {
+    const size_t smem = smem_actor + smem_critic;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_actor_critic_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, smem, g, gl, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_actor_critic_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, smem, g, gl, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_actor_critic_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, smem, g, gl, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_actor_critic_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, smem, g, gl, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_actor_critic_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, smem, g, gl, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_actor_critic_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, smem_actor,
+                                                                  smem_critic, g, gl, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_actor_critic_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, smem_actor,
+                                                                   smem_critic, g, gl, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_actor_critic_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, smem_actor,
+                                                                    smem_critic, g, gl, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+extern "C" int b200gym_rollout_actor_critic(b200gym_t *h, const float *actor_dev, const float *critic_dev,
+                                            int n_layers, int h1, int h2, int32_t T, const float *noise_dev,
+                                            float *outputs_dev, void *actions_out_dev, float *obs_dev,
+                                            double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                            float *final_obs_dev, float *values_dev, float *advantages_dev,
+                                            float gamma, float gamma_lambda, float *last_obs_dev,
+                                            const float *first_obs_dev, void *stream, int activation) {
+    if (!h) return fail(h, "b200gym_rollout_actor_critic: null handle");
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "b200gym_rollout_actor_critic: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)",
+                    activation);
+    if (n_layers != 1 && n_layers != 2)
+        return fail(h, "b200gym_rollout_actor_critic: n_layers must be 1 or 2 (got %d)", n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "b200gym_rollout_actor_critic: hidden widths must be 1 .. %d (got %d, %d)", kMlpMaxWidth, h1,
+                    h2);
+    if (T < 1) return fail(h, "b200gym_rollout_actor_critic: T must be at least 1 (got %d)", T);
+    if (!(gamma >= 0.0f && gamma <= 1.0f && gamma_lambda >= 0.0f && gamma_lambda <= 1.0f))
+        return fail(h, "b200gym_rollout_actor_critic: gamma and gamma_lambda must be in [0, 1] (got %g, %g)",
+                    (double)gamma, (double)gamma_lambda);
+    if (!actor_dev || !critic_dev || !noise_dev || !outputs_dev || !actions_out_dev || !obs_dev || !reward_dev ||
+        !terminated_dev || !truncated_dev || !values_dev || !advantages_dev || !last_obs_dev)
+        return fail(h, "b200gym_rollout_actor_critic: null buffer");
+    if (!final_obs_dev || !h->cfg.autoreset)
+        return fail(h, "b200gym_rollout_actor_critic: the truncation bootstrap needs autoreset and final_obs_dev");
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "b200gym_rollout_actor_critic: a Box2D env needs first_obs_dev");
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t Pa = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    const int64_t Pc = h2 == 0 ? h1 * D + h1 + h1 + 1 : h1 * D + h1 + (int64_t)h2 * h1 + h2 + h2 + 1;
+    // the shared copies start 16-byte aligned, so h1 % 4 == 0 is all the 16-byte rows of either net need
+    const bool vec = h1 % 4 == 0;
+    const ActorCriticArgs p{{{actor_dev, 0, h1, h2, vec ? 1 : 0, nullptr, nullptr, nullptr}, noise_dev, outputs_dev},
+                            critic_dev, values_dev, advantages_dev};
+    // at most 37.9 KB (Acrobot at (64, 64): 4803 + 4673 floats): no opt-in needed
+    const size_t smem_actor = (size_t)(Pa + 3) / 4 * 16, smem_critic = (size_t)(Pc + 3) / 4 * 16;
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_actor_critic<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, smem_actor,
+                                                             smem_critic, gamma, gamma_lambda, st);
+    return launch_rollout_actor_critic<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, smem_actor,
+                                                         smem_critic, gamma, gamma_lambda, st);
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------

@@ -830,6 +830,122 @@ __device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t
     a.elapsed[i] = elapsed;
 }
 
+// ---- on-policy collection with a critic (b200gym_rollout_actor_critic) --------------------------------------------
+
+// The arguments of a b200gym_rollout_actor_critic launch: the actor and its noise and outputs (one actor shared by every
+// env, so actor.mlp.stride is 0), the critic (the actor's widths, one output), and slice 0 of the [T + 1][n] values and
+// of the [T][n] advantages.  Until gae_kernel runs, advantages[t][i] holds V(final observation) where step t of env i
+// truncated without terminating, and nothing anywhere else
+struct ActorCriticArgs {
+    MlpNoisyArgs actor;
+    const float *critic;
+    float *values;
+    float *advantages;
+};
+
+// The sink of an actor-critic rollout: LinearSink's, plus a register copy of the step's flags and of its final
+// observation, from which the driver evaluates the critic where the step truncated without terminating
+template <int KIND>
+struct CriticSink : LinearSink<KIND, false> {
+    using Base = LinearSink<KIND, false>;
+    float (&fin)[bgym::Env<KIND>::D];
+    uint8_t &te, &tr;
+    template <typename I>
+    __device__ __forceinline__ void scalars(I i, double reward, uint8_t term, uint8_t trunc) const {
+        Base::scalars(i, reward, term, trunc);
+        te = term;
+        tr = trunc;
+    }
+    template <int D, typename I>
+    __device__ __forceinline__ void final_obs(I i, const float (&v)[D]) const {
+        Base::template final_obs<D>(i, v);
+#pragma unroll
+        for (int k = 0; k < D; k++) fin[k] = v[k];
+    }
+};
+
+// T steps of env i under the noisy actor at wa with the critic at wc (rollout_actor_critic_kernel): rollout_mlp_noisy_env's
+// loop, written out again so that no pre-existing kernel changes, with the critic evaluated at every step on the
+// observation the actor reads, V(o) stored to values[t], and on the final observation of a step that truncated without
+// terminating, V stored to the holding slot advantages[t][i].  After the loop, values[T] = V(the observation the call
+// leaves the env at).  The caller's autoreset must be on: the bootstrap reads the final observations.  wa and wc are
+// the CTA's shared copies (mlp_stage_pair), so both nets read the same widths and the same vec
+template <int KIND, int ACT = B200GYM_MLP_RELU>
+__device__ __forceinline__ void rollout_actor_critic_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                         const float *wa, const float *wc, const ActorCriticArgs &p) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    const int h1 = p.actor.mlp.h1, h2 = p.actor.mlp.h2;
+    const bool vec = p.actor.mlp.vec != 0;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D], fin[E::D];
+    E::observe(s, o);
+    MlpNoisyActions<KIND, false, ACT> src{wa, h1, h2, vec, o, p.actor.noise, p.actor.outputs};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    uint8_t te = 0, tr = 0;
+    CriticSink<KIND> sink{{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                           o, ret, len, ended},
+                          fin, te, tr};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    float *values = p.values, *held = p.advantages;
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        float v[1];
+        mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, o, v);
+        store_once(values + i, v[0]);
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        if (tr && !te) {
+            mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, fin, v);
+            store_once(held + i, v[0]);
+        }
+        act += n;
+        values += n;
+        held += n;
+        src.next(n);
+        sink.next(n);
+    }
+    float v[1];
+    mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, o, v);
+    store_once(values + i, v[0]);
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
+// The GAE recursion of env i over the T steps of a b200gym_rollout_actor_critic call (gae_kernel), in float32, every
+// operation rounded, no fused multiply-add (the library is built with -fmad=false, the host build with
+// -ffp-contract=off), with g = gamma and gl = gamma * gae_lambda already rounded to float32:
+//   r = (float)reward[t]; adv[T] = +0.0; for t = T-1 .. 0:
+//   terminated: delta = r - V[t]; else truncated: delta = (r + g * Vf[t]) - V[t]; else delta = (r + g * V[t+1]) - V[t]
+//   adv[t] = delta if terminated or truncated, else delta + gl * adv[t+1]
+// Vf[t] is read from adv's own slot t (rollout_actor_critic_env leaves it there), which the step then overwrites.  All
+// arrays are [T][n] but values, [T + 1][n]
+__host__ __device__ __forceinline__ void gae_env(int64_t i, int64_t n, int32_t T, float g, float gl,
+                                                 const double *reward, const uint8_t *term, const uint8_t *trunc,
+                                                 const float *values, float *adv) {
+    float next = 0.0f;
+    for (int32_t t = T - 1; t >= 0; t--) {
+        const int64_t k = (int64_t)t * n + i;
+        const float r = (float)reward[k], v = values[k];
+        const bool te = term[k] != 0, tr = trunc[k] != 0;
+        float delta;
+        if (te) delta = r - v;
+        else if (tr) delta = (r + g * adv[k]) - v;
+        else delta = (r + g * values[k + n]) - v;
+        next = (te || tr) ? delta : delta + gl * next;
+        adv[k] = next;
+    }
+}
+
 // ---- rollouts from snapshot rows (b200gym_rollout_from) ------------------------------------------------------------
 
 // The snapshot row of a classic kind (b200gym.cu, snapshot_save_kernel): the PCG64 record {state_hi, state_lo, inc_hi,

@@ -28,6 +28,7 @@ Two output backends:
     ``infos`` that only appear when some env finished.
 """
 import ctypes
+import math
 import os
 import time
 
@@ -750,6 +751,114 @@ class B200VectorEnv:
                                                         self._stream(), act)))
         return actions, outputs, obs, reward, term, trunc, infos
 
+    def rollout_actor_critic(self, actor, critic, hidden, noise, *, gamma, gae_lambda, activation="relu"):
+        """One on-policy collection step of PPO / A2C: ``rollout_mlp_noisy()`` with a critic evaluated next to each env's
+        state, and the GAE advantages -> ``(actions, outputs, values, advantages, obs, rewards, terminateds,
+        truncateds, infos)``.
+
+        ``actions``, ``outputs``, ``obs``, ``rewards``, ``terminateds``, ``truncateds`` and ``infos`` are bit for bit
+        what ``rollout_mlp_noisy(actor, hidden, noise, activation=activation)`` returns, and the env is left where that
+        call leaves it.  ``actor`` is one packed actor, shape (P_actor,): per-env rows (N, P) raise ``ValueError``,
+        because PPO and A2C train one network and per-env rows would double the kernels for no caller.  ``critic`` is
+        one packed critic of shape (P_critic,), ``parameters_to_vector(nn.Sequential(nn.Linear(D, h1), act,
+        [nn.Linear(h1, h2), act,] nn.Linear(h_last, 1)))``: the actor's ``hidden`` and ``activation`` (the defaults of
+        CleanRL and Stable-Baselines3), ``rollout_mlp()``'s arithmetic with one output.  Both float32, contiguous, on
+        the env's device.
+
+        ``values`` is float32 (T + 1, N): ``values[t]`` is V(the observation step t acts on), starting at the one the
+        env last returned, and ``values[T]`` is V(the observation the call leaves the env at), CleanRL's
+        ``next_value``, bit-equal to the next call's ``values[0]``.  ``advantages`` is float32 (T, N), every float32
+        operation rounded, no fused multiply-add, with ``g = float32(gamma)``, ``gl = float32(gamma * gae_lambda)``
+        (the product in float64), ``r[t] = float32(rewards[t])`` and ``Vf[t]`` = V(``infos["final_observation"][t]``)::
+
+            adv[T] = +0.0
+            for t = T-1 .. 0:
+                if terminated[t]:   delta = r[t] - values[t]
+                elif truncated[t]:  delta = (r[t] + g * Vf[t]) - values[t]
+                else:               delta = (r[t] + g * values[t+1]) - values[t]
+                adv[t] = delta if (terminated[t] or truncated[t]) else delta + gl * adv[t+1]
+
+        That is CleanRL's recursion with Stable-Baselines3's bootstrap of a time-limit end from the final observation.
+        ``gamma`` and ``gae_lambda`` are required keywords, real and finite in [0, 1].  The env must autoreset (the
+        bootstrap reads the final observations); ``autoreset=False`` raises ``error.Error``.
+
+        A CleanRL-shaped PPO collection, Discrete actions::
+
+            actor = nn.Sequential(nn.Linear(D, 64), nn.Tanh(), nn.Linear(64, 64), nn.Tanh(), nn.Linear(64, K)).cuda()
+            critic = nn.Sequential(nn.Linear(D, 64), nn.Tanh(), nn.Linear(64, 64), nn.Tanh(), nn.Linear(64, 1)).cuda()
+            pa = torch.nn.utils.parameters_to_vector(actor.parameters()).detach()
+            pc = torch.nn.utils.parameters_to_vector(critic.parameters()).detach()
+            first_obs = obs_now                                            # what the env last returned
+            u = torch.rand(T, N, K, device=dev).clamp_(min=torch.finfo(torch.float32).tiny)
+            g = -torch.log(-torch.log(u))                                 # Gumbel: samples softmax(logits)
+            a, logits, values, adv, obs, r, te, tr, info = envs.rollout_actor_critic(
+                pa, pc, (64, 64), g, gamma=0.99, gae_lambda=0.95, activation="tanh")
+            obs_in = torch.cat([first_obs[None], obs[:-1]])               # the inputs the actions were taken at
+            logp = torch.distributions.Categorical(logits=logits).log_prob(a)
+            returns = adv + values[:-1]
+            obs_now = obs[-1]
+
+        For Box actions draw ``std * torch.randn(T, N, K)`` instead of ``g``; then ``outputs`` is the mean and
+        ``logp = torch.distributions.Normal(mean, std).log_prob(a).sum(-1)``.
+
+        Guards and the start from the current state are ``rollout_mlp_noisy()``'s.  The classic-control kinds run the
+        rollout in one launch, both nets staged in shared memory, then one launch for the advantages; they may be
+        captured in a CUDA graph, and replays read the current contents of ``actor``, ``critic`` and ``noise``, while
+        ``gamma`` and ``gae_lambda`` are fixed at capture.  The Box2D kinds compose the same results launch by launch
+        and cannot be captured (DESIGN.md §4.17)."""
+        what = "rollout_actor_critic"
+        captured = self._rollout_guards(what)
+        if not self.autoreset:
+            raise error.Error(f"{what}() needs autoreset=True: the bootstrap of a truncated episode reads its final "
+                              "observation, which only an autoresetting env reports")
+        h1, h2, per_env, act = self._mlp_params(actor, hidden, activation, what)
+        if per_env:
+            raise ValueError(f"{what}() takes one actor shared by every env, shape ({actor.shape[1]},); got per-env rows "
+                             f"{tuple(actor.shape)}")
+        self._critic_params(critic, hidden, what)
+        g, gl = self._gae_coefficients(gamma, gae_lambda, what)
+        T = self._noise_steps(noise, what)
+        self._refuse_box2d_capture(what)
+        torch = _torch()
+        outputs = torch.empty_like(noise)
+        values = torch.empty((T + 1, self.num_envs), dtype=torch.float32, device=self.device)
+        advantages = torch.empty((T, self.num_envs), dtype=torch.float32, device=self.device)
+        vp = ctypes.c_void_p
+        actions, obs, reward, term, trunc, infos = self._policy_rollout(
+            what, T, False, captured, lambda T, outs, last, first: (
+                self._lib.b200gym_rollout_actor_critic(
+                    self._handle, vp(actor.data_ptr()), vp(critic.data_ptr()), len(hidden), h1, h2, T,
+                    vp(noise.data_ptr()), vp(outputs.data_ptr()), *outs[:6], vp(values.data_ptr()),
+                    vp(advantages.data_ptr()), g, gl, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act)))
+        return actions, outputs, values, advantages, obs, reward, term, trunc, infos
+
+    def _critic_params(self, critic, hidden, what):
+        """Check rollout_actor_critic()'s critic, D -> hidden -> 1, without a CUDA call."""
+        torch = _torch()
+        sizes = [self.obs_dim] + [int(h) for h in hidden] + [1]
+        P = sum(o * i + o for i, o in zip(sizes[:-1], sizes[1:]))
+        if not isinstance(critic, torch.Tensor):
+            raise ValueError(f"{what}() needs critic as a torch tensor, got {type(critic).__name__}")
+        if critic.dtype != torch.float32:
+            raise ValueError(f"{what}() needs a float32 critic, got {critic.dtype}")
+        if critic.device != self.device:
+            raise ValueError(f"{what}() needs the critic on {self.device}, got {critic.device}")
+        if not critic.is_contiguous():
+            raise ValueError(f"{what}() needs a contiguous critic")
+        if tuple(critic.shape) != (P,):
+            raise ValueError(f"{what}() with hidden {tuple(sizes[1:-1])} needs one critic of shape ({P},), shared by "
+                             f"every env; got {tuple(critic.shape)}")
+
+    @staticmethod
+    def _gae_coefficients(gamma, gae_lambda, what):
+        """Check gamma and gae_lambda (real, finite, in [0, 1]) -> (float32(gamma), float32(gamma * gae_lambda)),
+        the product taken in float64, as Python floats that hold float32 values."""
+        for name, x in (("gamma", gamma), ("gae_lambda", gae_lambda)):
+            if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)) or not (
+                    math.isfinite(float(x)) and 0.0 <= float(x) <= 1.0):
+                raise ValueError(f"{what}() needs {name} a real number in [0, 1], got {x!r}")
+        return float(np.float32(float(gamma))), float(np.float32(float(gamma) * float(gae_lambda)))
+
     def rollout_from(self, snap, actions, *, rows=None, states=False):
         """T steps of B branches, each from a snapshot row, without touching this env -> ``(returns, lengths, ended)``,
         and with ``states=True`` also an ``EnvSnapshot`` of the B end states.
@@ -846,20 +955,20 @@ class B200VectorEnv:
             return returns, lengths, ended, EnvSnapshot(snap.header, end_rows, end_obs)
         return returns, lengths, ended
 
-    def _noise_steps(self, noise):
-        """Check rollout_mlp_noisy()'s noise without a CUDA call -> T."""
+    def _noise_steps(self, noise, what="rollout_mlp_noisy"):
+        """Check rollout_mlp_noisy()'s or rollout_actor_critic()'s noise without a CUDA call -> T."""
         torch = _torch()
         K = int(self.single_action_space.n if self.discrete else self.act_dim)
         if not isinstance(noise, torch.Tensor):
-            raise ValueError(f"rollout_mlp_noisy() needs noise as a torch tensor, got {type(noise).__name__}")
+            raise ValueError(f"{what}() needs noise as a torch tensor, got {type(noise).__name__}")
         if noise.dtype != torch.float32:
-            raise ValueError(f"rollout_mlp_noisy() needs float32 noise, got {noise.dtype}")
+            raise ValueError(f"{what}() needs float32 noise, got {noise.dtype}")
         if noise.device != self.device:
-            raise ValueError(f"rollout_mlp_noisy() needs noise on {self.device}, got {noise.device}")
+            raise ValueError(f"{what}() needs noise on {self.device}, got {noise.device}")
         if not noise.is_contiguous():
-            raise ValueError("rollout_mlp_noisy() needs contiguous noise")
+            raise ValueError(f"{what}() needs contiguous noise")
         if noise.dim() != 3 or tuple(noise.shape[1:]) != (self.num_envs, K) or not 1 <= noise.shape[0] <= 2 ** 31 - 1:
-            raise ValueError(f"rollout_mlp_noisy() needs noise (T, {self.num_envs}, {K}) with 1 <= T < 2**31, got "
+            raise ValueError(f"{what}() needs noise (T, {self.num_envs}, {K}) with 1 <= T < 2**31, got "
                              f"{tuple(noise.shape)}")
         return int(noise.shape[0])
 

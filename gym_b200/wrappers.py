@@ -83,6 +83,13 @@ class VectorWrapper:
                           "a fused rollout of the wrapped env would skip it; call step() with the policy's actions T "
                           "times instead")
 
+    def rollout_actor_critic(self, actor, critic, hidden, noise, *, gamma, gae_lambda, activation="relu"):
+        """Refused, as rollout(): step the wrapper with the policy's actions instead."""
+        from gym_b200 import error
+        raise error.Error(f"{type(self).__name__} does not support rollout_actor_critic(): it acts after every step, "
+                          "and a fused rollout of the wrapped env would skip it; call step() with the policy's actions "
+                          "T times instead")
+
     def rollout_from(self, snap, actions, *, rows=None, states=False):
         """Refused, as rollout(): restore the snapshot into the wrapper's env and step the wrapper instead."""
         from gym_b200 import error

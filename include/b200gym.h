@@ -297,6 +297,31 @@ int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_dev, int per
                                   float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
                                   int activation);
 
+/*
+ * b200gym_rollout_mlp_noisy_act with one actor shared by every env (actor_dev, P floats), plus a critic and the GAE
+ * advantages: one on-policy collection step of PPO / A2C.
+ *   critic_dev        the packed critic D -> h1 (-> h2) -> 1, the actor's widths and activation, b200gym_rollout_mlp's
+ *                     arithmetic with K = 1
+ *   final_obs_dev     required: the bootstrap of a truncated episode reads it, so the handle must autoreset
+ *   values_dev        float32 [T + 1][n]: values[t] = V(the observation step t acts on), values[T] = V(the observation
+ *                     the call leaves the env at)
+ *   advantages_dev    float32 [T][n], from g = gamma and gl = gamma * gae_lambda (both in [0, 1], rounded to float32 by
+ *                     the caller), every float32 operation rounded, no fused multiply-add, adv[T] = +0.0, and for
+ *                     t = T-1 .. 0 with r = (float)reward[t]:
+ *                       terminated:       delta = r - values[t]
+ *                       else truncated:   delta = (r + g * V(final_obs[t])) - values[t]
+ *                       else:             delta = (r + g * values[t + 1]) - values[t]
+ *                       adv[t] = delta if terminated or truncated, else delta + gl * adv[t + 1]
+ * Classic-control kinds: the rollout in ONE launch, then one GAE launch.  Box2D kinds: per step, a critic launch, the
+ * policy launch and the b200gym_step sequence, then a critic launch on the final observations; then the GAE launch.
+ */
+int b200gym_rollout_actor_critic(b200gym_t *h, const float *actor_dev, const float *critic_dev, int n_layers, int h1,
+                                 int h2, int32_t T, const float *noise_dev, float *outputs_dev, void *actions_out_dev,
+                                 float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                 float *final_obs_dev, float *values_dev, float *advantages_dev, float gamma,
+                                 float gamma_lambda, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                 int activation);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
