@@ -149,6 +149,12 @@ SIGNATURES = {
                                              _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200gym_rollout_actor_critic": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32] + [_vp] * 10 +
                                      [ctypes.c_float, ctypes.c_float, _vp, _vp, _vp, _i32]),
+    "b200gym_rollout_mlp_noisy_norm": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, ctypes.c_double,
+                                               ctypes.c_float]),
+    "b200gym_rollout_actor_critic_norm": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32] + [_vp] * 10 +
+                                          [ctypes.c_float, ctypes.c_float, _vp, _vp, _vp, _i32, _vp, _vp,
+                                           ctypes.c_double, ctypes.c_float, _vp, ctypes.c_float]),
     "b200gym_invalid_actions": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_invalid_seen": (_i32, [_vp]),
     "b200gym_host_buffers": (_i32, [_vp, ctypes.POINTER(HostIO)]),

@@ -111,6 +111,7 @@ struct b200gym {
     unsigned long long *snap_bad_dev = nullptr;   // device alias
     unsigned char *snap_scratch = nullptr;        // b200gym_clone: n rows
     b200gym *from_batch = nullptr;                // b200gym_rollout_from, Box2D kinds: scratch batch (lazily created)
+    float *norm_rows = nullptr;                   // normalised rollouts, Box2D kinds: n rows of D network inputs (lazily)
     // per-env wrapper chain (b200gym_subenv_set); the host-buffer path runs it inside its calls
     struct {
         bool on = false, out_f64 = false, episode = false;
@@ -508,6 +509,59 @@ __global__ void __launch_bounds__(kThreads) gae_kernel(const double *reward, con
                                                        float gl) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) gae_env(i, n, T, g, gl, reward, term, trunc, values, adv);
+}
+
+// The CTA's shared copies of an observation normaliser's mean[D] and sd[D] = norm_sd(var[D], eps), computed by the
+// first D threads; read from device memory at every launch, so a replayed CUDA graph uses the current statistics.  The
+// caller's next __syncthreads (the parameters' staging) publishes them
+template <int D>
+__device__ __forceinline__ void norm_stage(const ObsNormArgs &q, double (&mean)[D], double (&sd)[D]) {
+    if (threadIdx.x < D) {
+        mean[threadIdx.x] = q.mean[threadIdx.x];
+        sd[threadIdx.x] = norm_sd(q.var[threadIdx.x], q.eps);
+    }
+}
+
+// rollout_mlp_noisy_kernel's shared-policy path with normalised inputs (rollout_mlp_noisy_norm_env); launch bounds as
+// the shared-policy noisy kernels
+template <int KIND, int ACT>
+__global__ void __launch_bounds__(kThreads, 2)
+    rollout_mlp_noisy_norm_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpNoisyArgs p,
+                                  const ObsNormArgs q) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    using Src = MlpNoisyActions<KIND, false, ACT>;
+    __shared__ double mean[Src::D], sd[Src::D];
+    norm_stage<Src::D>(q, mean, sd);
+    const float *w = mlp_stage(p.mlp.params, mlp_param_count<Src::K, Src::D>(p.mlp.h1, p.mlp.h2));
+    if (i < a.n) rollout_mlp_noisy_norm_env<KIND, ACT>(a, i, T, last_obs, w, p, mean, sd, q.clip);
+}
+
+// rollout_actor_critic_kernel with normalised inputs for both nets (rollout_actor_critic_norm_env)
+template <int KIND, int ACT>
+__global__ void __launch_bounds__(kThreads, 2)
+    rollout_actor_critic_norm_kernel(const StepArgs a, const int32_t T, float *last_obs, const ActorCriticArgs p,
+                                     const ObsNormArgs q) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    using Src = MlpNoisyActions<KIND, false, ACT>;
+    __shared__ double mean[Src::D], sd[Src::D];
+    norm_stage<Src::D>(q, mean, sd);
+    const int h1 = p.actor.mlp.h1, h2 = p.actor.mlp.h2;
+    const float *wc = mlp_stage_pair(p.actor.mlp.params, mlp_param_count<Src::K, Src::D>(h1, h2), p.critic,
+                                     mlp_param_count<1, Src::D>(h1, h2));
+    extern __shared__ float4 mlp_shared[];
+    if (i < a.n)
+        rollout_actor_critic_norm_env<KIND, ACT>(a, i, T, last_obs, reinterpret_cast<const float *>(mlp_shared), wc, p,
+                                                 mean, sd, q.clip);
+}
+
+// gae_kernel with the rewards scaled by the return statistics (gae_scaled_env): sd = norm_sd(ret_var[0], eps), read
+// at every launch
+__global__ void __launch_bounds__(kThreads) gae_scaled_kernel(const double *reward, const uint8_t *term,
+                                                              const uint8_t *trunc, const float *values, float *adv,
+                                                              int64_t n, int32_t T, float g, float gl,
+                                                              const double *ret_var, double eps, float clip) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) gae_scaled_env(i, n, T, g, gl, norm_sd(__ldg(ret_var), eps), clip, reward, term, trunc, values, adv);
 }
 
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
@@ -1537,6 +1591,20 @@ __global__ void rms_apply_kernel(const float *x, float *out, const double *rewar
     }
 }
 
+// The normalised rows x[n][D] of observation rows o[n][D] (norm_obs_elem), one thread per element: the input rows of
+// the Box2D kinds' policy and critic launches when the observations are normalised
+__global__ void __launch_bounds__(kThreads) norm_rows_kernel(const float *o, float *x, int64_t total, int D,
+                                                             const ObsNormArgs q) {
+    __shared__ double mean[kMaxNormDim], sd[kMaxNormDim];
+    if (threadIdx.x < D) {
+        mean[threadIdx.x] = q.mean[threadIdx.x];
+        sd[threadIdx.x] = norm_sd(q.var[threadIdx.x], q.eps);
+    }
+    __syncthreads();
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < total) x[k] = norm_obs_elem(o[k], mean[k % D], sd[k % D], q.clip);
+}
+
 // ---- cross-GPU step barrier for the fused all-gather ---------------------------------------
 // flags[r] (uint64, in every rank's gather allocation) = number of steps whose results rank r has fully written
 // into THIS rank's buffers.  One launch per step, after the step kernel on the same stream: lane p publishes
@@ -2111,6 +2179,7 @@ extern "C" void b200gym_destroy(b200gym_t *h) {
     if (h->snap_bad) cudaFreeHost(h->snap_bad);
     cudaFree(h->snap_scratch);
     if (h->from_batch) b200gym_destroy(h->from_batch);
+    cudaFree(h->norm_rows);
     if (h->sub.final64) cudaFreeHost(h->sub.final64);
     if (h->sub.ep_r) cudaFreeHost(h->sub.ep_r);
     if (h->sub.ep_l) cudaFreeHost(h->sub.ep_l);
@@ -2704,18 +2773,23 @@ static int launch_rollout_linear_kind(b200gym *h, const StepArgs &a, int32_t T, 
 // runs in one scratch slice, and the policy launch of step t + 1 (or one last launch, with args_at(T - 1)) folds step t
 // into the summary.  kernel / entry: names for the error messages.  hook(t, obs_in, s, after): launches of the
 // caller's own around step t, made before the policy launch (after false, obs_in the policy's input) and after the
-// step sequence (after true, s the step's outputs); non-zero fails the rollout
+// step sequence (after true, s the step's outputs); non-zero fails the rollout.  input(obs): the rows the policy and
+// the hook read in place of the observation rows obs of step t, made by launches of the caller's own before both;
+// nullptr fails the rollout
 struct NoStepHook {
     int operator()(int32_t, const float *, const StepArgs &, bool) const { return 0; }
 };
+struct RawStepInput {
+    const float *operator()(const float *obs) const { return obs; }
+};
 
-template <typename Args, typename ArgsAt, typename Hook = NoStepHook>
+template <typename Args, typename ArgsAt, typename Hook = NoStepHook, typename Input = RawStepInput>
 static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
                                        const float *first_obs, const ArgsAt &args_at,
                                        void (*policy)(const float *, void *, const Args, const double *,
                                                       const uint8_t *, const uint8_t *, int64_t, int32_t, int, int),
                                        size_t smem, bool summary, cudaStream_t st, const char *kernel,
-                                       const char *entry, const Hook &hook = Hook{}) {
+                                       const char *entry, const Hook &hook = Hook{}, const Input &input = Input{}) {
     const int64_t n = h->n, D = h->D, cols = std::max(h->A, 1);
     const size_t act_row = (size_t)n * cols * (h->A == 0 ? sizeof(long long) : sizeof(float));
     const int action_dtype = h->A == 0 ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
@@ -2736,7 +2810,11 @@ static int launch_rollout_policy_box2d(b200gym *h, const StepArgs &a, int32_t T,
     const unsigned blocks = (unsigned)blocks_for(n);
     int rc = 0;
     for (int32_t t = 0; t < T && !rc; t++) {
-        const float *obs_in = t == 0 ? first_obs : s.obs;
+        const float *obs_in = input(t == 0 ? first_obs : s.obs);
+        if (!obs_in) {
+            rc = 1;
+            break;
+        }
         if (!summary) {
             s.actions = static_cast<const unsigned char *>(a.actions) + (size_t)t * act_row;
             s.obs = a.obs + t * n * D;
@@ -3146,6 +3224,269 @@ extern "C" int b200gym_rollout_actor_critic(b200gym_t *h, const float *actor_dev
                                                              smem_critic, gamma, gamma_lambda, st);
     return launch_rollout_actor_critic<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, smem_actor,
                                                          smem_critic, gamma, gamma_lambda, st);
+}
+
+// ---- normalised observations and rewards (b200gym_rollout_mlp_noisy_norm, b200gym_rollout_actor_critic_norm) ----
+// The Box2D kinds' network inputs: norm_rows_kernel from the observation rows o into the handle's scratch rows, made
+// on first use (these kinds refuse CUDA-graph capture).  nullptr on failure, with the error set
+static const float *launch_norm_rows(b200gym *h, const float *o, const ObsNormArgs &q, cudaStream_t st,
+                                     const char *entry) {
+    const int64_t total = h->n * h->D;
+    if (!h->norm_rows && cudaMalloc((void **)&h->norm_rows, (size_t)total * sizeof(float)) != cudaSuccess) {
+        h->norm_rows = nullptr;
+        fail(h, "%s: cannot allocate the normalised input rows", entry);
+        return nullptr;
+    }
+    norm_rows_kernel<<<blocks_for(total), kThreads, 0, st>>>(o, h->norm_rows, total, (int)h->D, q);
+    if (cudaGetLastError() != cudaSuccess) {
+        fail(h, "norm_rows_kernel: launch failed");
+        return nullptr;
+    }
+    return h->norm_rows;
+}
+
+// The statistics checks both entry points share; `what` names the caller in the error
+static int norm_args_check(b200gym *h, const char *what, const double *mean, const double *var, double eps, float clip) {
+    if ((mean == nullptr) != (var == nullptr)) return fail(h, "%s: give both obs_mean_dev and obs_var_dev, or neither", what);
+    if (!(eps >= 0.0 && std::isfinite(eps))) return fail(h, "%s: eps must be finite and at least 0 (got %g)", what, eps);
+    if (!(clip > 0.0f)) return fail(h, "%s: clip_obs must be above 0, +inf for none (got %g)", what, (double)clip);
+    if (!mean && !std::isinf(clip)) return fail(h, "%s: clip_obs needs obs_mean_dev and obs_var_dev", what);
+    if (mean && h->D > kMaxNormDim) return fail(h, "%s: obs_dim %d is above %d", what, h->D, kMaxNormDim);
+    return 0;
+}
+
+template <int KIND, int ACT>
+static int launch_rollout_mlp_noisy_norm_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                              const MlpNoisyArgs &p, const ObsNormArgs &q, size_t smem,
+                                              cudaStream_t st) {
+    rollout_mlp_noisy_norm_kernel<KIND, ACT><<<blocks_for(h->n), kThreads, smem, st>>>(a, T, last_obs, p, q);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// launch_rollout_mlp_noisy_box2d's sequence with the policy reading the normalised rows of its input
+template <int K, int D, bool DISCRETE, int ACT>
+static int launch_rollout_mlp_noisy_norm_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                               const float *first_obs, const MlpNoisyArgs &p, const ObsNormArgs &q,
+                                               size_t smem, cudaStream_t st) {
+    const int64_t slice = h->n * K;
+    const char *entry = "b200gym_rollout_mlp_noisy_norm";
+    return launch_rollout_policy_box2d(
+        h, a, T, last_obs, first_obs,
+        [&](int32_t t) {
+            MlpNoisyArgs r = p;
+            r.noise = p.noise + t * slice;
+            r.outputs = p.outputs + t * slice;
+            return r;
+        },
+        mlp_noisy_policy_kernel<K, D, DISCRETE, false, ACT>, smem, false, st, "mlp_noisy_policy_kernel", entry,
+        NoStepHook{}, [&](const float *o) { return launch_norm_rows(h, o, q, st, entry); });
+}
+
+template <int ACT>
+static int launch_rollout_mlp_noisy_norm(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                         const float *first_obs, const MlpNoisyArgs &p, const ObsNormArgs &q,
+                                         size_t smem, cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_noisy_norm_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_noisy_norm_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_noisy_norm_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_noisy_norm_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_noisy_norm_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_noisy_norm_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, q, smem, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_noisy_norm_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, q, smem, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_noisy_norm_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, q, smem, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+extern "C" int b200gym_rollout_mlp_noisy_norm(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                              int h2, int32_t T, const float *noise_dev, float *outputs_dev,
+                                              void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                              uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                              float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                              int activation, const double *obs_mean_dev, const double *obs_var_dev,
+                                              double eps, float clip_obs) {
+    const char *what = "b200gym_rollout_mlp_noisy_norm";
+    if (!h) return fail(h, "%s: null handle", what);
+    if (int rc = norm_args_check(h, what, obs_mean_dev, obs_var_dev, eps, clip_obs)) return rc;
+    if (!obs_mean_dev)   // not normalised: b200gym_rollout_mlp_noisy_act's own checks and kernels
+        return b200gym_rollout_mlp_noisy_act(h, params_dev, per_env, n_layers, h1, h2, T, noise_dev, outputs_dev,
+                                             actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev,
+                                             final_obs_dev, last_obs_dev, first_obs_dev, stream, activation);
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "%s: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)", what, activation);
+    if (per_env) return fail(h, "%s: normalised inputs need one policy shared by every env (per_env = 0)", what);
+    if (n_layers != 1 && n_layers != 2) return fail(h, "%s: n_layers must be 1 or 2 (got %d)", what, n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "%s: hidden widths must be 1 .. %d (got %d, %d)", what, kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (!params_dev || !noise_dev || !outputs_dev || !actions_out_dev || !obs_dev || !reward_dev || !terminated_dev ||
+        !truncated_dev || !last_obs_dev)
+        return fail(h, "%s: null buffer", what);
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "%s: a Box2D env needs first_obs_dev", what);
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    const bool vec = h1 % 4 == 0;   // the shared copy starts 16-byte aligned
+    const MlpNoisyArgs p{{params_dev, 0, h1, h2, vec ? 1 : 0, nullptr, nullptr, nullptr}, noise_dev, outputs_dev};
+    const ObsNormArgs q{obs_mean_dev, obs_var_dev, eps, clip_obs};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_mlp_noisy_norm<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, q, smem, st);
+    return launch_rollout_mlp_noisy_norm<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, q, smem, st);
+}
+
+// launch_gae, or gae_scaled_kernel where the rewards are scaled (ret_var not null)
+static int launch_gae_norm(b200gym *h, const StepArgs &a, int32_t T, const ActorCriticArgs &p, float g, float gl,
+                           const double *ret_var, double eps, float clip_r, cudaStream_t st) {
+    if (!ret_var) return launch_gae(h, a, T, p, g, gl, st);
+    gae_scaled_kernel<<<blocks_for(h->n), kThreads, 0, st>>>(a.reward, a.terminated, a.truncated, p.values,
+                                                             p.advantages, h->n, T, g, gl, ret_var, eps, clip_r);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// The rollout launch: rollout_actor_critic_norm_kernel, or rollout_actor_critic_kernel where the observations are not
+// normalised (q.mean null: only the rewards are)
+template <int KIND, int ACT>
+static int launch_rollout_actor_critic_norm_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                                 const ActorCriticArgs &p, const ObsNormArgs &q, size_t smem,
+                                                 cudaStream_t st) {
+    if (q.mean) rollout_actor_critic_norm_kernel<KIND, ACT><<<blocks_for(h->n), kThreads, smem, st>>>(a, T, last_obs, p, q);
+    else rollout_actor_critic_kernel<KIND, ACT><<<blocks_for(h->n), kThreads, smem, st>>>(a, T, last_obs, p);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// launch_rollout_actor_critic_box2d's sequence with the critic and the policy reading the normalised rows of their
+// input (a norm_rows_kernel launch before them), and each critic launch on final or last observations after one too
+template <int K, int D, bool DISCRETE, int ACT>
+static int launch_rollout_actor_critic_norm_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                                  const float *first_obs, const ActorCriticArgs &p,
+                                                  const ObsNormArgs &q, size_t smem_actor, size_t smem_critic,
+                                                  cudaStream_t st) {
+    const int64_t n = h->n, slice = n * K;
+    const char *entry = "b200gym_rollout_actor_critic_norm";
+    const MlpPolicyArgs c{p.critic, 0, p.actor.mlp.h1, p.actor.mlp.h2, p.actor.mlp.vec, nullptr, nullptr, nullptr};
+    const unsigned blocks = blocks_for(n);
+    auto input = [&](const float *o) { return q.mean ? launch_norm_rows(h, o, q, st, entry) : o; };
+    auto critic = [&](const float *obs, float *out) {
+        if (!obs) return 1;
+        mlp_policy_kernel<1, D, false, false, ACT><<<blocks, kThreads, smem_critic, st>>>(obs, out, c, nullptr, nullptr,
+                                                                                        nullptr, n, -1, 1, 0);
+        return cudaGetLastError() != cudaSuccess ? fail(h, "mlp_policy_kernel (critic): launch failed") : 0;
+    };
+    int rc = launch_rollout_policy_box2d(
+        h, a, T, last_obs, first_obs,
+        [&](int32_t t) {
+            MlpNoisyArgs r = p.actor;
+            r.noise = p.actor.noise + t * slice;
+            r.outputs = p.actor.outputs + t * slice;
+            return r;
+        },
+        mlp_noisy_policy_kernel<K, D, DISCRETE, false, ACT>, smem_actor, false, st, "mlp_noisy_policy_kernel", entry,
+        [&](int32_t t, const float *obs_in, const StepArgs &s, bool after) {
+            return after ? critic(input(s.final_obs), p.advantages + t * n) : critic(obs_in, p.values + t * n);
+        },
+        input);
+    if (!rc) rc = critic(input(last_obs), p.values + (int64_t)T * n);
+    return rc;
+}
+
+template <int ACT>
+static int launch_rollout_actor_critic_norm(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                            const float *first_obs, const ActorCriticArgs &p, const ObsNormArgs &q,
+                                            size_t smem_actor, size_t smem_critic, cudaStream_t st) {
+    const size_t smem = smem_actor + smem_critic;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_actor_critic_norm_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_actor_critic_norm_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_actor_critic_norm_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_actor_critic_norm_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_actor_critic_norm_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, q, smem, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_actor_critic_norm_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, q, smem_actor,
+                                                                       smem_critic, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_actor_critic_norm_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, q, smem_actor,
+                                                                        smem_critic, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_actor_critic_norm_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, q,
+                                                                         smem_actor, smem_critic, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+extern "C" int b200gym_rollout_actor_critic_norm(b200gym_t *h, const float *actor_dev, const float *critic_dev,
+                                                 int n_layers, int h1, int h2, int32_t T, const float *noise_dev,
+                                                 float *outputs_dev, void *actions_out_dev, float *obs_dev,
+                                                 double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                                 float *final_obs_dev, float *values_dev, float *advantages_dev,
+                                                 float gamma, float gamma_lambda, float *last_obs_dev,
+                                                 const float *first_obs_dev, void *stream, int activation,
+                                                 const double *obs_mean_dev, const double *obs_var_dev, double eps,
+                                                 float clip_obs, const double *ret_var_dev, float clip_reward) {
+    const char *what = "b200gym_rollout_actor_critic_norm";
+    if (!h) return fail(h, "%s: null handle", what);
+    if (int rc = norm_args_check(h, what, obs_mean_dev, obs_var_dev, eps, clip_obs)) return rc;
+    if (!(clip_reward > 0.0f)) return fail(h, "%s: clip_reward must be above 0, +inf for none (got %g)", what,
+                                           (double)clip_reward);
+    if (!ret_var_dev && !std::isinf(clip_reward)) return fail(h, "%s: clip_reward needs ret_var_dev", what);
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "%s: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)", what, activation);
+    if (n_layers != 1 && n_layers != 2) return fail(h, "%s: n_layers must be 1 or 2 (got %d)", what, n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "%s: hidden widths must be 1 .. %d (got %d, %d)", what, kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (!(gamma >= 0.0f && gamma <= 1.0f && gamma_lambda >= 0.0f && gamma_lambda <= 1.0f))
+        return fail(h, "%s: gamma and gamma_lambda must be in [0, 1] (got %g, %g)", what, (double)gamma,
+                    (double)gamma_lambda);
+    if (!actor_dev || !critic_dev || !noise_dev || !outputs_dev || !actions_out_dev || !obs_dev || !reward_dev ||
+        !terminated_dev || !truncated_dev || !values_dev || !advantages_dev || !last_obs_dev)
+        return fail(h, "%s: null buffer", what);
+    if (!final_obs_dev || !h->cfg.autoreset)
+        return fail(h, "%s: the truncation bootstrap needs autoreset and final_obs_dev", what);
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "%s: a Box2D env needs first_obs_dev", what);
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t Pa = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    const int64_t Pc = h2 == 0 ? h1 * D + h1 + h1 + 1 : h1 * D + h1 + (int64_t)h2 * h1 + h2 + h2 + 1;
+    const bool vec = h1 % 4 == 0;   // as b200gym_rollout_actor_critic
+    const ActorCriticArgs p{{{actor_dev, 0, h1, h2, vec ? 1 : 0, nullptr, nullptr, nullptr}, noise_dev, outputs_dev},
+                            critic_dev, values_dev, advantages_dev};
+    const ObsNormArgs q{obs_mean_dev, obs_var_dev, eps, clip_obs};
+    const size_t smem_actor = (size_t)(Pa + 3) / 4 * 16, smem_critic = (size_t)(Pc + 3) / 4 * 16;
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rc =
+        activation == B200GYM_MLP_TANH
+            ? launch_rollout_actor_critic_norm<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, q, smem_actor,
+                                                                 smem_critic, st)
+            : launch_rollout_actor_critic_norm<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, q, smem_actor,
+                                                                 smem_critic, st);
+    return rc ? rc : launch_gae_norm(h, a, T, p, gamma, gamma_lambda, ret_var_dev, eps, clip_reward, st);
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------

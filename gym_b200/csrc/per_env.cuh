@@ -946,6 +946,156 @@ __host__ __device__ __forceinline__ void gae_env(int64_t i, int64_t n, int32_t T
     }
 }
 
+// ---- normalised observations and rewards (b200gym_rollout_mlp_noisy_norm, b200gym_rollout_actor_critic_norm) ------
+
+// The standard deviation of one column of a running variance, sqrt(var + eps) in float64 (normalize.py:94)
+__host__ __device__ __forceinline__ double norm_sd(double var, double eps) { return sqrt(var + eps); }
+
+// One normalised observation element: float32((float64(o) - mean) / sd), rms_apply_kernel's expression, then clamped to
+// [-clip, clip] with torch.clamp's bits: a NaN stays NaN, -0.0 stays -0.0, and clip = +inf clamps nothing
+__host__ __device__ __forceinline__ float norm_obs_elem(float o, double mean, double sd, float clip) {
+    const float x = (float)(((double)o - mean) / sd);
+    return x < -clip ? -clip : (x > clip ? clip : x);
+}
+
+// The network input x of observation o: norm_obs_elem per element, with mean[D] and sd[D] the CTA's shared copies
+template <int D>
+__host__ __device__ __forceinline__ void norm_obs(const float (&o)[D], const double *mean, const double *sd, float clip,
+                                                  float (&x)[D]) {
+#pragma unroll
+    for (int k = 0; k < D; k++) x[k] = norm_obs_elem(o[k], mean[k], sd[k], clip);
+}
+
+// The statistics a normalising launch reads, all fixed for the call: the observations' mean[D] and var[D] (float64,
+// caller-owned; staged with norm_sd once per CTA), eps, and the clip (+inf: none)
+struct ObsNormArgs {
+    const double *mean, *var;
+    double eps;
+    float clip;
+};
+
+// T steps of env i under the shared noisy policy at w with normalised inputs (rollout_mlp_noisy_norm_kernel):
+// rollout_mlp_noisy_env's loop, written out again so that no pre-existing kernel changes, with the policy reading x,
+// norm_obs of the observation o, in place of o.  o stays raw, so the sink stores the raw observations.  mean and sd are
+// the CTA's shared copies
+template <int KIND, int ACT = B200GYM_MLP_RELU>
+__device__ __forceinline__ void rollout_mlp_noisy_norm_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                           const float *w, const MlpNoisyArgs &p, const double *mean,
+                                                           const double *sd, float clip) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D], x[E::D];
+    E::observe(s, o);
+    norm_obs<E::D>(o, mean, sd, clip, x);
+    MlpNoisyActions<KIND, false, ACT> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, x, p.noise, p.outputs};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, false> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                 o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        norm_obs<E::D>(o, mean, sd, clip, x);
+        act += n;
+        src.next(n);
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
+// T steps of env i under the noisy actor at wa with the critic at wc, both reading normalised inputs
+// (rollout_actor_critic_norm_kernel): rollout_actor_critic_env's loop, written out again so that no pre-existing kernel
+// changes, with the actor and the critic reading x = norm_obs(o) in place of o, and the truncation bootstrap reading
+// norm_obs of the final observation.  o and the final observation stay raw for the sink
+template <int KIND, int ACT = B200GYM_MLP_RELU>
+__device__ __forceinline__ void rollout_actor_critic_norm_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                              const float *wa, const float *wc,
+                                                              const ActorCriticArgs &p, const double *mean,
+                                                              const double *sd, float clip) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    const int h1 = p.actor.mlp.h1, h2 = p.actor.mlp.h2;
+    const bool vec = p.actor.mlp.vec != 0;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D], x[E::D], fin[E::D];
+    E::observe(s, o);
+    norm_obs<E::D>(o, mean, sd, clip, x);
+    MlpNoisyActions<KIND, false, ACT> src{wa, h1, h2, vec, x, p.actor.noise, p.actor.outputs};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    uint8_t te = 0, tr = 0;
+    CriticSink<KIND> sink{{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                           o, ret, len, ended},
+                          fin, te, tr};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    float *values = p.values, *held = p.advantages;
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        float v[1];
+        mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, x, v);
+        store_once(values + i, v[0]);
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        if (tr && !te) {
+            norm_obs<E::D>(fin, mean, sd, clip, fin);
+            mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, fin, v);
+            store_once(held + i, v[0]);
+        }
+        norm_obs<E::D>(o, mean, sd, clip, x);
+        act += n;
+        values += n;
+        held += n;
+        src.next(n);
+        sink.next(n);
+    }
+    float v[1];
+    mlp_outputs<1, E::D, false, ACT>(wc, h1, h2, vec, x, v);
+    store_once(values + i, v[0]);
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
+// gae_env with scaled rewards (gae_scaled_kernel): r = float32(reward[t] / sd), then clamped to [-clip, clip] as
+// norm_obs_elem clamps (clip = +inf: none), in place of r = (float)reward[t]; sd = norm_sd of the return variance.
+// Written out again so that gae_env and gae_kernel keep their code
+__host__ __device__ __forceinline__ void gae_scaled_env(int64_t i, int64_t n, int32_t T, float g, float gl, double sd,
+                                                        float clip, const double *reward, const uint8_t *term,
+                                                        const uint8_t *trunc, const float *values, float *adv) {
+    float next = 0.0f;
+    for (int32_t t = T - 1; t >= 0; t--) {
+        const int64_t k = (int64_t)t * n + i;
+        const float q = (float)(reward[k] / sd), v = values[k];
+        const float r = q < -clip ? -clip : (q > clip ? clip : q);
+        const bool te = term[k] != 0, tr = trunc[k] != 0;
+        float delta;
+        if (te) delta = r - v;
+        else if (tr) delta = (r + g * adv[k]) - v;
+        else delta = (r + g * values[k + n]) - v;
+        next = (te || tr) ? delta : delta + gl * next;
+        adv[k] = next;
+    }
+}
+
 // ---- rollouts from snapshot rows (b200gym_rollout_from) ------------------------------------------------------------
 
 // The snapshot row of a classic kind (b200gym.cu, snapshot_save_kernel): the PCG64 record {state_hi, state_lo, inc_hi,

@@ -697,7 +697,8 @@ class B200VectorEnv:
                                               T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(),
                                               act)))
 
-    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu"):
+    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu", obs_norm=None, norm_epsilon=1e-8,
+                          clip_obs=None):
         """T steps of a stochastic MLP policy in closed loop, T = ``noise.shape[0]`` -> ``(actions, outputs, obs,
         rewards, terminateds, truncateds, infos)``: bit for bit what
         ``for t in range(T): z = mlp(obs); a = rule(z + noise[t]); obs, r, te, tr, info = self.step(a)`` returns,
@@ -736,22 +737,44 @@ class B200VectorEnv:
         Noise of -0.0 everywhere gives ``rollout_mlp()``'s actions (+0.0 would turn a -0.0 Box output into +0.0).
         Guards and the start from the current state are ``rollout_linear()``'s.  The classic-control kinds may be
         captured in a CUDA graph, and replays read the current contents of ``params`` and ``noise``, so filling the
-        noise and rolling out can be one graph; the Box2D kinds cannot (DESIGN.md §4.14)."""
-        captured = self._rollout_guards("rollout_mlp_noisy")
-        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, "rollout_mlp_noisy")
+        noise and rolling out can be one graph; the Box2D kinds cannot (DESIGN.md §4.14).
+
+        ``obs_norm=(mean, var)`` (keyword only; two float64 (D,) tensors, contiguous, on the env's device, such as
+        ``w.obs_rms.mean`` and ``w.obs_rms.var`` of a ``gym_b200.wrappers.NormalizeObservation`` ``w``) makes the policy
+        read normalised observations, per element, in float64 with ``eps = norm_epsilon`` (real, finite, >= 0)::
+
+            x = float32((float64(o) - mean) / sqrt(var + eps))
+            x = clamp(x, -c, c)        # only with clip_obs = c, a real number > 0 taken as float32; NaN stays NaN
+
+        which is ``((o.double() - mean) / torch.sqrt(var + eps)).float().clamp(-c, c)``: what NormalizeObservation
+        returns for these statistics without an update.  The returned ``obs`` and ``infos["final_observation"]`` stay
+        raw, so the caller can update its statistics from them.  The statistics are fixed for the call (the engine
+        never updates them) and need one shared policy: per-env ``params`` rows with ``obs_norm`` raise ``ValueError``,
+        as does ``clip_obs`` without ``obs_norm``.  A captured graph reads the current contents of ``mean`` and
+        ``var``; ``norm_epsilon`` and ``clip_obs`` are fixed at capture.  With the three keywords at their defaults the
+        call is the one above, unchanged (DESIGN.md §4.18)."""
+        what = "rollout_mlp_noisy"
+        captured = self._rollout_guards(what)
+        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, what)
         T = self._noise_steps(noise)
-        self._refuse_box2d_capture("rollout_mlp_noisy")
+        norm = self._norm_args(what, obs_norm, norm_epsilon, clip_obs, per_env=per_env)
+        self._refuse_box2d_capture(what)
         outputs = _torch().empty_like(noise)
         vp = ctypes.c_void_p
-        actions, obs, reward, term, trunc, infos = self._policy_rollout(
-            "rollout_mlp_noisy", T, False, captured, lambda T, outs, last, first: (
-                self._lib.b200gym_rollout_mlp_noisy_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden),
-                                                        h1, h2, T, vp(noise.data_ptr()), vp(outputs.data_ptr()),
-                                                        *outs[:6], vp(last.data_ptr()), vp(first.data_ptr()),
-                                                        self._stream(), act)))
+        if norm is None:
+            launch = lambda T, outs, last, first: self._lib.b200gym_rollout_mlp_noisy_act(  # noqa: E731
+                self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T, vp(noise.data_ptr()),
+                vp(outputs.data_ptr()), *outs[:6], vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act)
+        else:
+            launch = lambda T, outs, last, first: self._lib.b200gym_rollout_mlp_noisy_norm(  # noqa: E731
+                self._handle, vp(params.data_ptr()), 0, len(hidden), h1, h2, T, vp(noise.data_ptr()),
+                vp(outputs.data_ptr()), *outs[:6], vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act,
+                *norm[:4])
+        actions, obs, reward, term, trunc, infos = self._policy_rollout(what, T, False, captured, launch)
         return actions, outputs, obs, reward, term, trunc, infos
 
-    def rollout_actor_critic(self, actor, critic, hidden, noise, *, gamma, gae_lambda, activation="relu"):
+    def rollout_actor_critic(self, actor, critic, hidden, noise, *, gamma, gae_lambda, activation="relu", obs_norm=None,
+                             norm_epsilon=1e-8, clip_obs=None, reward_norm=None, clip_reward=None):
         """One on-policy collection step of PPO / A2C: ``rollout_mlp_noisy()`` with a critic evaluated next to each env's
         state, and the GAE advantages -> ``(actions, outputs, values, advantages, obs, rewards, terminateds,
         truncateds, infos)``.
@@ -805,7 +828,49 @@ class B200VectorEnv:
         rollout in one launch, both nets staged in shared memory, then one launch for the advantages; they may be
         captured in a CUDA graph, and replays read the current contents of ``actor``, ``critic`` and ``noise``, while
         ``gamma`` and ``gae_lambda`` are fixed at capture.  The Box2D kinds compose the same results launch by launch
-        and cannot be captured (DESIGN.md §4.17)."""
+        and cannot be captured (DESIGN.md §4.17).
+
+        ``obs_norm``, ``norm_epsilon`` and ``clip_obs`` are ``rollout_mlp_noisy()``'s: with ``obs_norm``, the actor, the
+        critic at every step, ``values[T]`` and the bootstrap ``Vf[t]`` all read the normalised observation.
+        ``reward_norm=var`` (a float64 (1,) tensor on the env's device, such as ``w.return_rms.var`` of a
+        ``gym_b200.wrappers.NormalizeReward``) scales the rewards the advantages read, NormalizeReward's division
+        without a mean::
+
+            r[t] = float32(rewards[t] / sqrt(var + eps))
+            r[t] = clamp(r[t], -c_r, c_r)      # only with clip_reward = c_r, as clip_obs
+
+        The returned ``rewards`` stay raw float64; ``values`` and ``advantages`` are in the scaled units.
+        ``clip_reward`` without ``reward_norm`` raises ``ValueError``.  Replays of a captured graph read the current
+        ``mean``, ``var`` and reward ``var``.  The engine never updates the statistics: a CleanRL-shaped continuous PPO
+        holds them fixed for one collection and updates them from it, in float64 (Chan's merge for the observations,
+        the discounted-return recurrence for the rewards)::
+
+            f64 = dict(dtype=torch.float64, device=dev)                          # RunningMeanStd's start
+            om, ov, oc = torch.zeros(D, **f64), torch.ones(D, **f64), 1e-4
+            rm, rv, rc = torch.zeros(1, **f64), torch.ones(1, **f64), 1e-4
+            ret = torch.zeros(N, **f64)
+            for update in range(num_updates):
+                eps_n = std * torch.randn(T, N, K, device=dev)
+                a, mean, values, adv, obs, r, te, tr, info = envs.rollout_actor_critic(
+                    pa, pc, (64, 64), eps_n, gamma=0.99, gae_lambda=0.95, activation="tanh",
+                    obs_norm=(om, ov), clip_obs=10.0, reward_norm=rv, clip_reward=10.0)
+                x = obs.double().reshape(-1, D)                                   # Chan et al. from T * N rows
+                bm, bv, bc = x.mean(0), x.var(0, unbiased=False), x.shape[0]
+                d, tot = bm - om, oc + bc
+                ov.copy_((ov * oc + bv * bc + d * d * oc * bc / tot) / tot); om.add_(d * bc / tot); oc = tot
+                rets = []
+                for t in range(T):                                                # NormalizeReward's recurrence
+                    ret = ret * 0.99 + r[t]
+                    rets.append(ret)
+                    ret = torch.where(te[t] | tr[t], torch.zeros_like(ret), ret)
+                y = torch.stack(rets).reshape(-1)
+                bm, bv, bc = y.mean(), y.var(unbiased=False), y.numel()
+                d, tot = bm - rm, rc + bc
+                rv.copy_((rv * rc + bv * bc + d * d * rc * bc / tot) / tot); rm.add_(d * bc / tot); rc = tot
+                # the PPO update reads obs normalised with the statistics of this collection: normalise before
+                # updating them, or keep a copy
+
+        With every new keyword at its default the call is the one above, unchanged (DESIGN.md §4.18)."""
         what = "rollout_actor_critic"
         captured = self._rollout_guards(what)
         if not self.autoreset:
@@ -818,19 +883,73 @@ class B200VectorEnv:
         self._critic_params(critic, hidden, what)
         g, gl = self._gae_coefficients(gamma, gae_lambda, what)
         T = self._noise_steps(noise, what)
+        norm = self._norm_args(what, obs_norm, norm_epsilon, clip_obs, reward_norm, clip_reward)
         self._refuse_box2d_capture(what)
         torch = _torch()
         outputs = torch.empty_like(noise)
         values = torch.empty((T + 1, self.num_envs), dtype=torch.float32, device=self.device)
         advantages = torch.empty((T, self.num_envs), dtype=torch.float32, device=self.device)
         vp = ctypes.c_void_p
+        entry = self._lib.b200gym_rollout_actor_critic if norm is None else self._lib.b200gym_rollout_actor_critic_norm
         actions, obs, reward, term, trunc, infos = self._policy_rollout(
-            what, T, False, captured, lambda T, outs, last, first: (
-                self._lib.b200gym_rollout_actor_critic(
-                    self._handle, vp(actor.data_ptr()), vp(critic.data_ptr()), len(hidden), h1, h2, T,
-                    vp(noise.data_ptr()), vp(outputs.data_ptr()), *outs[:6], vp(values.data_ptr()),
-                    vp(advantages.data_ptr()), g, gl, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act)))
+            what, T, False, captured, lambda T, outs, last, first: entry(
+                self._handle, vp(actor.data_ptr()), vp(critic.data_ptr()), len(hidden), h1, h2, T,
+                vp(noise.data_ptr()), vp(outputs.data_ptr()), *outs[:6], vp(values.data_ptr()),
+                vp(advantages.data_ptr()), g, gl, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act,
+                *(() if norm is None else norm)))
         return actions, outputs, values, advantages, obs, reward, term, trunc, infos
+
+    def _norm_args(self, what, obs_norm, eps, clip_obs, reward_norm=None, clip_reward=None, per_env=False):
+        """Check the normalisation keywords of rollout_mlp_noisy() / rollout_actor_critic() without a CUDA call ->
+        None when the observations and rewards are both left as they are, else the trailing arguments of the
+        ``_norm`` entry points: (mean, var, eps, clip_obs, reward var, clip_reward), pointers or None, clips as
+        float32 values with +inf for none."""
+        torch = _torch()
+        if isinstance(eps, (bool, np.bool_)) or not isinstance(eps, (int, float, np.integer, np.floating)) or not (
+                math.isfinite(float(eps)) and float(eps) >= 0.0):
+            raise ValueError(f"{what}() needs norm_epsilon a finite real number >= 0, got {eps!r}")
+
+        def clip(c, name, given):
+            if c is None:
+                return math.inf
+            if isinstance(c, (bool, np.bool_)) or not isinstance(c, (int, float, np.integer, np.floating)):
+                raise ValueError(f"{what}() needs {name} a finite real number > 0, got {c!r}")
+            with np.errstate(over="ignore"):
+                f = np.float32(float(c)) if math.isfinite(float(c)) else np.float32(np.nan)
+            if not (np.isfinite(f) and f > 0):
+                raise ValueError(f"{what}() needs {name} a finite real number > 0 (as float32), got {c!r}")
+            if not given:
+                raise ValueError(f"{what}() got {name} without the statistics it clips")
+            return float(f)
+
+        def stats(x, name, shape):
+            if not isinstance(x, torch.Tensor):
+                raise ValueError(f"{what}() needs {name} as a torch tensor, got {type(x).__name__}")
+            if x.dtype != torch.float64:
+                raise ValueError(f"{what}() needs float64 {name}, got {x.dtype}")
+            if x.device != self.device:
+                raise ValueError(f"{what}() needs {name} on {self.device}, got {x.device}")
+            if tuple(x.shape) != shape:
+                raise ValueError(f"{what}() needs {name} of shape {shape}, got {tuple(x.shape)}")
+            if not x.is_contiguous():
+                raise ValueError(f"{what}() needs a contiguous {name}")
+            return ctypes.c_void_p(x.data_ptr())
+
+        mean = var = rvar = None
+        if obs_norm is not None:
+            if not isinstance(obs_norm, (tuple, list)) or len(obs_norm) != 2:
+                raise ValueError(f"{what}() needs obs_norm as a (mean, var) pair, got {type(obs_norm).__name__}")
+            if per_env:
+                raise ValueError(f"{what}() with obs_norm needs one policy shared by every env, not per-env rows")
+            mean = stats(obs_norm[0], "obs_norm mean", (self.obs_dim,))
+            var = stats(obs_norm[1], "obs_norm var", (self.obs_dim,))
+        c_obs = clip(clip_obs, "clip_obs", obs_norm is not None)
+        if reward_norm is not None:
+            rvar = stats(reward_norm, "reward_norm", (1,))
+        c_rew = clip(clip_reward, "clip_reward", reward_norm is not None)
+        if obs_norm is None and reward_norm is None:
+            return None
+        return mean, var, float(eps), c_obs, rvar, c_rew
 
     def _critic_params(self, critic, hidden, what):
         """Check rollout_actor_critic()'s critic, D -> hidden -> 1, without a CUDA call."""

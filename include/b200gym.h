@@ -322,6 +322,40 @@ int b200gym_rollout_actor_critic(b200gym_t *h, const float *actor_dev, const flo
                                  float gamma_lambda, float *last_obs_dev, const float *first_obs_dev, void *stream,
                                  int activation);
 
+/*
+ * b200gym_rollout_mlp_noisy_act and b200gym_rollout_actor_critic with normalised network inputs: every observation a
+ * network reads (the actor's and the critic's inputs, the last observation and the final observation of a truncation)
+ * is, per element k, with sd[k] = sqrt(obs_var[k] + eps) in float64,
+ *   x[k] = (float)(((double)o[k] - obs_mean[k]) / sd[k]), then clamped to [-clip_obs, clip_obs] (a NaN stays NaN)
+ * NormalizeObservation's output for these statistics without an update.  The observations written out stay raw.
+ *   obs_mean_dev, obs_var_dev  float64 [D] each, read at every launch; both null: not normalised
+ *   eps                        finite, >= 0 (also the rewards' epsilon)
+ *   clip_obs                   > 0; +inf: no clip (the only value allowed without obs_mean_dev)
+ *   ret_var_dev                float64 [1], NormalizeReward's return variance; null: rewards not scaled.  Otherwise
+ *                              the advantages read r = (float)(reward[t] / sqrt(ret_var + eps)), clamped to
+ *                              [-clip_reward, clip_reward], in place of (float)reward[t]; the rewards written out stay
+ *                              raw
+ *   clip_reward                > 0; +inf: no clip (the only value allowed without ret_var_dev)
+ * Normalised inputs need one shared policy (per_env = 0).  b200gym_rollout_mlp_noisy_norm without obs_mean_dev is
+ * b200gym_rollout_mlp_noisy_act.  Classic-control kinds: the rollout in ONE launch (then the GAE launch); Box2D kinds:
+ * the launches of the calls without normalisation, each network launch after a launch that writes its normalised
+ * input rows into a scratch buffer the handle keeps.
+ */
+int b200gym_rollout_mlp_noisy_norm(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                                   int32_t T, const float *noise_dev, float *outputs_dev, void *actions_out_dev,
+                                   float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                   float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                   int activation, const double *obs_mean_dev, const double *obs_var_dev, double eps,
+                                   float clip_obs);
+int b200gym_rollout_actor_critic_norm(b200gym_t *h, const float *actor_dev, const float *critic_dev, int n_layers,
+                                      int h1, int h2, int32_t T, const float *noise_dev, float *outputs_dev,
+                                      void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                      uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                      float *values_dev, float *advantages_dev, float gamma, float gamma_lambda,
+                                      float *last_obs_dev, const float *first_obs_dev, void *stream, int activation,
+                                      const double *obs_mean_dev, const double *obs_var_dev, double eps,
+                                      float clip_obs, const double *ret_var_dev, float clip_reward);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
