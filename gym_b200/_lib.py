@@ -155,6 +155,10 @@ SIGNATURES = {
     "b200gym_rollout_actor_critic_norm": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32] + [_vp] * 10 +
                                           [ctypes.c_float, ctypes.c_float, _vp, _vp, _vp, _i32, _vp, _vp,
                                            ctypes.c_double, ctypes.c_float, _vp, ctypes.c_float]),
+    "b200gym_rollout_linear_norm": (_i32, [_vp, _vp, _vp, _i32, _i32] + [_vp] * 12 +
+                                    [_vp, _vp, ctypes.c_double, ctypes.c_float, _vp, _vp]),
+    "b200gym_rollout_mlp_norm": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32] + [_vp] * 12 +
+                                 [_i32, _vp, _vp, ctypes.c_double, ctypes.c_float, _vp, _vp]),
     "b200gym_invalid_actions": (_i32, [_vp, _vp, ctypes.POINTER(_i64)]),
     "b200gym_invalid_seen": (_i32, [_vp]),
     "b200gym_host_buffers": (_i32, [_vp, ctypes.POINTER(HostIO)]),

@@ -564,6 +564,59 @@ __global__ void __launch_bounds__(kThreads) gae_scaled_kernel(const double *rewa
     if (i < n) gae_scaled_env(i, n, T, g, gl, norm_sd(__ldg(ret_var), eps), clip, reward, term, trunc, values, adv);
 }
 
+// rollout_linear_kernel with normalised inputs and, in summary mode, the observation moments (rollout_linear_norm_env).
+// q.mean null: raw inputs; m.sum null: no moments.  Both branches are the same for every thread of the launch
+template <int KIND, bool SUMMARY>
+__global__ void __launch_bounds__(kThreads)
+    rollout_linear_norm_kernel(const StepArgs a, const int32_t T, float *last_obs, const LinearPolicyArgs p,
+                               const ObsNormArgs q, const ObsMomentArgs m) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    constexpr int D = bgym::Env<KIND>::D;
+    __shared__ double mean[D], sd[D];
+    if (q.mean) norm_stage<D>(q, mean, sd);
+    __syncthreads();
+    if (i < a.n) rollout_linear_norm_env<KIND, SUMMARY>(a, i, T, last_obs, p, q.mean ? mean : nullptr, sd, q.clip, m);
+}
+
+// rollout_mlp_kernel with normalised inputs and the observation moments (rollout_mlp_norm_env); q and m as
+// rollout_linear_norm_kernel's, PER_ENV, ACT and the launch bounds as rollout_mlp_kernel's
+template <int KIND, bool SUMMARY, bool PER_ENV, int ACT>
+__global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2)
+    rollout_mlp_norm_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpPolicyArgs p,
+                            const ObsNormArgs q, const ObsMomentArgs m) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    using Src = MlpActions<KIND, SUMMARY, PER_ENV, ACT>;
+    __shared__ double mean[Src::D], sd[Src::D];
+    if (q.mean) norm_stage<Src::D>(q, mean, sd);
+    const double *mu = q.mean ? mean : nullptr;
+    if constexpr (PER_ENV) {
+        __syncthreads();
+        if (i < a.n)
+            rollout_mlp_norm_env<KIND, SUMMARY, true, ACT>(a, i, T, last_obs, p.params + i * p.stride, p, mu, sd, q.clip,
+                                                           m);
+    } else {
+        const float *w = mlp_stage(p.params, mlp_param_count<Src::K, Src::D>(p.h1, p.h2));
+        if (i < a.n) rollout_mlp_norm_env<KIND, SUMMARY, false, ACT>(a, i, T, last_obs, w, p, mu, sd, q.clip, m);
+    }
+}
+
+// The observation moments of a Box2D summary-mode rollout, one step: env i adds its raw input row o[i] of step t
+// (moments_fold's arithmetic) where step t is its first episode's end or before it.  Launched before step t's policy
+// launch, which folds step t - 1 into the summary, so that is: t = 0 (onto +0.0), or neither the summary's `ended`
+// (folded up to step t - 2) nor step t - 1's flags set
+__global__ void __launch_bounds__(kThreads) obs_moments_kernel(const float *o, const uint8_t *ended,
+                                                               const uint8_t *term, const uint8_t *trunc, int64_t n,
+                                                               int D, int32_t t, const ObsMomentArgs m) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || (t > 0 && (ended[i] | term[i] | trunc[i]))) return;
+    for (int k = 0; k < D; k++) {
+        const int64_t e = i * D + k;
+        const double v = (double)o[e];
+        m.sum[e] = (t == 0 ? 0.0 : m.sum[e]) + v;
+        m.sumsq[e] = (t == 0 ? 0.0 : m.sumsq[e]) + v * v;
+    }
+}
+
 // --- asynchronous-copy helpers (sm_90a PTX) --------------------------------------------------------
 namespace acp {
 
@@ -3487,6 +3540,221 @@ extern "C" int b200gym_rollout_actor_critic_norm(b200gym_t *h, const float *acto
             : launch_rollout_actor_critic_norm<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, q, smem_actor,
                                                                  smem_critic, st);
     return rc ? rc : launch_gae_norm(h, a, T, p, gamma, gamma_lambda, ret_var_dev, eps, clip_reward, st);
+}
+
+// ---- normalised inputs and observation moments in the closed-loop rollouts (b200gym_rollout_linear_norm,
+// b200gym_rollout_mlp_norm) ----
+// The checks both entry points add to their calls without normalisation: the statistics (norm_args_check) and the
+// moment buffers, both or neither and only in summary mode
+static int norm_moments_check(b200gym *h, const char *what, const double *mean, const double *var, double eps,
+                              float clip, const double *sum, const double *sumsq, bool summary) {
+    if (int rc = norm_args_check(h, what, mean, var, eps, clip)) return rc;
+    if ((sum == nullptr) != (sumsq == nullptr))
+        return fail(h, "%s: give both obs_sum_dev and obs_sumsq_dev, or neither", what);
+    if (sum && !summary)
+        return fail(h, "%s: the observation moments need the summary mode (returns_dev, lengths_dev, ended_dev)", what);
+    return 0;
+}
+
+// launch_rollout_policy_box2d's sequence with the policy reading the normalised rows of its input (q.mean not null:
+// a norm_rows_kernel launch before it) and, in summary mode with m.sum not null, obs_moments_kernel folding the raw
+// input rows of step t before that step's launches, whose step sequence overwrites them (the one scratch slice)
+template <typename Args>
+static int launch_rollout_policy_norm_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                            const float *first_obs, const Args &p,
+                                            void (*policy)(const float *, void *, const Args, const double *,
+                                                           const uint8_t *, const uint8_t *, int64_t, int32_t, int,
+                                                           int),
+                                            size_t smem, const ObsNormArgs &q, const ObsMomentArgs &m, bool summary,
+                                            cudaStream_t st, const char *kernel, const char *entry) {
+    const unsigned blocks = blocks_for(h->n);
+    return launch_rollout_policy_box2d(
+        h, a, T, last_obs, first_obs, [&](int32_t) { return p; }, policy, smem, summary, st, kernel, entry,
+        [&](int32_t t, const float *, const StepArgs &s, bool after) {
+            if (after || !m.sum) return 0;
+            obs_moments_kernel<<<blocks, kThreads, 0, st>>>(t == 0 ? first_obs : s.obs, p.ended, s.terminated,
+                                                            s.truncated, h->n, (int)h->D, t, m);
+            return cudaGetLastError() != cudaSuccess ? fail(h, "obs_moments_kernel: launch failed") : 0;
+        },
+        [&](const float *o) { return q.mean ? launch_norm_rows(h, o, q, st, entry) : o; });
+}
+
+template <int KIND>
+static int launch_rollout_linear_norm_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                           const LinearPolicyArgs &p, const ObsNormArgs &q, const ObsMomentArgs &m,
+                                           bool summary, cudaStream_t st) {
+    const unsigned blocks = blocks_for(h->n);
+    if (summary) rollout_linear_norm_kernel<KIND, true><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p, q, m);
+    else rollout_linear_norm_kernel<KIND, false><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p, q, m);
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_rollout_linear_norm(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env,
+                                           int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                           uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                           double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev,
+                                           float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                           const double *obs_mean_dev, const double *obs_var_dev, double eps,
+                                           float clip_obs, double *obs_sum_dev, double *obs_sumsq_dev) {
+    const char *what = "b200gym_rollout_linear_norm";
+    if (!h) return fail(h, "%s: null handle", what);
+    const bool summary = returns_dev != nullptr;
+    if (int rc = norm_moments_check(h, what, obs_mean_dev, obs_var_dev, eps, clip_obs, obs_sum_dev, obs_sumsq_dev,
+                                    summary))
+        return rc;
+    if (!obs_mean_dev && !obs_sum_dev)   // neither: b200gym_rollout_linear's own checks and kernels
+        return b200gym_rollout_linear(h, weight_dev, bias_dev, per_env, T, actions_out_dev, obs_dev, reward_dev,
+                                      terminated_dev, truncated_dev, final_obs_dev, returns_dev, lengths_dev, ended_dev,
+                                      last_obs_dev, first_obs_dev, stream);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (!weight_dev || !bias_dev || !last_obs_dev) return fail(h, "%s: null buffer", what);
+    if (summary ? (!lengths_dev || !ended_dev || actions_out_dev || obs_dev || reward_dev || terminated_dev ||
+                   truncated_dev || final_obs_dev)
+                : (!actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || lengths_dev ||
+                   ended_dev))
+        return fail(h, "%s: give either the per-step outputs or returns, lengths and ended", what);
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "%s: a Box2D env needs first_obs_dev", what);
+    const int64_t K = h->A == 0 ? h->NACT : h->A;
+    const LinearPolicyArgs p{weight_dev, bias_dev, per_env ? K * h->D : 0, per_env ? K : 0, returns_dev, lengths_dev,
+                             ended_dev};
+    const ObsNormArgs q{obs_mean_dev, obs_var_dev, eps, clip_obs};
+    const ObsMomentArgs m{obs_sum_dev, obs_sumsq_dev};
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    float *last = last_obs_dev;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_linear_norm_kind<B200GYM_CARTPOLE>(h, a, T, last, p, q, m, summary, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_linear_norm_kind<B200GYM_MOUNTAINCAR>(h, a, T, last, p, q, m, summary, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_linear_norm_kind<B200GYM_MOUNTAINCAR_CONT>(h, a, T, last, p, q, m, summary, st);
+    case B200GYM_PENDULUM: return launch_rollout_linear_norm_kind<B200GYM_PENDULUM>(h, a, T, last, p, q, m, summary, st);
+    case B200GYM_ACROBOT: return launch_rollout_linear_norm_kind<B200GYM_ACROBOT>(h, a, T, last, p, q, m, summary, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_policy_norm_box2d(h, a, T, last, first_obs_dev, p, linear_policy_kernel<4, 8, true>, 0, q,
+                                                m, summary, st, "linear_policy_kernel", what);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_policy_norm_box2d(h, a, T, last, first_obs_dev, p, linear_policy_kernel<2, 8, false>, 0,
+                                                q, m, summary, st, "linear_policy_kernel", what);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_policy_norm_box2d(h, a, T, last, first_obs_dev, p, linear_policy_kernel<4, 24, false>, 0,
+                                                q, m, summary, st, "linear_policy_kernel", what);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+template <int KIND, int ACT>
+static int launch_rollout_mlp_norm_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                        const MlpPolicyArgs &p, const ObsNormArgs &q, const ObsMomentArgs &m,
+                                        bool per_env, size_t smem, bool summary, cudaStream_t st) {
+    const unsigned blocks = blocks_for(h->n);
+    if (per_env) {
+        if (summary) rollout_mlp_norm_kernel<KIND, true, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p, q, m);
+        else rollout_mlp_norm_kernel<KIND, false, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p, q, m);
+    } else {
+        if (summary)
+            rollout_mlp_norm_kernel<KIND, true, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p, q, m);
+        else rollout_mlp_norm_kernel<KIND, false, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p, q, m);
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+template <int K, int D, bool DISCRETE, int ACT>
+static int launch_rollout_mlp_norm_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                         const float *first_obs, const MlpPolicyArgs &p, const ObsNormArgs &q,
+                                         const ObsMomentArgs &m, bool per_env, size_t smem, bool summary,
+                                         cudaStream_t st) {
+    return launch_rollout_policy_norm_box2d(h, a, T, last_obs, first_obs, p,
+                                            per_env ? mlp_policy_kernel<K, D, DISCRETE, true, ACT>
+                                                    : mlp_policy_kernel<K, D, DISCRETE, false, ACT>,
+                                            per_env ? 0 : smem, q, m, summary, st, "mlp_policy_kernel",
+                                            "b200gym_rollout_mlp_norm");
+}
+
+template <int ACT>
+static int launch_rollout_mlp_norm(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
+                                   const MlpPolicyArgs &p, const ObsNormArgs &q, const ObsMomentArgs &m, bool pe,
+                                   size_t smem, bool summary, cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE:
+        return launch_rollout_mlp_norm_kind<B200GYM_CARTPOLE, ACT>(h, a, T, last_obs, p, q, m, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR:
+        return launch_rollout_mlp_norm_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, last_obs, p, q, m, pe, smem, summary, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_norm_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, last_obs, p, q, m, pe, smem, summary,
+                                                                          st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_norm_kind<B200GYM_PENDULUM, ACT>(h, a, T, last_obs, p, q, m, pe, smem, summary, st);
+    case B200GYM_ACROBOT:
+        return launch_rollout_mlp_norm_kind<B200GYM_ACROBOT, ACT>(h, a, T, last_obs, p, q, m, pe, smem, summary, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_mlp_norm_box2d<4, 8, true, ACT>(h, a, T, last_obs, first_obs, p, q, m, pe, smem, summary,
+                                                              st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_norm_box2d<2, 8, false, ACT>(h, a, T, last_obs, first_obs, p, q, m, pe, smem, summary,
+                                                               st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_norm_box2d<4, 24, false, ACT>(h, a, T, last_obs, first_obs, p, q, m, pe, smem, summary,
+                                                                st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+extern "C" int b200gym_rollout_mlp_norm(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                        int h2, int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                        uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                        double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev,
+                                        float *last_obs_dev, const float *first_obs_dev, void *stream, int activation,
+                                        const double *obs_mean_dev, const double *obs_var_dev, double eps,
+                                        float clip_obs, double *obs_sum_dev, double *obs_sumsq_dev) {
+    const char *what = "b200gym_rollout_mlp_norm";
+    if (!h) return fail(h, "%s: null handle", what);
+    const bool summary = returns_dev != nullptr;
+    if (int rc = norm_moments_check(h, what, obs_mean_dev, obs_var_dev, eps, clip_obs, obs_sum_dev, obs_sumsq_dev,
+                                    summary))
+        return rc;
+    if (!obs_mean_dev && !obs_sum_dev)   // neither: b200gym_rollout_mlp_act's own checks and kernels
+        return b200gym_rollout_mlp_act(h, params_dev, per_env, n_layers, h1, h2, T, actions_out_dev, obs_dev,
+                                       reward_dev, terminated_dev, truncated_dev, final_obs_dev, returns_dev,
+                                       lengths_dev, ended_dev, last_obs_dev, first_obs_dev, stream, activation);
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "%s: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)", what, activation);
+    if (n_layers != 1 && n_layers != 2) return fail(h, "%s: n_layers must be 1 or 2 (got %d)", what, n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "%s: hidden widths must be 1 .. %d (got %d, %d)", what, kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (!params_dev || !last_obs_dev) return fail(h, "%s: null buffer", what);
+    if (summary ? (!lengths_dev || !ended_dev || actions_out_dev || obs_dev || reward_dev || terminated_dev ||
+                   truncated_dev || final_obs_dev)
+                : (!actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || lengths_dev ||
+                   ended_dev))
+        return fail(h, "%s: give either the per-step outputs or returns, lengths and ended", what);
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !first_obs_dev) return fail(h, "%s: a Box2D env needs first_obs_dev", what);
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    // as b200gym_rollout_mlp_act
+    const bool vec = h1 % 4 == 0 && (!per_env || (P % 4 == 0 && reinterpret_cast<uintptr_t>(params_dev) % 16 == 0));
+    const MlpPolicyArgs p{params_dev, per_env ? P : 0, h1, h2, vec ? 1 : 0, returns_dev, lengths_dev, ended_dev};
+    const ObsNormArgs q{obs_mean_dev, obs_var_dev, eps, clip_obs};
+    const ObsMomentArgs m{obs_sum_dev, obs_sumsq_dev};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool pe = per_env != 0;
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_mlp_norm<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, q, m, pe, smem,
+                                                         summary, st);
+    return launch_rollout_mlp_norm<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, q, m, pe, smem, summary,
+                                                     st);
 }
 
 // ---- per-env wrapper chains (csrc/subenv.cuh) --------------------------------

@@ -1096,6 +1096,158 @@ __host__ __device__ __forceinline__ void gae_scaled_env(int64_t i, int64_t n, in
     }
 }
 
+// ---- normalised inputs and observation moments in the closed-loop rollouts (b200gym_rollout_linear_norm,
+// b200gym_rollout_mlp_norm) ----------------------------------------------------------------------------------------
+
+// The observation moments of a summary-mode rollout: env i's rows sum[i][D] and sumsq[i][D], float64; both null: none
+struct ObsMomentArgs {
+    double *sum, *sumsq;
+};
+
+// The policy's input x of observation o: norm_obs with the CTA's shared statistics, or o itself where the rollout is
+// not normalised (mean null, the same for every thread of the launch)
+template <int D>
+__host__ __device__ __forceinline__ void norm_obs_or_raw(const float (&o)[D], const double *mean, const double *sd,
+                                                         float clip, float (&x)[D]) {
+    if (mean) {
+        norm_obs<D>(o, mean, sd, clip, x);
+    } else {
+#pragma unroll
+        for (int k = 0; k < D; k++) x[k] = o[k];
+    }
+}
+
+// One step of the observation moments: s[k] = s[k] + float64(o[k]) and q[k] = q[k] + float64(o[k]) * float64(o[k]),
+// every operation rounded (no fused multiply-add: -fmad=false on the device, -ffp-contract=off in the host build)
+template <int D>
+__host__ __device__ __forceinline__ void moments_fold(const float (&o)[D], double (&s)[D], double (&q)[D]) {
+#pragma unroll
+    for (int k = 0; k < D; k++) {
+        const double v = (double)o[k];
+        s[k] = s[k] + v;
+        q[k] = q[k] + v * v;
+    }
+}
+
+// T steps of env i under its linear policy with normalised inputs (rollout_linear_norm_kernel): rollout_linear_env's
+// loop, written out again so that no pre-existing kernel changes, with the policy reading x = norm_obs_or_raw(o) in
+// place of o, computed at the top of each step so that only o is live across the step.  o stays raw, so the sink
+// stores the raw observations.  SUMMARY with m.sum not null: the moments of the raw inputs of steps 0 .. len - 1 (the
+// first episode's), folded in step order from +0.0 before each step's action while the episode has not ended, then
+// stored to env i's rows
+template <int KIND, bool SUMMARY>
+__device__ __forceinline__ void rollout_linear_norm_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                        const LinearPolicyArgs &p, const double *mean, const double *sd,
+                                                        float clip, const ObsMomentArgs &m) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    using Src = LinearActions<KIND, SUMMARY>;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D], x[E::D];
+    E::observe(s, o);
+    Src src{{}, {}, x};
+    const float *w = p.weight + i * p.w_stride, *b = p.bias + i * p.b_stride;
+#pragma unroll
+    for (int k = 0; k < Src::K * E::D; k++) src.w[k] = __ldg(w + k);
+#pragma unroll
+    for (int j = 0; j < Src::K; j++) src.b[j] = __ldg(b + j);
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    const bool moments = SUMMARY && m.sum != nullptr;
+    double ms[E::D], mq[E::D];
+#pragma unroll
+    for (int k = 0; k < E::D; k++) ms[k] = mq[k] = 0.0;
+    LinearSink<KIND, SUMMARY> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                   o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        if (moments && !ended) moments_fold<E::D>(o, ms, mq);
+        norm_obs_or_raw<E::D>(o, mean, sd, clip, x);
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+    if constexpr (SUMMARY) {
+        p.returns[i] = ret;
+        p.lengths[i] = len;
+        p.ended[i] = ended ? 1 : 0;
+        if (moments) {
+#pragma unroll
+            for (int k = 0; k < E::D; k++) {
+                m.sum[i * E::D + k] = ms[k];
+                m.sumsq[i * E::D + k] = mq[k];
+            }
+        }
+    }
+}
+
+// T steps of env i under its MLP policy at w with normalised inputs (rollout_mlp_norm_kernel): rollout_mlp_env's loop,
+// written out again so that no pre-existing kernel changes, with MlpActions reading x = norm_obs_or_raw(o) in place of
+// o; the moments as rollout_linear_norm_env's.  GLOBAL and ACT as rollout_mlp_env
+template <int KIND, bool SUMMARY, bool GLOBAL, int ACT>
+__device__ __forceinline__ void rollout_mlp_norm_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                     const float *w, const MlpPolicyArgs &p, const double *mean,
+                                                     const double *sd, float clip, const ObsMomentArgs &m) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D], x[E::D];
+    E::observe(s, o);
+    const MlpActions<KIND, SUMMARY, GLOBAL, ACT> src{w, p.h1, p.h2, p.vec != 0, x};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    const bool moments = SUMMARY && m.sum != nullptr;
+    double ms[E::D], mq[E::D];
+#pragma unroll
+    for (int k = 0; k < E::D; k++) ms[k] = mq[k] = 0.0;
+    LinearSink<KIND, SUMMARY> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                   o, ret, len, ended};
+    const ActT *act = reinterpret_cast<const ActT *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        if (moments && !ended) moments_fold<E::D>(o, ms, mq);
+        norm_obs_or_raw<E::D>(o, mean, sd, clip, x);
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+    if constexpr (SUMMARY) {
+        p.returns[i] = ret;
+        p.lengths[i] = len;
+        p.ended[i] = ended ? 1 : 0;
+        if (moments) {
+#pragma unroll
+            for (int k = 0; k < E::D; k++) {
+                m.sum[i * E::D + k] = ms[k];
+                m.sumsq[i * E::D + k] = mq[k];
+            }
+        }
+    }
+}
+
 // ---- rollouts from snapshot rows (b200gym_rollout_from) ------------------------------------------------------------
 
 // The snapshot row of a classic kind (b200gym.cu, snapshot_save_kernel): the PCG64 record {state_hi, state_lo, inc_hi,

@@ -641,7 +641,8 @@ class B200VectorEnv:
         self._sample_end(bit_generator, state, actions.numel(), captured)
         return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
 
-    def rollout_linear(self, weight, bias, T, *, summary=False):
+    def rollout_linear(self, weight, bias, T, *, summary=False, obs_norm=None, norm_epsilon=1e-8, clip_obs=None,
+                       obs_moments=False):
         """T steps of a linear policy in closed loop: bit for bit what
         ``for t in range(T): a = policy(obs); obs, r, te, tr, info = self.step(a)`` returns, stacked, with ``obs``
         starting at the observation the env last returned, and the env left where that loop leaves it.
@@ -660,15 +661,63 @@ class B200VectorEnv:
         The classic-control kinds run the T steps in one launch, the policy next to each env's state, and start from
         the observation of the current state (after ``set_state()``, that is the first input).  They may be captured in
         a CUDA graph: replays read the current contents of ``weight`` and ``bias``.  The Box2D kinds launch the policy
-        and the step once per step and cannot be captured (DESIGN.md §4.12)."""
-        captured = self._rollout_guards("rollout_linear")
-        per_env = self._linear_params(weight, bias)
-        vp = ctypes.c_void_p
-        return self._policy_rollout("rollout_linear", T, summary, captured, lambda T, outs, last, first: (
-            self._lib.b200gym_rollout_linear(self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env), T,
-                                             *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+        and the step once per step and cannot be captured (DESIGN.md §4.12).
 
-    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu"):
+        ``obs_norm=(mean, var)``, ``norm_epsilon`` and ``clip_obs`` (keyword only) are ``rollout_mlp_noisy()``'s: the
+        policy reads ``((o.double() - mean) / torch.sqrt(var + eps)).float().clamp(-c, c)`` in place of ``o``, while
+        the returned ``obs`` and ``infos["final_observation"]`` stay raw.  The statistics are one shared (D,) pair,
+        fixed for the call, and per-env ``weight`` / ``bias`` rows are allowed with them: ES and ARS perturb the policy
+        and share the statistics.  ``obs_moments=True`` needs ``summary=True`` (full mode returns the observations
+        themselves; there it raises ``ValueError``) and returns ``(returns, lengths, ended, obs_sum, obs_sumsq)``, the
+        last two float64 (N, D): with ``o_t`` the raw float32 observation the policy read at step t (step 0's is the
+        one the env last returned), over env i's first-episode inputs t = 0 .. ``lengths[i] - 1`` in step order,
+        every operation rounded, no fused multiply-add::
+
+            s = +0.0;  s = s + float64(o_t[k])
+            q = +0.0;  q = q + float64(o_t[k]) * float64(o_t[k])
+
+        so the count is ``lengths``.  It works with or without ``obs_norm``.  An ARS-V2 loop (Mania et al. 2018) with
+        float64 running statistics, starting from the identity (V2-t keeps the b best directions' updates)::
+
+            f64 = dict(dtype=torch.float64, device=dev)
+            mean, var, count = torch.zeros(D, **f64), torch.ones(D, **f64), 0
+            M = torch.zeros(K, D, device=dev)                                  # the policy, zero bias
+            for it in range(iters):
+                delta = torch.randn(N // 2, K, D, device=dev)
+                W = torch.cat([M + nu * delta, M - nu * delta])                   # (N, K, D): +-directions
+                ret, length, ended, s, q = envs.rollout_linear(
+                    W, torch.zeros(N, K, device=dev), 1000, summary=True,
+                    obs_norm=(mean, var), obs_moments=True)
+                r = ret.float().reshape(2, -1)
+                M += alpha / (N // 2 * r.std()) * ((r[0] - r[1])[:, None, None] * delta).sum(0)
+                c = length.sum().item()                                           # Chan's merge of (c, S, Q)
+                if c:
+                    bm = s.sum(0) / c
+                    bv = q.sum(0) / c - bm * bm
+                    d, tot = bm - mean, count + c
+                    var.copy_((var * count + bv * c + d * d * count * c / tot) / tot)
+                    mean.add_(d * c / tot)
+                    count = tot
+
+        Replays of a captured graph read the current ``mean`` and ``var``; ``norm_epsilon`` and ``clip_obs`` are fixed
+        at capture.  With the four keywords at their defaults the call is the one above, unchanged (DESIGN.md
+        §4.19)."""
+        what = "rollout_linear"
+        captured = self._rollout_guards(what)
+        per_env = self._linear_params(weight, bias)
+        norm, moments = self._policy_norm_args(what, summary, obs_norm, norm_epsilon, clip_obs, obs_moments)
+        vp = ctypes.c_void_p
+        if norm is None:
+            return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first: (
+                self._lib.b200gym_rollout_linear(self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()), int(per_env),
+                                                 T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream())))
+        return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first, s=None, q=None: (
+            self._lib.b200gym_rollout_linear_norm(self._handle, vp(weight.data_ptr()), vp(bias.data_ptr()),
+                                                  int(per_env), T, *outs, vp(last.data_ptr()), vp(first.data_ptr()),
+                                                  self._stream(), *norm, s, q)), moments)
+
+    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu", obs_norm=None, norm_epsilon=1e-8,
+                    clip_obs=None, obs_moments=False):
         """T steps of an MLP policy in closed loop: ``rollout_linear()`` with the policy
         D -> hidden[0] (-> hidden[1]) -> K, the activation after every hidden layer and nothing after the last.
 
@@ -688,14 +737,32 @@ class B200VectorEnv:
           build they run with.  Another torch or CUDA build is not covered by that check (DESIGN.md §4.15).
 
         The action is taken from the K outputs as ``rollout_linear()`` takes it from its logits.  Returns, guards,
-        capture and the start from the current state are ``rollout_linear()``'s (DESIGN.md §4.13)."""
-        captured = self._rollout_guards("rollout_mlp")
+        capture and the start from the current state are ``rollout_linear()``'s (DESIGN.md §4.13).
+
+        ``obs_norm``, ``norm_epsilon``, ``clip_obs`` and ``obs_moments`` are ``rollout_linear()``'s, per-env ``params``
+        rows included.  The deterministic evaluation of a CleanRL-style tanh actor trained on normalised observations
+        (``rollout_actor_critic(..., obs_norm=(om, ov), clip_obs=10.0)``) reads the inputs it was trained on::
+
+            ret, length, ended = envs.rollout_mlp(pa, (64, 64), 1000, summary=True, activation="tanh",
+                                                  obs_norm=(om, ov), clip_obs=10.0)
+            score = ret[ended].mean()                  # the mean first-episode return of the episodes that ended
+
+        For Box kinds the action is the actor's mean output, unclipped, as ``rollout_linear()`` takes it (DESIGN.md
+        §4.19)."""
+        what = "rollout_mlp"
+        captured = self._rollout_guards(what)
         h1, h2, per_env, act = self._mlp_params(params, hidden, activation)
+        norm, moments = self._policy_norm_args(what, summary, obs_norm, norm_epsilon, clip_obs, obs_moments)
         vp = ctypes.c_void_p
-        return self._policy_rollout("rollout_mlp", T, summary, captured, lambda T, outs, last, first: (
-            self._lib.b200gym_rollout_mlp_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2,
-                                              T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(),
-                                              act)))
+        if norm is None:
+            return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first: (
+                self._lib.b200gym_rollout_mlp_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1,
+                                                  h2, T, *outs, vp(last.data_ptr()), vp(first.data_ptr()),
+                                                  self._stream(), act)))
+        return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first, s=None, q=None: (
+            self._lib.b200gym_rollout_mlp_norm(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2,
+                                               T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act,
+                                               *norm, s, q)), moments)
 
     def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu", obs_norm=None, norm_epsilon=1e-8,
                           clip_obs=None):
@@ -951,6 +1018,20 @@ class B200VectorEnv:
             return None
         return mean, var, float(eps), c_obs, rvar, c_rew
 
+    def _policy_norm_args(self, what, summary, obs_norm, eps, clip_obs, obs_moments):
+        """Check rollout_linear()'s / rollout_mlp()'s normalisation and moment keywords without a CUDA call ->
+        (None, False) when all four are at their defaults; else the statistics' arguments of the ``_norm`` entry points
+        (mean, var, eps, clip_obs) and whether the moments are asked for."""
+        if not isinstance(obs_moments, (bool, np.bool_)):
+            raise ValueError(f"{what}() needs obs_moments True or False, got {obs_moments!r}")
+        if obs_moments and not summary:
+            raise ValueError(f"{what}() takes obs_moments=True only with summary=True: the full mode returns the "
+                             "observations themselves")
+        norm = self._norm_args(what, obs_norm, eps, clip_obs)
+        if norm is None and not obs_moments:
+            return None, False
+        return (norm[:4] if norm is not None else (None, None, float(eps), math.inf)), bool(obs_moments)
+
     def _critic_params(self, critic, hidden, what):
         """Check rollout_actor_critic()'s critic, D -> hidden -> 1, without a CUDA call."""
         torch = _torch()
@@ -1099,15 +1180,18 @@ class B200VectorEnv:
                            "returned, which alternate between two buffers from call to call, so a replay would read a "
                            "stale set")
 
-    def _policy_rollout(self, what, T, summary, captured, launch):
+    def _policy_rollout(self, what, T, summary, captured, launch, moments=False):
         """The checks after the parameters', the outputs, and the call of rollout_linear() / rollout_mlp() /
         rollout_mlp_noisy(), whose entry point ``launch(T, outs, last, first)`` calls with the output pointers, the
-        buffer that receives the last observations and the observations the env last returned."""
+        buffer that receives the last observations and the observations the env last returned.  ``moments`` (summary
+        mode only): the launch is also given the pointers of two new float64 (N, D) tensors, obs_sum and obs_sumsq,
+        and they are returned after the summary."""
         if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
             raise ValueError(f"{what}(T) needs an integer 1 <= T < 2**31, got {T!r}")
         T = int(T)
         self._refuse_box2d_capture(what)
         first = self._out[self._flip]["obs"]   # the observations the env last returned, before the flip below
+        sums = ()
         torch = _torch()
         n, dev, vp = self.num_envs, self.device, ctypes.c_void_p
         if summary:
@@ -1117,15 +1201,17 @@ class B200VectorEnv:
             self._flip ^= 1
             last = self._out[self._flip]["obs"]
             outs = [None] * 6 + [vp(returns.data_ptr()), vp(lengths.data_ptr()), vp(ended.data_ptr())]
+            if moments:
+                sums = tuple(torch.empty((n, self.obs_dim), dtype=torch.float64, device=dev) for _ in range(2))
         else:
             actions = torch.empty((T, n) if self.discrete else (T, n, self.act_dim),
                                   dtype=torch.int64 if self.discrete else torch.float32, device=dev)
             obs, reward, term, trunc, final_obs, last = self._rollout_outputs(T)
             outs = [vp(actions.data_ptr()), vp(obs.data_ptr()), vp(reward.data_ptr()), vp(term.data_ptr()),
                     vp(trunc.data_ptr()), vp(final_obs.data_ptr()) if self.autoreset else None, None, None, None]
-        _lib.check(launch(T, outs, last, first), self._handle)
+        _lib.check(launch(T, outs, last, first, *(vp(x.data_ptr()) for x in sums)), self._handle)
         if summary:
-            return returns, lengths, ended
+            return (returns, lengths, ended) + sums
         return actions, obs, reward, term, trunc, FinalInfos(final_obs, term, trunc, None, captured)
 
     def _linear_params(self, weight, bias):

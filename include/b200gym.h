@@ -356,6 +356,34 @@ int b200gym_rollout_actor_critic_norm(b200gym_t *h, const float *actor_dev, cons
                                       const double *obs_mean_dev, const double *obs_var_dev, double eps,
                                       float clip_obs, const double *ret_var_dev, float clip_reward);
 
+/*
+ * b200gym_rollout_linear and b200gym_rollout_mlp_act with normalised policy inputs and, in summary mode, the moments of
+ * the raw observations the policy read.  Every observation the policy reads is normalised as in
+ * b200gym_rollout_mlp_noisy_norm; the observations written out stay raw.
+ *   obs_mean_dev, obs_var_dev, eps, clip_obs  as b200gym_rollout_mlp_noisy_norm (both null: raw inputs)
+ *   obs_sum_dev, obs_sumsq_dev  float64 [n][D] each, summary mode only; both null: no moments.  Otherwise, with o_t
+ *                   env i's raw float32 input of step t (step 0's: the observation the env last returned), for
+ *                   t = 0 .. lengths[i] - 1 in step order, every operation rounded:
+ *                       s = +0.0;  s = s + (double)o_t[k]              -> obs_sum[i][k]
+ *                       q = +0.0;  q = q + (double)o_t[k] * (double)o_t[k]   -> obs_sumsq[i][k]
+ * Per-env rows (per_env = 1) are allowed: the statistics are one [D] pair shared by every env.  With null statistics
+ * and null moment buffers each is the call without _norm.  Classic-control kinds: ONE launch.  Box2D kinds: the
+ * launches of the call without _norm, the policy launch after a launch that writes its normalised input rows into a
+ * scratch buffer the handle keeps, and in summary mode one launch per step that folds the moments.
+ */
+int b200gym_rollout_linear_norm(b200gym_t *h, const float *weight_dev, const float *bias_dev, int per_env, int32_t T,
+                                void *actions_out_dev, float *obs_dev, double *reward_dev, uint8_t *terminated_dev,
+                                uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
+                                uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                const double *obs_mean_dev, const double *obs_var_dev, double eps, float clip_obs,
+                                double *obs_sum_dev, double *obs_sumsq_dev);
+int b200gym_rollout_mlp_norm(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                             int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                             uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev,
+                             int32_t *lengths_dev, uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev,
+                             void *stream, int activation, const double *obs_mean_dev, const double *obs_var_dev,
+                             double eps, float clip_obs, double *obs_sum_dev, double *obs_sumsq_dev);
+
 /* Number of invalid Discrete actions seen since the last call (synchronises `stream`). */
 int b200gym_invalid_actions(b200gym_t *h, void *stream, int64_t *count_out);
 
