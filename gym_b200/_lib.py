@@ -172,6 +172,8 @@ SIGNATURES = {
     "b200gym_clone": (_i32, [_vp, _vp, _vp]),
     "b200gym_snapshot_index_error": (_i32, [_vp]),
     "b200gym_rollout_from": (_i32, [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200gym_rollout_from_mlp": (_i32, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32,
+                                        _vp, _vp, ctypes.c_double, ctypes.c_float, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200gym_lunar_get_bodies": (_i32, [_vp, _vp, _vp, _vp]),
     "b200gym_lunar_wind_idx": (_i32, [_vp, _vp, _vp, _i32]),
     "b200gym_walker_get_bodies": (_i32, [_vp, _vp, _vp, _vp]),

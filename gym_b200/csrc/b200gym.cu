@@ -4413,6 +4413,34 @@ static int launch_rollout_from_kind(b200gym *h, const StepArgs &a, int32_t T, co
     return 0;
 }
 
+// The handle's scratch batch of at least B envs, created or grown here, with the snapshot rows of p loaded into envs
+// [0, B).  nullptr on failure, with h's error set
+static b200gym *from_batch_load(b200gym *h, const RolloutFromArgs &p, int64_t B, cudaStream_t st, const char *who) {
+    if (!h->from_batch || h->from_batch->n < B) {
+        if (h->from_batch) b200gym_destroy(h->from_batch);
+        h->from_batch = nullptr;
+        b200gym *s = nullptr;
+        if (b200gym_create(&h->cfg, B, h->device, &s)) {
+            fail(h, "%s: cannot create the scratch batch: %s", who, b200gym_last_error(nullptr));
+            return nullptr;
+        }
+        h->from_batch = s;
+        // the envs a bad row index leaves unloaded step from a valid state: seeded (a zero PCG64 record only ever
+        // draws zero, on which BipedalWalker's terrain draws never finish), then reset
+        const uint32_t seed[4] = {0u, 0u, 0u, 0u};
+        if (b200gym_seed_range(s, seed, 0, st) || launch_reset(s, nullptr, nullptr, nullptr, st)) {
+            fail(h, "%s: %s", who, s->err.c_str());
+            return nullptr;
+        }
+    }
+    b200gym *s = h->from_batch;
+    if (snap_prepare(s, who) || snap_load(s, p.rows, p.n_rows, p.row_idx, nullptr, B, st, h->snap_bad_dev)) {
+        fail(h, "%s", s->err.c_str());
+        return nullptr;
+    }
+    return s;
+}
+
 // A Box2D rollout from rows, composed of what the engine has: the rows loaded into a handle-owned scratch batch of at
 // least B envs (envs [0, B) used), the step sequence of launch_step_box2d per step into one slice of outputs, the fold
 // after each step, and with end states a save of the scratch batch.  Its steps take milliseconds, so fusing them would
@@ -4420,22 +4448,8 @@ static int launch_rollout_from_kind(b200gym *h, const StepArgs &a, int32_t T, co
 static int launch_rollout_from_box2d(b200gym *h, const RolloutFromArgs &p, int64_t B, const void *actions,
                                      int action_dtype, int32_t T, cudaStream_t st) {
     const char *who = "b200gym_rollout_from";
-    if (!h->from_batch || h->from_batch->n < B) {
-        if (h->from_batch) b200gym_destroy(h->from_batch);
-        h->from_batch = nullptr;
-        b200gym *s = nullptr;
-        if (b200gym_create(&h->cfg, B, h->device, &s))
-            return fail(h, "%s: cannot create the scratch batch: %s", who, b200gym_last_error(nullptr));
-        h->from_batch = s;
-        // the envs a bad row index leaves unloaded step from a valid state: seeded (a zero PCG64 record only ever
-        // draws zero, on which BipedalWalker's terrain draws never finish), then reset
-        const uint32_t seed[4] = {0u, 0u, 0u, 0u};
-        if (b200gym_seed_range(s, seed, 0, st) || launch_reset(s, nullptr, nullptr, nullptr, st))
-            return fail(h, "%s: %s", who, s->err.c_str());
-    }
-    b200gym *s = h->from_batch;
-    if (snap_prepare(s, who)) return fail(h, "%s", s->err.c_str());
-    if (snap_load(s, p.rows, p.n_rows, p.row_idx, nullptr, B, st, h->snap_bad_dev)) return fail(h, "%s", s->err.c_str());
+    b200gym *s = from_batch_load(h, p, B, st, who);
+    if (!s) return 1;
     const int64_t D = h->D;
     const size_t obs_bytes = ((size_t)B * D * sizeof(float) + 15) / 16 * 16;
     const size_t r_bytes = ((size_t)B * sizeof(double) + 15) / 16 * 16, f_bytes = ((size_t)B + 15) / 16 * 16;
@@ -4513,4 +4527,240 @@ extern "C" int b200gym_rollout_from(b200gym_t *h, const void *snap_rows_dev, int
     case B200GYM_ACROBOT: return launch_rollout_from_kind<B200GYM_ACROBOT>(h, a, T, p, st);
     }
     return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+// ---- closed-loop MLP-policy rollouts from snapshot rows (b200gym_rollout_from_mlp) ----
+// Branch b's T steps from its row under its MLP policy (rollout_from_mlp_env), one thread per branch: s_flags as
+// rollout_from_kernel's, a shared policy staged per CTA as rollout_mlp_kernel's (PER_BRANCH: branch b's row read from
+// device memory), and the statistics as rollout_mlp_norm_kernel's (q.mean null: raw inputs).  Launch bounds as
+// rollout_mlp_kernel's
+template <int KIND, bool STATES, bool PER_BRANCH, int ACT>
+__global__ void __launch_bounds__(kThreads, PER_BRANCH ? 1 : 2)
+    rollout_from_mlp_kernel(const StepArgs a, const int32_t T, const RolloutFromMlpArgs p, const ObsNormArgs q) {
+    __shared__ uint8_t s_flags[kThreads];
+    using Src = MlpActions<KIND, true, PER_BRANCH, ACT>;
+    constexpr int K = Src::K, D = Src::D;
+    __shared__ double mean[D], sd[D];
+    if (q.mean) norm_stage<D>(q, mean, sd);
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float *w;
+    if constexpr (PER_BRANCH) {
+        __syncthreads();
+        w = p.mlp.params + b * p.mlp.stride;
+    } else {
+        w = mlp_stage(p.mlp.params, mlp_param_count<K, D>(p.mlp.h1, p.mlp.h2));
+    }
+    if (b >= a.n) return;
+    StepArgs c = a;
+    c.flags = s_flags;
+    rollout_from_mlp_env<KIND, STATES, PER_BRANCH, ACT>(c, b, (int)threadIdx.x, T, w, p, q.mean ? mean : nullptr, sd,
+                                                        q.clip);
+}
+
+// The Box2D path's step-0 inputs: snapshot observation row row_idx[b] (row b without indices) into obs[b], zeros for a
+// branch whose index is out of range (its outputs are zeroed at the end)
+__global__ void __launch_bounds__(kThreads) rollout_from_obs_kernel(const float *snap_obs, const RolloutFromArgs p,
+                                                                    int64_t B, int D, float *obs) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int64_t row = p.row_idx ? p.row_idx[b] : b;
+    const bool ok = row >= 0 && row < p.n_rows;
+    for (int k = 0; k < D; k++) obs[b * D + k] = ok ? snap_obs[row * D + k] : 0.0f;
+}
+
+// ... and, with rollout_from_skip_kernel, zero the `bytes` bytes of step-0 action of every skipped branch
+__global__ void __launch_bounds__(kThreads) rollout_from_first_skip_kernel(const RolloutFromArgs p, int64_t B,
+                                                                           unsigned char *first, int bytes) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int64_t row = p.row_idx[b];
+    if (row >= 0 && row < p.n_rows) return;
+    for (int k = 0; k < bytes; k++) first[b * bytes + k] = 0;
+}
+
+template <int KIND, int ACT>
+static int launch_rollout_from_mlp_kind(b200gym *h, const StepArgs &a, int32_t T, const RolloutFromMlpArgs &p,
+                                        const ObsNormArgs &q, bool per_branch, size_t smem, cudaStream_t st) {
+    if (snap_row_bytes(KIND) != classic_row_bytes<KIND>())
+        return fail(h, "b200gym_rollout_from_mlp: row layout mismatch for kind %d", KIND);
+    const unsigned blocks = blocks_for(a.n);
+    const bool states = p.from.end_rows != nullptr;
+    if (per_branch) {
+        if (states) rollout_from_mlp_kernel<KIND, true, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, p, q);
+        else rollout_from_mlp_kernel<KIND, false, true, ACT><<<blocks, kThreads, 0, st>>>(a, T, p, q);
+    } else {
+        if (states) rollout_from_mlp_kernel<KIND, true, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, p, q);
+        else rollout_from_mlp_kernel<KIND, false, false, ACT><<<blocks, kThreads, smem, st>>>(a, T, p, q);
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// A Box2D rollout from rows under an MLP policy, composed as launch_rollout_from_box2d's: the rows loaded into the
+// scratch batch, the step-0 inputs gathered from the snapshot's observation rows, and per step the policy launch of
+// b200gym_rollout_mlp (mlp_policy_kernel) or b200gym_rollout_mlp_noisy (mlp_noisy_policy_kernel, its outputs to a
+// scratch slice), after a norm_rows_kernel launch when normalising, then launch_step_box2d and the fold.  Step 0's
+// actions are copied out; the end states and skipped branches as launch_rollout_from_box2d's
+template <int K, int D, bool DISCRETE, int ACT>
+static int launch_rollout_from_mlp_box2d(b200gym *h, const RolloutFromMlpArgs &p, const float *snap_obs, int64_t B,
+                                         int32_t T, const ObsNormArgs &q, bool per_branch, size_t smem,
+                                         cudaStream_t st) {
+    const char *who = "b200gym_rollout_from_mlp";
+    b200gym *s = from_batch_load(h, p.from, B, st, who);
+    if (!s) return 1;
+    const int action_dtype = DISCRETE ? B200GYM_ACT_I64 : B200GYM_ACT_F32;
+    const size_t act_bytes = DISCRETE ? sizeof(long long) : (size_t)K * sizeof(float);   // Box kinds: K = A
+    auto up16 = [](size_t x) { return (x + 15) / 16 * 16; };
+    const size_t obs_bytes = up16((size_t)B * D * sizeof(float)), a_bytes = up16((size_t)B * act_bytes);
+    const size_t r_bytes = up16((size_t)B * sizeof(double)), f_bytes = up16((size_t)B);
+    const size_t z_bytes = p.noise ? up16((size_t)B * K * sizeof(float)) : 0;
+    void *scratch = nullptr;
+    CK(h, cudaMallocAsync(&scratch, 3 * obs_bytes + a_bytes + r_bytes + 2 * f_bytes + z_bytes, st));
+    unsigned char *base = static_cast<unsigned char *>(scratch);
+    float *first_obs = reinterpret_cast<float *>(base), *obs = reinterpret_cast<float *>(base + obs_bytes);
+    float *x = reinterpret_cast<float *>(base + 2 * obs_bytes);
+    void *actions = base + 3 * obs_bytes;
+    double *reward = reinterpret_cast<double *>(base + 3 * obs_bytes + a_bytes);
+    uint8_t *term = base + 3 * obs_bytes + a_bytes + r_bytes, *trunc = term + f_bytes;
+    float *outputs = reinterpret_cast<float *>(trunc + f_bytes);
+    StepArgs a = make_args(s, actions, obs, reward, term, trunc, nullptr);
+    a.count = B;
+    a.invalid = h->invalid;
+    a.invalid_seen = h->invalid_seen_dev;
+    const unsigned blocks = blocks_for(B);
+    const size_t pol_smem = per_branch ? 0 : smem;
+    int rc = 0;
+    rollout_from_obs_kernel<<<blocks, kThreads, 0, st>>>(snap_obs, p.from, B, D, first_obs);
+    if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: rollout_from_obs_kernel launch failed", who);
+    for (int32_t t = 0; t < T && !rc; t++) {
+        const float *in = t == 0 ? first_obs : obs;
+        if (q.mean) {
+            norm_rows_kernel<<<blocks_for(B * D), kThreads, 0, st>>>(in, x, B * D, D, q);
+            if (cudaGetLastError() != cudaSuccess) {
+                rc = fail(h, "norm_rows_kernel: launch failed");
+                break;
+            }
+            in = x;
+        }
+        if (p.noise) {
+            const MlpNoisyArgs r{p.mlp, p.noise + (int64_t)t * B * K, outputs};
+            if (per_branch)
+                mlp_noisy_policy_kernel<K, D, DISCRETE, true, ACT><<<blocks, kThreads, 0, st>>>(
+                    in, actions, r, nullptr, nullptr, nullptr, B, -1, 1, 0);
+            else
+                mlp_noisy_policy_kernel<K, D, DISCRETE, false, ACT><<<blocks, kThreads, pol_smem, st>>>(
+                    in, actions, r, nullptr, nullptr, nullptr, B, -1, 1, 0);
+        } else {
+            if (per_branch)
+                mlp_policy_kernel<K, D, DISCRETE, true, ACT><<<blocks, kThreads, 0, st>>>(
+                    in, actions, p.mlp, nullptr, nullptr, nullptr, B, -1, 1, 0);
+            else
+                mlp_policy_kernel<K, D, DISCRETE, false, ACT><<<blocks, kThreads, pol_smem, st>>>(
+                    in, actions, p.mlp, nullptr, nullptr, nullptr, B, -1, 1, 0);
+        }
+        if (cudaGetLastError() != cudaSuccess) {
+            rc = fail(h, "%s: policy launch failed", who);
+            break;
+        }
+        if (t == 0 && cudaMemcpyAsync(p.first_actions, actions, (size_t)B * act_bytes, cudaMemcpyDeviceToDevice, st)) {
+            rc = fail(h, "%s: copy of the step-0 actions failed", who);
+            break;
+        }
+        if (launch_step_box2d(s, a, action_dtype, st)) {
+            rc = fail(h, "%s", s->err.c_str());
+            break;
+        }
+        rollout_from_fold_kernel<<<blocks, kThreads, 0, st>>>(p.from, B, reward, term, trunc, t);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: rollout_from_fold_kernel launch failed", who);
+    }
+    if (!rc && p.from.end_rows) {
+        if (snap_save(s, nullptr, B, p.from.end_rows, st)) rc = fail(h, "%s", s->err.c_str());
+        else if (cudaMemcpyAsync(p.from.end_obs, obs, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToDevice, st))
+            rc = fail(h, "%s: copy of the end observations failed", who);
+    }
+    if (!rc && p.from.row_idx) {
+        rollout_from_skip_kernel<<<blocks, kThreads, 0, st>>>(p.from, B, snap_row_bytes(h->cfg.kind), D);
+        rollout_from_first_skip_kernel<<<blocks, kThreads, 0, st>>>(p.from, B,
+                                                                    static_cast<unsigned char *>(p.first_actions),
+                                                                    (int)act_bytes);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(h, "%s: skip launch failed", who);
+    }
+    cudaFreeAsync(scratch, st);
+    return rc;
+}
+
+template <int ACT>
+static int launch_rollout_from_mlp(b200gym *h, const StepArgs &a, int32_t T, const RolloutFromMlpArgs &p,
+                                   const float *snap_obs, const ObsNormArgs &q, bool pb, size_t smem, cudaStream_t st) {
+    const int64_t B = a.n;
+    switch (h->cfg.kind) {
+    case B200GYM_CARTPOLE: return launch_rollout_from_mlp_kind<B200GYM_CARTPOLE, ACT>(h, a, T, p, q, pb, smem, st);
+    case B200GYM_MOUNTAINCAR: return launch_rollout_from_mlp_kind<B200GYM_MOUNTAINCAR, ACT>(h, a, T, p, q, pb, smem, st);
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_from_mlp_kind<B200GYM_MOUNTAINCAR_CONT, ACT>(h, a, T, p, q, pb, smem, st);
+    case B200GYM_PENDULUM: return launch_rollout_from_mlp_kind<B200GYM_PENDULUM, ACT>(h, a, T, p, q, pb, smem, st);
+    case B200GYM_ACROBOT: return launch_rollout_from_mlp_kind<B200GYM_ACROBOT, ACT>(h, a, T, p, q, pb, smem, st);
+    case B200GYM_LUNARLANDER:
+        return launch_rollout_from_mlp_box2d<4, 8, true, ACT>(h, p, snap_obs, B, T, q, pb, smem, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_from_mlp_box2d<2, 8, false, ACT>(h, p, snap_obs, B, T, q, pb, smem, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_from_mlp_box2d<4, 24, false, ACT>(h, p, snap_obs, B, T, q, pb, smem, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+extern "C" int b200gym_rollout_from_mlp(b200gym_t *h, const void *snap_rows_dev, const float *snap_obs_dev,
+                                        int64_t n_rows, const int64_t *row_idx_dev, int64_t B, const float *params_dev,
+                                        int per_branch, int n_layers, int h1, int h2, int32_t T, const float *noise_dev,
+                                        int activation, const double *obs_mean_dev, const double *obs_var_dev,
+                                        double eps, float clip_obs, double *returns_dev, int32_t *lengths_dev,
+                                        uint8_t *ended_dev, void *first_actions_dev, void *end_rows_dev,
+                                        float *end_obs_dev, void *stream) {
+    const char *what = "b200gym_rollout_from_mlp";
+    if (!h) return fail(h, "%s: null handle", what);
+    if (B < 1) return fail(h, "%s: B must be at least 1 (got %lld)", what, (long long)B);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (n_rows < 0 || (!row_idx_dev && n_rows < B))
+        return fail(h, "%s: %lld rows cannot start %lld branches without row indices", what, (long long)n_rows,
+                    (long long)B);
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "%s: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)", what, activation);
+    if (n_layers != 1 && n_layers != 2) return fail(h, "%s: n_layers must be 1 or 2 (got %d)", what, n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "%s: hidden widths must be 1 .. %d (got %d, %d)", what, kMlpMaxWidth, h1, h2);
+    if (int rc = norm_args_check(h, what, obs_mean_dev, obs_var_dev, eps, clip_obs)) return rc;
+    if (noise_dev && per_branch && obs_mean_dev)
+        return fail(h, "%s: normalised inputs with noise need one policy shared by every branch (per_branch = 0)", what);
+    if (!params_dev || !returns_dev || !lengths_dev || !ended_dev || !first_actions_dev)
+        return fail(h, "%s: null buffer", what);
+    if (!end_rows_dev != !end_obs_dev) return fail(h, "%s: give both end_rows_dev and end_obs_dev, or neither", what);
+    if (snap_check_ptr(h, snap_rows_dev, what)) return 1;
+    if (end_rows_dev && (uintptr_t)end_rows_dev % 128 != 0) return fail(h, "%s: end_rows_dev must be 128-byte aligned", what);
+    const bool box2d = h->is_lunar || h->is_walker;
+    if (box2d && !snap_obs_dev) return fail(h, "%s: a Box2D env needs snap_obs_dev", what);
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = h->A == 0 ? h->NACT : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    // as b200gym_rollout_mlp_act
+    const bool vec = h1 % 4 == 0 && (!per_branch || (P % 4 == 0 && reinterpret_cast<uintptr_t>(params_dev) % 16 == 0));
+    DeviceGuard guard(h->device);
+    if (row_idx_dev && snap_prepare(h, what)) return 1;
+    const RolloutFromMlpArgs p{{static_cast<const unsigned char *>(snap_rows_dev), n_rows, row_idx_dev, returns_dev,
+                                lengths_dev, ended_dev, static_cast<unsigned char *>(end_rows_dev), end_obs_dev,
+                                h->snap_bad_dev},
+                               {params_dev, per_branch ? P : 0, h1, h2, vec ? 1 : 0, nullptr, nullptr, nullptr},
+                               noise_dev,
+                               first_actions_dev};
+    const ObsNormArgs q{obs_mean_dev, obs_var_dev, eps, clip_obs};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;
+    cudaStream_t st = (cudaStream_t)stream;
+    StepArgs a = make_args(h, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    a.state = nullptr; a.elapsed = nullptr; a.flags = nullptr; a.rng = nullptr; a.lunar_rec = nullptr;   // not h's envs
+    a.n = B; a.count = B;
+    const bool pb = per_branch != 0;
+    if (activation == B200GYM_MLP_TANH)
+        return launch_rollout_from_mlp<B200GYM_MLP_TANH>(h, a, T, p, snap_obs_dev, q, pb, smem, st);
+    return launch_rollout_from_mlp<B200GYM_MLP_RELU>(h, a, T, p, snap_obs_dev, q, pb, smem, st);
 }

@@ -1347,6 +1347,113 @@ __device__ __forceinline__ void rollout_from_env(const StepArgs &a, int64_t b, I
     }
 }
 
+// ---- closed-loop MLP-policy rollouts from snapshot rows (b200gym_rollout_from_mlp) ---------------------------------
+
+// The arguments of a b200gym_rollout_from_mlp launch: the rows, outputs and end states as rollout_from's (from), the
+// policy (mlp: branch b's parameters are params + b * stride; no summary pointers), the noise (null: none; otherwise
+// slice 0 of [T][B][K]) and the action each branch took at step 0, [B] long long (Discrete) or [B][A] float (Box)
+struct RolloutFromMlpArgs {
+    RolloutFromArgs from;
+    MlpPolicyArgs mlp;
+    const float *noise;
+    void *first_actions;
+};
+
+// T steps of branch b under its MLP policy at w (rollout_from_mlp_kernel): rollout_from_env's row load, flag byte and
+// end row with rollout_mlp_env's policy step, written out again so that no pre-existing kernel changes.  Step 0's
+// input is observe() of the row's state, as rollout_mlp_env's is of the env's.  The policy reads x = norm_obs_or_raw(o)
+// (mean null: o itself); with noise, the action is taken from z + noise[t][b] (noisy_outputs' adds, without its
+// stores), and without, from z itself, so the deterministic actions are rollout_mlp_env's bits.  Both choices are the
+// same for every thread of the launch.  Nothing is stored per step but the action of step 0; a skipped branch gets
+// zeros.  GLOBAL and ACT as rollout_mlp_env, STATES as rollout_from_env
+template <int KIND, bool STATES, bool GLOBAL, int ACT, typename I>
+__device__ __forceinline__ void rollout_from_mlp_env(const StepArgs &a, int64_t b, I f, int32_t T, const float *w,
+                                                     const RolloutFromMlpArgs &p, const double *mean, const double *sd,
+                                                     float clip) {
+    using E = bgym::Env<KIND>;
+    using ActT = typename std::conditional<E::A == 0, long long, float>::type;
+    constexpr int K = MlpActions<KIND, true, GLOBAL, ACT>::K, R = classic_row_bytes<KIND>(), C = R / 16;
+    static_assert(E::A <= 1, "one action element per branch");
+    const RolloutFromArgs &q = p.from;
+    ActT *first = static_cast<ActT *>(p.first_actions);
+    const int64_t row = q.row_idx ? q.row_idx[b] : b;
+    if (row < 0 || row >= q.n_rows) {
+        *reinterpret_cast<volatile unsigned long long *>(q.bad) = 1ULL;
+        q.returns[b] = 0.0;
+        q.lengths[b] = 0;
+        q.ended[b] = 0;
+        first[b] = (ActT)0;
+        if constexpr (STATES) {
+            ulonglong2 *out = reinterpret_cast<ulonglong2 *>(q.end_rows + b * R);
+#pragma unroll
+            for (int c = 0; c < C; c++) out[c] = make_ulonglong2(0ULL, 0ULL);
+#pragma unroll
+            for (int k = 0; k < E::D; k++) q.end_obs[b * E::D + k] = 0.0f;
+        }
+        return;
+    }
+    const ulonglong2 *in = reinterpret_cast<const ulonglong2 *>(q.rows + row * R);
+    bgym::Pcg64 g = bgym::pcg64_load(reinterpret_cast<const uint64_t *>(in));
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k += 2) {
+        const ulonglong2 v = __ldg(in + 2 + k / 2);
+        s[k] = __longlong_as_double((long long)v.x);
+        s[k + 1] = __longlong_as_double((long long)v.y);
+    }
+    const ulonglong2 tail = __ldg(in + 2 + E::S / 2);   // {elapsed | flags << 32, 0}
+    int32_t elapsed = (int32_t)(uint32_t)tail.x;
+    a.flags[f] = (uint8_t)(tail.x >> 32);
+    float o[E::D], x[E::D];
+    E::observe(s, o);
+    const int h1 = p.mlp.h1, h2 = p.mlp.h2;
+    const bool vec = p.mlp.vec != 0;
+    const float *noise = p.noise ? p.noise + b * K : nullptr;
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, true> sink{{s, elapsed, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, o, ret, len, ended};
+    for (int32_t t = 0; t < T; t++) {
+        norm_obs_or_raw<E::D>(o, mean, sd, clip, x);
+        float z[K];
+        mlp_outputs<K, E::D, GLOBAL, ACT>(w, h1, h2, vec, x, z);
+        if (noise) {
+            float e[K];
+#pragma unroll
+            for (int k = 0; k < K; k++) e[k] = load_once(noise + k);
+#pragma unroll
+            for (int k = 0; k < K; k++) z[k] = z[k] + e[k];
+            noise += a.n * K;
+        }
+        ActT v;
+        if constexpr (E::A == 0) v = (ActT)argmax_first<K>(z);
+        else v = z[0];
+        if (t == 0) first[b] = v;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(v, action_int, a0);
+        if (advance_env<KIND>(a, sink, f, s, elapsed, action_int, a0)) reset_env_from<KIND>(sink, f, g);
+    }
+    q.returns[b] = ret;
+    q.lengths[b] = len;
+    q.ended[b] = ended ? 1 : 0;
+    if constexpr (STATES) {
+        static_assert(E::S % 2 == 0 && 2 + E::S / 2 + 1 <= C, "row layout");
+        ulonglong2 *out = reinterpret_cast<ulonglong2 *>(q.end_rows + b * R);
+        out[0] = make_ulonglong2((unsigned long long)(uint64_t)(g.state >> 64), (unsigned long long)(uint64_t)g.state);
+        out[1] = make_ulonglong2((unsigned long long)(uint64_t)(g.inc >> 64), (unsigned long long)(uint64_t)g.inc);
+#pragma unroll
+        for (int k = 0; k < E::S; k += 2)
+            out[2 + k / 2] = make_ulonglong2((unsigned long long)__double_as_longlong(s[k]),
+                                             (unsigned long long)__double_as_longlong(s[k + 1]));
+        out[2 + E::S / 2] = make_ulonglong2((unsigned long long)(uint32_t)elapsed |
+                                                ((unsigned long long)a.flags[f] << 32), 0ULL);
+#pragma unroll
+        for (int c = 2 + E::S / 2 + 1; c < C; c++) out[c] = make_ulonglong2(0ULL, 0ULL);
+        store_row<E::D>(q.end_obs, b, o);
+    }
+}
+
 // reset(options={"low", "high"}) of env i (reset_kernel): state, TimeLimit counter, flags and, if obs is given, the
 // observation row.  References as in lunar_reset_env.
 template <int KIND>

@@ -1101,51 +1101,18 @@ class B200VectorEnv:
         read the current contents of ``snap.rows``, ``rows`` and ``actions`` (the first call with CUDA-tensor ``rows``
         allocates the env's index-error flag, so make one outside the capture).  The Box2D kinds load the rows into a
         scratch batch the env keeps and step it launch by launch; they cannot be captured (DESIGN.md §4.16)."""
-        captured = self._rollout_guards("rollout_from", reset_needed=False)
-        if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
-                         _lib.KIND_BIPEDALWALKER_HARDCORE):
-            refuse_capture("rollout_from() of a Box2D env", "it steps a scratch batch that is created on first use, "
-                           "through a scratch allocation per call")
-        if not isinstance(snap, EnvSnapshot):
-            raise error.Error(f"rollout_from() needs an EnvSnapshot, got {type(snap).__name__}")
-        R = self.snapshot_row_bytes
-        check_compatible(snap.header, self.kind, R, self._snapshot_config())
+        captured, r, idx, B = self._from_rows("rollout_from", snap, rows)
         torch = _torch()
-        r = snap.rows
-        if not (isinstance(r, torch.Tensor) and r.dtype == torch.uint8 and r.device == self.device and r.dim() == 2
-                and r.shape[1] == R and r.is_contiguous()):
-            raise error.Error(f"rollout_from() needs the snapshot's rows as a contiguous uint8 (m, {R}) tensor on "
-                              f"{self.device}")
         m = int(r.shape[0])
-        if rows is None:
-            idx, B = None, m
-        elif isinstance(rows, torch.Tensor) and rows.is_cuda:
-            if rows.dim() != 1 or rows.dtype.is_floating_point or rows.dtype == torch.bool or rows.device != self.device:
-                raise error.Error(f"rollout_from() rows must be a 1-D integer tensor on {self.device}, got {rows.dtype} "
-                                  f"of shape {tuple(rows.shape)} on {rows.device}")
-            idx, B = rows, int(rows.shape[0])
-        else:
-            if captured:
-                raise error.Error("rollout_from() cannot be captured in a CUDA graph with host rows: the host-to-device "
-                                  "copy cannot be replayed; pass a CUDA tensor")
-            idx = host_indices(rows.numpy() if isinstance(rows, torch.Tensor) else rows, m, "rollout_from rows")
-            B = int(idx.shape[0])
-        if B < 1:
-            raise error.Error("rollout_from() needs at least one branch, got B = 0")
         act, code = self._device_actions(actions, captured, steps=True, n=B, what="rollout_from()")
         T = int(act.shape[0])
         if T > 2 ** 31 - 1:
             raise error.Error(f"rollout_from() needs T < 2**31, got {T}")
         if self.discrete and code != _lib.ACT_I64:
             act, code = act.to(torch.int64), _lib.ACT_I64
-        if idx is not None:
-            idx = (torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx).to(self.device, torch.int64).contiguous()
-        dev, vp = self.device, ctypes.c_void_p
-        returns = torch.empty(B, dtype=torch.float64, device=dev)
-        lengths = torch.empty(B, dtype=torch.int32, device=dev)
-        ended = torch.empty(B, dtype=torch.bool, device=dev)
-        end_rows = torch.empty((B, R), dtype=torch.uint8, device=dev) if states else None
-        end_obs = torch.empty((B, self.obs_dim), dtype=torch.float32, device=dev) if states else None
+        idx = self._device_rows(idx)
+        vp = ctypes.c_void_p
+        returns, lengths, ended, end_rows, end_obs = self._from_outputs(B, states)
         _lib.check(self._lib.b200gym_rollout_from(
             self._handle, vp(r.data_ptr()), m, None if idx is None else vp(idx.data_ptr()), B, vp(act.data_ptr()), code,
             T, vp(returns.data_ptr()), vp(lengths.data_ptr()), vp(ended.data_ptr()),
@@ -1155,8 +1122,165 @@ class B200VectorEnv:
             return returns, lengths, ended, EnvSnapshot(snap.header, end_rows, end_obs)
         return returns, lengths, ended
 
-    def _noise_steps(self, noise, what="rollout_mlp_noisy"):
-        """Check rollout_mlp_noisy()'s or rollout_actor_critic()'s noise without a CUDA call -> T."""
+    def rollout_from_mlp(self, snap, params, hidden, T, *, noise=None, rows=None, states=False, activation="relu",
+                         obs_norm=None, norm_epsilon=1e-8, clip_obs=None):
+        """T steps of an MLP policy in closed loop on B branches, each from a snapshot row, without touching this env
+        -> ``(returns, lengths, ended, first_actions)``, and with ``states=True`` also an ``EnvSnapshot`` of the B end
+        states.
+
+        ``snap``, ``rows`` and ``states`` are ``rollout_from()``'s: B = ``len(rows)``, or ``len(snap)`` without rows;
+        rows may repeat; an out-of-range CUDA-tensor row skips its branch and makes the next call raise.  ``params``,
+        ``hidden`` and ``activation`` are ``rollout_mlp()``'s, with per-policy rows indexed by branch: shape (P,) is
+        one policy for every branch, (B, P) one per branch (branch b's row b, not row ``rows[b]``).  ``T`` is an
+        integer, 1 <= T < 2**31.  ``noise`` is None (the deterministic policy) or float32 (T, B, K), contiguous, on the
+        env's device, with ``rollout_mlp_noisy()``'s rule ``rule(z + noise[t])``; a shape that disagrees with T or B
+        raises ``ValueError``.  ``obs_norm``, ``norm_epsilon`` and ``clip_obs`` are ``rollout_mlp()``'s; ``noise``
+        together with per-branch rows and ``obs_norm`` is refused, as ``rollout_mlp_noisy()`` refuses per-env rows
+        with ``obs_norm``.
+
+        ``returns`` (float64), ``lengths`` (int32) and ``ended`` (bool), each (B,), are ``rollout_from()``'s fold over
+        each branch's first episode.  ``first_actions`` is the action each branch took at step 0, int64 (B,) for
+        Discrete kinds and float32 (B, A) for Box kinds: the action a planner executes.  A skipped branch gets 0.
+
+        Bit for bit, with ``twin`` a fresh env of the same id and config with B envs::
+
+            twin.restore(EnvSnapshot(snap.header, snap.rows[rows], snap.obs[rows]))
+            a, obs, r, te, tr, info = twin.rollout_mlp(params, hidden, T, activation=..., obs_norm=..., ...)  # no noise
+            a, z, obs, r, te, tr, info = twin.rollout_mlp_noisy(params, hidden, noise, activation=..., ...)  # noise
+
+        the results are ``rollout_from()``'s fold of ``r``, ``te`` and ``tr``, ``first_actions == a[0]``, and the end
+        states are ``twin.snapshot()``.  The classic kinds' step 0 reads ``observe()`` of the row's state, the Box2D
+        kinds' ``snap.obs[rows]``, which is what the restored twin reads.  This env's state, RNG records, TimeLimit
+        counters, flags, observation buffers and action-space generator do not move, and it needs no ``reset()``.
+
+        MCTS leaf evaluation with a Gumbel-sampled tanh actor, K samples from each of R leaves (CartPole)::
+
+            rows = torch.arange(R, device=dev).repeat_interleave(K)            # R * K branches
+            u = torch.rand(T, R * K, 2, device=dev).clamp_(min=torch.finfo(torch.float32).tiny)
+            g = -torch.log(-torch.log(u))                                       # samples softmax(actor(o))
+            ret, length, ended, a0 = real.rollout_from_mlp(leaves, pa, (64, 64), T, noise=g, rows=rows,
+                                                           activation="tanh")
+            value = ret.view(R, K).mean(1)                                      # each leaf's Monte-Carlo value
+
+        MPPI on Pendulum with a policy prior, R roots of ``real`` and K samples of ``policy(o) + noise[t]`` each::
+
+            snap = real.snapshot(roots)
+            rows = torch.arange(R, device=dev).repeat_interleave(K)
+            eps = sigma * torch.randn(T, R * K, 1, device=dev)
+            ret, _, _, a0 = real.rollout_from_mlp(snap, prior, (64, 64), T, noise=eps, rows=rows, activation="tanh")
+            w = torch.softmax(ret.view(R, K) / temperature, dim=1)              # weights of the K samples of each root
+            u = (w[..., None] * a0.view(R, K, 1)).sum(1)                        # the action each root executes
+
+        ES with antithetic per-branch policies on common start states, P pairs from S rows::
+
+            delta = torch.randn(P, theta.numel(), device=dev)
+            pop = torch.cat([theta + sigma * delta, theta - sigma * delta]).repeat_interleave(S, 0)   # (2 * P * S, n)
+            rows = torch.arange(S, device=dev).repeat(2 * P)                    # every policy from the same S rows
+            ret, _, _, _ = real.rollout_from_mlp(starts, pop, (64, 64), T, rows=rows, activation="tanh")
+            f = ret.view(2, P, S).mean(2)
+            theta += alpha / (2 * P * sigma) * ((f[0] - f[1])[:, None] * delta).sum(0)
+
+        Refused where ``rollout_from()`` is (``backend="numpy"``, ``wrappers=``, a pending async call), and for bad
+        parameters, noise or statistics, before any CUDA call and with the messages of ``rollout_from()``,
+        ``rollout_mlp()`` and ``rollout_mlp_noisy()``.  The classic-control kinds run in one launch, one thread per
+        branch, and may be captured in a CUDA graph: replays read the current ``snap.rows``, ``rows``, ``params``,
+        ``noise`` and statistics.  The Box2D kinds compose the twin launch by launch in ``rollout_from()``'s scratch
+        batch and cannot be captured (DESIGN.md §4.20)."""
+        what = "rollout_from_mlp"
+        captured, r, idx, B = self._from_rows(what, snap, rows)
+        if isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or not 1 <= int(T) <= 2 ** 31 - 1:
+            raise ValueError(f"{what}(T) needs an integer 1 <= T < 2**31, got {T!r}")
+        T = int(T)
+        h1, h2, per_branch, act = self._mlp_params(params, hidden, activation, what, n=B)
+        if noise is not None and self._noise_steps(noise, what, n=B) != T:
+            raise ValueError(f"{what}() needs noise of T = {T} steps, got {tuple(noise.shape)}")
+        norm = self._norm_args(what, obs_norm, norm_epsilon, clip_obs, per_env=per_branch and noise is not None)
+        mean, var, eps, c_obs = norm[:4] if norm is not None else (None, None, float(norm_epsilon), math.inf)
+        torch = _torch()
+        m = int(r.shape[0])
+        box2d = self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
+                              _lib.KIND_BIPEDALWALKER_HARDCORE)
+        o = snap.obs
+        if box2d and not (isinstance(o, torch.Tensor) and o.dtype == torch.float32 and o.device == self.device
+                          and tuple(o.shape) == (m, self.obs_dim) and o.is_contiguous()):
+            raise error.Error(f"{what}() of a Box2D env needs the snapshot's observations as a contiguous float32 "
+                              f"({m}, {self.obs_dim}) tensor on {self.device}")
+        idx = self._device_rows(idx)
+        vp = ctypes.c_void_p
+        returns, lengths, ended, end_rows, end_obs = self._from_outputs(B, states)
+        first = torch.empty(B, dtype=torch.int64, device=self.device) if self.discrete else torch.empty(
+            (B, self.act_dim), dtype=torch.float32, device=self.device)
+        _lib.check(self._lib.b200gym_rollout_from_mlp(
+            self._handle, vp(r.data_ptr()), vp(o.data_ptr()) if box2d else None, m,
+            None if idx is None else vp(idx.data_ptr()), B, vp(params.data_ptr()), int(per_branch), len(hidden), h1,
+            h2, T, None if noise is None else vp(noise.data_ptr()), act, mean, var, eps, c_obs,
+            vp(returns.data_ptr()), vp(lengths.data_ptr()), vp(ended.data_ptr()), vp(first.data_ptr()),
+            vp(end_rows.data_ptr()) if states else None, vp(end_obs.data_ptr()) if states else None, self._stream()),
+            self._handle)
+        if states:
+            return returns, lengths, ended, first, EnvSnapshot(snap.header, end_rows, end_obs)
+        return returns, lengths, ended, first
+
+    def _from_rows(self, what, snap, rows):
+        """The guards of rollout_from() / rollout_from_mlp() and their snapshot and rows checks, all before any CUDA
+        call -> (whether a CUDA graph is being captured, the snapshot's rows, the row indices (None, a CUDA tensor or
+        a checked host int64 array), B)."""
+        captured = self._rollout_guards(what, reset_needed=False)
+        if self.kind in (_lib.KIND_LUNARLANDER, _lib.KIND_LUNARLANDER_CONT, _lib.KIND_BIPEDALWALKER,
+                         _lib.KIND_BIPEDALWALKER_HARDCORE):
+            refuse_capture(f"{what}() of a Box2D env", "it steps a scratch batch that is created on first use, "
+                           "through a scratch allocation per call")
+        if not isinstance(snap, EnvSnapshot):
+            raise error.Error(f"{what}() needs an EnvSnapshot, got {type(snap).__name__}")
+        R = self.snapshot_row_bytes
+        check_compatible(snap.header, self.kind, R, self._snapshot_config())
+        torch = _torch()
+        r = snap.rows
+        if not (isinstance(r, torch.Tensor) and r.dtype == torch.uint8 and r.device == self.device and r.dim() == 2
+                and r.shape[1] == R and r.is_contiguous()):
+            raise error.Error(f"{what}() needs the snapshot's rows as a contiguous uint8 (m, {R}) tensor on "
+                              f"{self.device}")
+        m = int(r.shape[0])
+        if rows is None:
+            idx, B = None, m
+        elif isinstance(rows, torch.Tensor) and rows.is_cuda:
+            if rows.dim() != 1 or rows.dtype.is_floating_point or rows.dtype == torch.bool or rows.device != self.device:
+                raise error.Error(f"{what}() rows must be a 1-D integer tensor on {self.device}, got {rows.dtype} "
+                                  f"of shape {tuple(rows.shape)} on {rows.device}")
+            idx, B = rows, int(rows.shape[0])
+        else:
+            if captured:
+                raise error.Error(f"{what}() cannot be captured in a CUDA graph with host rows: the host-to-device "
+                                  "copy cannot be replayed; pass a CUDA tensor")
+            idx = host_indices(rows.numpy() if isinstance(rows, torch.Tensor) else rows, m, f"{what} rows")
+            B = int(idx.shape[0])
+        if B < 1:
+            raise error.Error(f"{what}() needs at least one branch, got B = 0")
+        return captured, r, idx, B
+
+    def _device_rows(self, idx):
+        """_from_rows()'s row indices as the entry points take them: None, or int64 on the env's device."""
+        if idx is None:
+            return None
+        torch = _torch()
+        return (torch.from_numpy(idx) if isinstance(idx, np.ndarray) else idx).to(self.device, torch.int64).contiguous()
+
+    def _from_outputs(self, B, states):
+        """The outputs of rollout_from() / rollout_from_mlp(): returns, lengths, ended, and with states the end rows
+        and observations (else None, None)."""
+        torch = _torch()
+        dev = self.device
+        returns = torch.empty(B, dtype=torch.float64, device=dev)
+        lengths = torch.empty(B, dtype=torch.int32, device=dev)
+        ended = torch.empty(B, dtype=torch.bool, device=dev)
+        end_rows = torch.empty((B, self.snapshot_row_bytes), dtype=torch.uint8, device=dev) if states else None
+        end_obs = torch.empty((B, self.obs_dim), dtype=torch.float32, device=dev) if states else None
+        return returns, lengths, ended, end_rows, end_obs
+
+    def _noise_steps(self, noise, what="rollout_mlp_noisy", n=None):
+        """Check rollout_mlp_noisy()'s or rollout_actor_critic()'s noise without a CUDA call -> T.  n: the batch it
+        is drawn for (rollout_from_mlp()'s B), the env's num_envs when not given."""
+        n = self.num_envs if n is None else n
         torch = _torch()
         K = int(self.single_action_space.n if self.discrete else self.act_dim)
         if not isinstance(noise, torch.Tensor):
@@ -1167,8 +1291,8 @@ class B200VectorEnv:
             raise ValueError(f"{what}() needs noise on {self.device}, got {noise.device}")
         if not noise.is_contiguous():
             raise ValueError(f"{what}() needs contiguous noise")
-        if noise.dim() != 3 or tuple(noise.shape[1:]) != (self.num_envs, K) or not 1 <= noise.shape[0] <= 2 ** 31 - 1:
-            raise ValueError(f"{what}() needs noise (T, {self.num_envs}, {K}) with 1 <= T < 2**31, got "
+        if noise.dim() != 3 or tuple(noise.shape[1:]) != (n, K) or not 1 <= noise.shape[0] <= 2 ** 31 - 1:
+            raise ValueError(f"{what}() needs noise (T, {n}, {K}) with 1 <= T < 2**31, got "
                              f"{tuple(noise.shape)}")
         return int(noise.shape[0])
 
@@ -1236,9 +1360,11 @@ class B200VectorEnv:
                              f"{tuple(bias.shape)}")
         return per_env
 
-    def _mlp_params(self, params, hidden, activation, what="rollout_mlp"):
+    def _mlp_params(self, params, hidden, activation, what="rollout_mlp", n=None):
         """Check rollout_mlp()'s or rollout_mlp_noisy()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden
-        layer), per_env, the b200gym_mlp_activation code)."""
+        layer), per_env, the b200gym_mlp_activation code).  n: the number of per-env rows (rollout_from_mlp()'s B),
+        the env's num_envs when not given."""
+        n = self.num_envs if n is None else n
         torch = _torch()
         if not isinstance(activation, str) or activation not in _lib.MLP_ACTIVATIONS:
             raise ValueError(f"{what}() needs activation 'relu' or 'tanh', got {activation!r}")
@@ -1258,10 +1384,10 @@ class B200VectorEnv:
             raise ValueError(f"{what}() needs params on {self.device}, got {params.device}")
         if not params.is_contiguous():
             raise ValueError(f"{what}() needs contiguous params")
-        per_env = tuple(params.shape) == (self.num_envs, P)
+        per_env = tuple(params.shape) == (n, P)
         if not (per_env or tuple(params.shape) == (P,)):
             raise ValueError(f"{what}() with hidden {tuple(widths)} needs params ({P},) for one policy or "
-                             f"({self.num_envs}, {P}) for one per env; got {tuple(params.shape)}")
+                             f"({n}, {P}) for one per env; got {tuple(params.shape)}")
         return widths[0], widths[1] if len(widths) == 2 else 0, per_env, _lib.MLP_ACTIVATIONS[activation]
 
     def _rollout_guards(self, what, reset_needed=True):

@@ -97,6 +97,13 @@ class VectorWrapper:
                           "fused rollout of the wrapped env would skip it; restore() the snapshot and call step() T "
                           "times instead")
 
+    def rollout_from_mlp(self, snap, params, hidden, T, **kwargs):
+        """Refused, as rollout_from()."""
+        from gym_b200 import error
+        raise error.Error(f"{type(self).__name__} does not support rollout_from_mlp(): it acts after every step, and a "
+                          "fused rollout of the wrapped env would skip it; restore() the snapshot and call step() T "
+                          "times instead")
+
     def close(self, **kwargs):
         return self.env.close(**kwargs)
 

@@ -500,6 +500,32 @@ int b200gym_rollout_from(b200gym_t *h, const void *snap_rows_dev, int64_t n_rows
                          uint8_t *ended_dev, void *end_rows_dev, float *end_obs_dev, void *stream);
 
 /*
+ * b200gym_rollout_from with each branch's actions taken by an MLP policy from its own observations: branch b is what a
+ * fresh handle of B envs computes after loading row row_idx_dev[b] (and, Box2D kinds, observation row row_idx_dev[b])
+ * into env b and running b200gym_rollout_mlp_norm (noise_dev NULL) or b200gym_rollout_mlp_noisy_norm with the same
+ * policy, noise and statistics, folded as b200gym_rollout_from folds.
+ *   snap_rows_dev, n_rows, row_idx_dev, B, T, returns_dev, lengths_dev, ended_dev, end_rows_dev, end_obs_dev
+ *                  b200gym_rollout_from's
+ *   snap_obs_dev   Box2D kinds: the snapshot's [n_rows][obs_dim] float32 observation rows, step 0's inputs; ignored
+ *                  (may be NULL) for the classic kinds, whose step 0 reads observe() of the row's state
+ *   params_dev, n_layers, h1, h2, activation   b200gym_rollout_mlp_act's; per_branch: [B][P], branch b's policy row b
+ *   noise_dev      NULL (the action from the outputs z), or [T][B][K] float32 (from z + noise[t][b], one rounded add)
+ *   obs_mean_dev, obs_var_dev, eps, clip_obs   b200gym_rollout_mlp_norm's (both NULL: raw inputs, clip_obs +inf);
+ *                  with noise_dev they need per_branch = 0, as b200gym_rollout_mlp_noisy_norm
+ *   first_actions_dev   [B] int64 (Discrete kinds) or [B][act_dim] float32 (Box kinds): the action of step 0; zero for
+ *                  a skipped branch
+ * Classic-control kinds: ONE launch, one thread per branch (rollout_from_mlp_kernel); may be captured in a CUDA graph,
+ * replays reading the current rows, indices, parameters, noise and statistics.  Box2D kinds: composed launch by
+ * launch in the scratch batch of b200gym_rollout_from; not capturable.
+ */
+int b200gym_rollout_from_mlp(b200gym_t *h, const void *snap_rows_dev, const float *snap_obs_dev, int64_t n_rows,
+                             const int64_t *row_idx_dev, int64_t B, const float *params_dev, int per_branch,
+                             int n_layers, int h1, int h2, int32_t T, const float *noise_dev, int activation,
+                             const double *obs_mean_dev, const double *obs_var_dev, double eps, float clip_obs,
+                             double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev, void *first_actions_dev,
+                             void *end_rows_dev, float *end_obs_dev, void *stream);
+
+/*
  * LunarLander only (state_dim is 0 for it; get/set_state handle the TimeLimit counters and RNG):
  * the three rigid bodies {lander, leg(-1), leg(+1)} of every env as float32 [n][18] =
  * 3 x {c.x, c.y, angle, v.x, v.y, omega} and int32 [n][6] = {game_over, leg0 contact, leg1 contact,
