@@ -34,6 +34,9 @@ ACT_I64, ACT_I32, ACT_U8, ACT_F32 = 0, 1, 2, 3
 # enum b200gym_mlp_activation, by the name rollout_mlp(activation=) takes
 MLP_ACTIVATIONS = {"relu": 0, "tanh": 1}
 
+# enum b200gym_mlp_head, by the name rollout_mlp(head=) takes
+MLP_HEADS = {"tanh": 1, "tanh_normal": 2}
+
 
 class Config(ctypes.Structure):
     """struct b200gym_config"""
@@ -147,6 +150,10 @@ SIGNATURES = {
                                        _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200gym_rollout_mlp_noisy_act": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                              _vp, _vp, _vp, _vp, _vp, _i32]),
+    "b200gym_rollout_mlp_head": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _vp, _vp, _vp, _vp, _vp, _i32, _i32]),
+    "b200gym_rollout_mlp_noisy_head": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _vp, _vp, _vp, _vp, _i32, _i32]),
     "b200gym_rollout_actor_critic": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32] + [_vp] * 10 +
                                      [ctypes.c_float, ctypes.c_float, _vp, _vp, _vp, _i32]),
     "b200gym_rollout_mlp_noisy_norm": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
@@ -203,6 +210,7 @@ SIGNATURES = {
     "b200gym_box2d_list_counts": (_i32, [_vp, _vp, _i32, _vp, _vp]),
     "b200gym_selftest_trig": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "b200gym_selftest_tanh": (_i32, [_vp, _i64, _vp, _vp]),
+    "b200gym_selftest_exp": (_i32, [_vp, _i64, _vp, _vp]),
     "b200gym_selftest_box2d": (_i32, [_i32, _vp, _i64, _vp, _vp]),
     "b200gym_selftest": (_i32, [_i32, _i64, ctypes.c_uint64, ctypes.POINTER(_i64)]),
 }

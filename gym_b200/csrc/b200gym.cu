@@ -476,6 +476,97 @@ __global__ void __launch_bounds__(kThreads) mlp_noisy_policy_kernel(const float 
     }
 }
 
+// ... with the actions taken from each env's MLP policy through head HEAD, a b200gym_mlp_head (rollout_mlp_head_env);
+// SUMMARY, PER_ENV, ACT and the launch bounds as rollout_mlp_kernel.  Classic Box kinds only
+template <int KIND, bool SUMMARY, bool PER_ENV, int ACT, int HEAD>
+__global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2)
+    rollout_mlp_head_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpHeadArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (PER_ENV) {
+        if (i < a.n)
+            rollout_mlp_head_env<KIND, SUMMARY, true, ACT, HEAD>(a, i, T, last_obs, p.mlp.params + i * p.mlp.stride, p);
+    } else {
+        using Src = MlpHeadActions<KIND, SUMMARY, false, ACT, HEAD>;
+        const float *w = mlp_stage(p.mlp.params, mlp_param_count<Src::K, Src::D>(p.mlp.h1, p.mlp.h2));
+        if (i < a.n) rollout_mlp_head_env<KIND, SUMMARY, false, ACT, HEAD>(a, i, T, last_obs, w, p);
+    }
+}
+
+// ... with the caller's noise going into head HEAD (rollout_mlp_noisy_head_env); PER_ENV, ACT and the launch bounds as
+// rollout_mlp_kernel.  Classic Box kinds only
+template <int KIND, bool PER_ENV, int ACT, int HEAD>
+__global__ void __launch_bounds__(kThreads, PER_ENV ? 1 : 2)
+    rollout_mlp_noisy_head_kernel(const StepArgs a, const int32_t T, float *last_obs, const MlpHeadArgs p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (PER_ENV) {
+        if (i < a.n)
+            rollout_mlp_noisy_head_env<KIND, true, ACT, HEAD>(a, i, T, last_obs, p.mlp.params + i * p.mlp.stride, p);
+    } else {
+        using Src = MlpNoisyHeadActions<KIND, false, ACT, HEAD>;
+        const float *w = mlp_stage(p.mlp.params, mlp_param_count<Src::K, Src::D>(p.mlp.h1, p.mlp.h2));
+        if (i < a.n) rollout_mlp_noisy_head_env<KIND, false, ACT, HEAD>(a, i, T, last_obs, w, p);
+    }
+}
+
+// One step's actions of a Box2D MLP-policy rollout through head HEAD: mlp_policy_kernel for a Box kind with the K
+// outputs going through the deterministic head (head_action) into the A actions
+template <int K, int D, bool PER_ENV, int ACT, int HEAD>
+__global__ void __launch_bounds__(kThreads) mlp_head_policy_kernel(const float *obs, void *actions, const MlpHeadArgs p,
+                                                                   const double *reward, const uint8_t *term,
+                                                                   const uint8_t *trunc, int64_t n, int32_t t_prev,
+                                                                   int act, int init) {
+    constexpr int A = HEAD == B200GYM_HEAD_TANH_NORMAL ? K / 2 : K;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float *w = nullptr;
+    if (act)
+        w = PER_ENV ? p.mlp.params + i * p.mlp.stride
+                    : mlp_stage(p.mlp.params, mlp_param_count<K, D>(p.mlp.h1, p.mlp.h2));
+    if (i >= n) return;
+    if (init) {
+        p.mlp.returns[i] = 0.0;
+        p.mlp.lengths[i] = 0;
+        p.mlp.ended[i] = 0;
+    } else if (t_prev >= 0 && !p.mlp.ended[i]) {   // step t_prev is the first episode end or before it
+        p.mlp.returns[i] = p.mlp.returns[i] + reward[i];
+        p.mlp.lengths[i] = t_prev + 1;
+        p.mlp.ended[i] = (term[i] | trunc[i]) != 0;
+    }
+    if (!act) return;
+    float o[D], z[K], e[A] = {}, y[A];
+#pragma unroll
+    for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
+    mlp_outputs<K, D, PER_ENV, ACT>(w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, z);
+    head_action<HEAD, false>(z, e, p.bounds, y);
+#pragma unroll
+    for (int j = 0; j < A; j++) static_cast<float *>(actions)[i * A + j] = y[j];
+}
+
+// One step's actions of a Box2D noisy MLP-policy rollout through head HEAD: mlp_head_policy_kernel with the step's
+// noise slice going into the head and the outputs to the step's outputs slice (the launch passes p.noise and p.outputs
+// at that step's slice).  No summary mode: reward, term, trunc, t_prev, act and init are the launcher's and unused here
+template <int K, int D, bool PER_ENV, int ACT, int HEAD>
+__global__ void __launch_bounds__(kThreads) mlp_noisy_head_policy_kernel(const float *obs, void *actions,
+                                                                         const MlpHeadArgs p, const double *,
+                                                                         const uint8_t *, const uint8_t *, int64_t n,
+                                                                         int32_t, int, int) {
+    constexpr int A = HEAD == B200GYM_HEAD_TANH_NORMAL ? K / 2 : K;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float *w = PER_ENV ? p.mlp.params + i * p.mlp.stride
+                             : mlp_stage(p.mlp.params, mlp_param_count<K, D>(p.mlp.h1, p.mlp.h2));
+    if (i >= n) return;
+    float o[D], z[K], e[A], y[A];
+#pragma unroll
+    for (int k = 0; k < D; k++) o[k] = obs[i * D + k];
+    mlp_outputs<K, D, PER_ENV, ACT>(w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, o, z);
+#pragma unroll
+    for (int k = 0; k < A; k++) e[k] = load_once(p.noise + i * A + k);
+#pragma unroll
+    for (int k = 0; k < K; k++) store_once(p.outputs + i * K + k, z[k]);
+    head_action<HEAD, true>(z, e, p.bounds, y);
+#pragma unroll
+    for (int j = 0; j < A; j++) static_cast<float *>(actions)[i * A + j] = y[j];
+}
+
 // The CTA's shared copies of two nets, mlp_stage's for each: the `na` floats at a, then, from the next 16-byte boundary,
 // the `nc` floats at c.  Returns the copy of c; the copy of a is at the start of the dynamic shared memory
 __device__ __forceinline__ const float *mlp_stage_pair(const float *a, int64_t na, const float *c, int64_t nc) {
@@ -1726,6 +1817,14 @@ __global__ void __launch_bounds__(kThreads) selftest_tanh_kernel(const float *x,
     y[i] = mlp_tanh(x[i]);
 }
 
+// device self-test: the exp of the SAC head (head_exp) evaluated on caller-supplied arguments (the caller compares
+// with torch.exp on the same device)
+__global__ void __launch_bounds__(kThreads) selftest_exp_kernel(const float *x, int64_t n, float *y) {
+    const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    y[i] = head_exp(x[i]);
+}
+
 static inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 // ---------------------------------------------------------------------------
@@ -2376,6 +2475,16 @@ extern "C" int b200gym_selftest_tanh(const float *x_dev, int64_t n, float *y_dev
     if (dev < 0) return fail(nullptr, "b200gym_selftest_tanh: x is not a device pointer");
     DeviceGuard guard(dev);
     selftest_tanh_kernel<<<blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, n, y_dev);
+    CK(nullptr, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int b200gym_selftest_exp(const float *x_dev, int64_t n, float *y_dev, void *stream) {
+    if (!x_dev || !y_dev || n <= 0) return fail(nullptr, "b200gym_selftest_exp: bad argument");
+    const int dev = device_of(x_dev);
+    if (dev < 0) return fail(nullptr, "b200gym_selftest_exp: x is not a device pointer");
+    DeviceGuard guard(dev);
+    selftest_exp_kernel<<<blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, n, y_dev);
     CK(nullptr, cudaGetLastError());
     return 0;
 }
@@ -3149,6 +3258,163 @@ extern "C" int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_d
     if (activation == B200GYM_MLP_TANH)
         return launch_rollout_mlp_noisy<B200GYM_MLP_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
     return launch_rollout_mlp_noisy<B200GYM_MLP_RELU>(h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, st);
+}
+
+// ---- squashed-head MLP rollouts (b200gym_rollout_mlp_head, b200gym_rollout_mlp_noisy_head) ----
+// noisy: the noisy kernels (p.noise and p.outputs set), else the deterministic ones, summary mode included
+template <int KIND, int ACT, int HEAD>
+static int launch_rollout_mlp_head_kind(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                        const MlpHeadArgs &p, bool per_env, size_t smem, bool summary, bool noisy,
+                                        cudaStream_t st) {
+    const unsigned blocks = blocks_for(h->n);
+    if (noisy) {
+        if (per_env)
+            rollout_mlp_noisy_head_kernel<KIND, true, ACT, HEAD><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+        else rollout_mlp_noisy_head_kernel<KIND, false, ACT, HEAD><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+    } else if (per_env) {
+        if (summary)
+            rollout_mlp_head_kernel<KIND, true, true, ACT, HEAD><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+        else rollout_mlp_head_kernel<KIND, false, true, ACT, HEAD><<<blocks, kThreads, 0, st>>>(a, T, last_obs, p);
+    } else {
+        if (summary)
+            rollout_mlp_head_kernel<KIND, true, false, ACT, HEAD><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+        else rollout_mlp_head_kernel<KIND, false, false, ACT, HEAD><<<blocks, kThreads, smem, st>>>(a, T, last_obs, p);
+    }
+    CK(h, cudaGetLastError());
+    return 0;
+}
+
+// The policy launch of step t of a noisy rollout reads noise slice t and writes outputs slice t
+template <int K, int D, int ACT, int HEAD>
+static int launch_rollout_mlp_head_box2d(b200gym *h, const StepArgs &a, int32_t T, float *last_obs,
+                                         const float *first_obs, const MlpHeadArgs &p, bool per_env, size_t smem,
+                                         bool summary, bool noisy, cudaStream_t st) {
+    constexpr int A = HEAD == B200GYM_HEAD_TANH_NORMAL ? K / 2 : K;
+    if (noisy) {
+        const int64_t n = h->n;
+        return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs,
+                                           [&](int32_t t) {
+                                               MlpHeadArgs q = p;
+                                               q.noise = p.noise + t * n * A;
+                                               q.outputs = p.outputs + t * n * K;
+                                               return q;
+                                           },
+                                           per_env ? mlp_noisy_head_policy_kernel<K, D, true, ACT, HEAD>
+                                                   : mlp_noisy_head_policy_kernel<K, D, false, ACT, HEAD>,
+                                           per_env ? 0 : smem, false, st, "mlp_noisy_head_policy_kernel",
+                                           "b200gym_rollout_mlp_noisy_head");
+    }
+    return launch_rollout_policy_box2d(h, a, T, last_obs, first_obs, [&](int32_t) { return p; },
+                                       per_env ? mlp_head_policy_kernel<K, D, true, ACT, HEAD>
+                                               : mlp_head_policy_kernel<K, D, false, ACT, HEAD>,
+                                       per_env ? 0 : smem, summary, st, "mlp_head_policy_kernel",
+                                       "b200gym_rollout_mlp_head");
+}
+
+template <int ACT, int HEAD>
+static int launch_rollout_mlp_head(b200gym *h, const StepArgs &a, int32_t T, float *last_obs, const float *first_obs,
+                                   const MlpHeadArgs &p, bool pe, size_t smem, bool summary, bool noisy,
+                                   cudaStream_t st) {
+    switch (h->cfg.kind) {
+    case B200GYM_MOUNTAINCAR_CONT:
+        return launch_rollout_mlp_head_kind<B200GYM_MOUNTAINCAR_CONT, ACT, HEAD>(h, a, T, last_obs, p, pe, smem,
+                                                                                 summary, noisy, st);
+    case B200GYM_PENDULUM:
+        return launch_rollout_mlp_head_kind<B200GYM_PENDULUM, ACT, HEAD>(h, a, T, last_obs, p, pe, smem, summary,
+                                                                         noisy, st);
+    case B200GYM_LUNARLANDER_CONT:
+        return launch_rollout_mlp_head_box2d<head_outputs<HEAD>(2), 8, ACT, HEAD>(h, a, T, last_obs, first_obs, p, pe,
+                                                                                  smem, summary, noisy, st);
+    case B200GYM_BIPEDALWALKER:
+    case B200GYM_BIPEDALWALKER_HARDCORE:
+        return launch_rollout_mlp_head_box2d<head_outputs<HEAD>(4), 24, ACT, HEAD>(h, a, T, last_obs, first_obs, p,
+                                                                                   pe, smem, summary, noisy, st);
+    }
+    return fail(h, "bad kind %d", h->cfg.kind);
+}
+
+// The checks and launches of both entry points: noisy (b200gym_rollout_mlp_noisy_head) reads noise_dev and writes
+// outputs_dev, and has no summary mode; `what` names the entry point in the messages
+static int rollout_mlp_head(const char *what, b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                            int h2, int32_t T, bool noisy, const float *noise_dev, float *outputs_dev,
+                            void *actions_out_dev, float *obs_dev, double *reward_dev, uint8_t *terminated_dev,
+                            uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev, int32_t *lengths_dev,
+                            uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                            int activation, int head) {
+    if (!h) return fail(h, "%s: null handle", what);
+    if (head != B200GYM_HEAD_TANH && head != B200GYM_HEAD_TANH_NORMAL)
+        return fail(h, "%s: head must be B200GYM_HEAD_TANH or B200GYM_HEAD_TANH_NORMAL (got %d)", what, head);
+    if (activation != B200GYM_MLP_RELU && activation != B200GYM_MLP_TANH)
+        return fail(h, "%s: activation must be B200GYM_MLP_RELU or B200GYM_MLP_TANH (got %d)", what, activation);
+    const int kind = h->cfg.kind;
+    if (kind != B200GYM_MOUNTAINCAR_CONT && kind != B200GYM_PENDULUM && kind != B200GYM_LUNARLANDER_CONT &&
+        kind != B200GYM_BIPEDALWALKER && kind != B200GYM_BIPEDALWALKER_HARDCORE)
+        return fail(h, "%s: a head needs a Box action space (kind %d is Discrete)", what, kind);
+    if (n_layers != 1 && n_layers != 2) return fail(h, "%s: n_layers must be 1 or 2 (got %d)", what, n_layers);
+    if (h1 < 1 || h1 > kMlpMaxWidth || (n_layers == 2 && (h2 < 1 || h2 > kMlpMaxWidth)))
+        return fail(h, "%s: hidden widths must be 1 .. %d (got %d, %d)", what, kMlpMaxWidth, h1, h2);
+    if (T < 1) return fail(h, "%s: T must be at least 1 (got %d)", what, T);
+    if (!params_dev || !last_obs_dev || (noisy && (!noise_dev || !outputs_dev)))
+        return fail(h, "%s: null buffer", what);
+    const bool summary = returns_dev != nullptr;
+    if (summary ? (noisy || !lengths_dev || !ended_dev || actions_out_dev || obs_dev || reward_dev || terminated_dev ||
+                   truncated_dev || final_obs_dev)
+                : (!actions_out_dev || !obs_dev || !reward_dev || !terminated_dev || !truncated_dev || lengths_dev ||
+                   ended_dev))
+        return fail(h, "%s: give %s", what,
+                    noisy ? "the per-step outputs" : "either the per-step outputs or returns, lengths and ended");
+    if ((h->is_lunar || h->is_walker) && !first_obs_dev) return fail(h, "%s: a Box2D env needs first_obs_dev", what);
+    if (n_layers == 1) h2 = 0;
+    const int64_t K = head == B200GYM_HEAD_TANH_NORMAL ? 2 * h->A : h->A, D = h->D;
+    const int64_t P = h2 == 0 ? h1 * D + h1 + K * h1 + K : h1 * D + h1 + (int64_t)h2 * h1 + h2 + K * h2 + K;
+    // as b200gym_rollout_mlp
+    const bool vec = h1 % 4 == 0 && (!per_env || (P % 4 == 0 && reinterpret_cast<uintptr_t>(params_dev) % 16 == 0));
+    // the kind's action bounds, and CleanRL's action_scale and action_bias from them, in float32
+    const float high = kind == B200GYM_PENDULUM ? 2.0f : 1.0f, low = -high;
+    const HeadBounds bounds{low, high, (high - low) / 2.0f, (high + low) / 2.0f};
+    const MlpHeadArgs p{{params_dev, per_env ? P : 0, h1, h2, vec ? 1 : 0, returns_dev, lengths_dev, ended_dev},
+                        noise_dev, outputs_dev, bounds};
+    const size_t smem = (size_t)(P + 3) / 4 * 16;   // at most 24.5 KB (BipedalWalker's SAC actor at (64, 64))
+    DeviceGuard guard(h->device);
+    const StepArgs a = make_args(h, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev, final_obs_dev);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool pe = per_env != 0;
+    if (activation == B200GYM_MLP_TANH) {
+        if (head == B200GYM_HEAD_TANH_NORMAL)
+            return launch_rollout_mlp_head<B200GYM_MLP_TANH, B200GYM_HEAD_TANH_NORMAL>(
+                h, a, T, last_obs_dev, first_obs_dev, p, pe, smem, summary, noisy, st);
+        return launch_rollout_mlp_head<B200GYM_MLP_TANH, B200GYM_HEAD_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe,
+                                                                            smem, summary, noisy, st);
+    }
+    if (head == B200GYM_HEAD_TANH_NORMAL)
+        return launch_rollout_mlp_head<B200GYM_MLP_RELU, B200GYM_HEAD_TANH_NORMAL>(h, a, T, last_obs_dev, first_obs_dev,
+                                                                                   p, pe, smem, summary, noisy, st);
+    return launch_rollout_mlp_head<B200GYM_MLP_RELU, B200GYM_HEAD_TANH>(h, a, T, last_obs_dev, first_obs_dev, p, pe,
+                                                                        smem, summary, noisy, st);
+}
+
+extern "C" int b200gym_rollout_mlp_head(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                        int h2, int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                        uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                        double *returns_dev, int32_t *lengths_dev, uint8_t *ended_dev,
+                                        float *last_obs_dev, const float *first_obs_dev, void *stream, int activation,
+                                        int head) {
+    return rollout_mlp_head("b200gym_rollout_mlp_head", h, params_dev, per_env, n_layers, h1, h2, T, false, nullptr,
+                            nullptr, actions_out_dev, obs_dev, reward_dev, terminated_dev, truncated_dev,
+                            final_obs_dev, returns_dev, lengths_dev, ended_dev, last_obs_dev, first_obs_dev, stream,
+                            activation, head);
+}
+
+extern "C" int b200gym_rollout_mlp_noisy_head(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1,
+                                              int h2, int32_t T, const float *noise_dev, float *outputs_dev,
+                                              void *actions_out_dev, float *obs_dev, double *reward_dev,
+                                              uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev,
+                                              float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                              int activation, int head) {
+    return rollout_mlp_head("b200gym_rollout_mlp_noisy_head", h, params_dev, per_env, n_layers, h1, h2, T, true,
+                            noise_dev, outputs_dev, actions_out_dev, obs_dev, reward_dev, terminated_dev,
+                            truncated_dev, final_obs_dev, nullptr, nullptr, nullptr, last_obs_dev, first_obs_dev,
+                            stream, activation, head);
 }
 
 // ---- on-policy collection with a critic (b200gym_rollout_actor_critic) ----

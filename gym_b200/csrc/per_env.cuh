@@ -830,6 +830,191 @@ __device__ __forceinline__ void rollout_mlp_noisy_env(const StepArgs &a, int64_t
     a.elapsed[i] = elapsed;
 }
 
+// ---- squashed-head MLP rollouts (b200gym_rollout_mlp_head, b200gym_rollout_mlp_noisy_head) -------------------------
+
+// The exp of the SAC head's standard deviation: CUDA's expf on the device, which compiles to the same instructions with
+// and without -fmad (DESIGN.md §4.21), and the C library's expf in the host build.  b200gym_selftest_exp evaluates it
+__host__ __device__ __forceinline__ float head_exp(float x) { return expf(x); }
+
+// The number of network outputs of head HEAD (b200gym_mlp_head) for a Box action of A dimensions
+template <int HEAD>
+__host__ __device__ constexpr int head_outputs(int A) {
+    static_assert(HEAD == B200GYM_HEAD_TANH || HEAD == B200GYM_HEAD_TANH_NORMAL, "unknown MLP head");
+    return HEAD == B200GYM_HEAD_TANH_NORMAL ? 2 * A : A;
+}
+
+// The kind's action bounds and CleanRL's action_scale and action_bias from them (b200gym_mlp_head), the same for every
+// action dimension of the kinds a head runs on
+struct HeadBounds {
+    float low, high, scale, bias;
+};
+
+// v clamped to [lo, hi] with a NaN staying NaN, as torch.clamp and np.clip do (fminf / fmaxf would drop it)
+__host__ __device__ __forceinline__ float head_clamp(float v, float lo, float hi) {
+    return v < lo ? lo : (v > hi ? hi : v);
+}
+
+// The A actions of head HEAD from the K network outputs z: deterministic (NOISY false; e is not read), or with the
+// step's noise e.  Every product and sum is one rounded float32 operation, in the order b200gym_mlp_head gives
+template <int HEAD, bool NOISY, int K, int A>
+__host__ __device__ __forceinline__ void head_action(const float (&z)[K], const float (&e)[A], const HeadBounds &b,
+                                                     float (&act)[A]) {
+    static_assert(K == head_outputs<HEAD>(A), "K must be the head's output count");
+#pragma unroll
+    for (int k = 0; k < A; k++) {
+        if constexpr (HEAD == B200GYM_HEAD_TANH_NORMAL && NOISY) {
+            const float ls = -5.0f + 3.5f * (mlp_tanh(z[A + k]) + 1.0f);
+            const float x = z[k] + e[k] * head_exp(ls);
+            act[k] = mlp_tanh(x) * b.scale + b.bias;
+        } else {
+            const float v = mlp_tanh(z[k]) * b.scale + b.bias;
+            if constexpr (NOISY) act[k] = head_clamp(v + e[k], b.low, b.high);
+            else act[k] = v;
+        }
+    }
+}
+
+// The arguments of a b200gym_rollout_mlp_head / b200gym_rollout_mlp_noisy_head launch: the policy (mlp), for the noisy
+// one slice 0 of the [T][n][A] noise it reads and of the [T][n][K] outputs it writes (null otherwise), and the bounds
+struct MlpHeadArgs {
+    MlpPolicyArgs mlp;
+    const float *noise;
+    float *outputs;
+    HeadBounds bounds;
+};
+
+// MlpHeadActions: MlpActions for a Box kind, with the action taken from the K = head_outputs<HEAD>(A) outputs through
+// the deterministic head
+template <int KIND, bool SUMMARY, bool GLOBAL, int ACT, int HEAD>
+struct MlpHeadActions {
+    static constexpr int A = bgym::Env<KIND>::A, K = head_outputs<HEAD>(A), D = bgym::Env<KIND>::D;
+    static_assert(A == 1, "the classic Box kinds take one action");
+    const float *w;
+    int h1, h2;
+    bool vec;
+    HeadBounds b;
+    const float (&o)[D];
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
+        float z[K], e[A] = {}, y[A];
+        mlp_outputs<K, D, GLOBAL, ACT>(w, h1, h2, vec, o, z);
+        head_action<HEAD, false>(z, e, b, y);
+        const ActT v = y[0];
+        if constexpr (!SUMMARY) store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+};
+
+// MlpNoisyHeadActions: MlpHeadActions with the step's noise (A per env) going into the head.  The outputs z go to
+// `outputs` and the action to the row of actions, both written once; noise and outputs point at row t of their
+// [T][n][A] and [T][n][K] arrays and move on by one row per step (next)
+template <int KIND, bool GLOBAL, int ACT, int HEAD>
+struct MlpNoisyHeadActions {
+    static constexpr int A = bgym::Env<KIND>::A, K = head_outputs<HEAD>(A), D = bgym::Env<KIND>::D;
+    static_assert(A == 1, "the classic Box kinds take one action");
+    const float *w;
+    int h1, h2;
+    bool vec;
+    HeadBounds b;
+    const float (&o)[D];
+    const float *noise;
+    float *outputs;
+    template <typename ActT>
+    __device__ __forceinline__ ActT action(const ActT *row, int64_t i) const {
+        float z[K], e[A], y[A];
+        mlp_outputs<K, D, GLOBAL, ACT>(w, h1, h2, vec, o, z);
+#pragma unroll
+        for (int k = 0; k < A; k++) e[k] = load_once(noise + i * A + k);
+#pragma unroll
+        for (int k = 0; k < K; k++) store_once(outputs + i * K + k, z[k]);
+        head_action<HEAD, true>(z, e, b, y);
+        const ActT v = y[0];
+        store_once(const_cast<ActT *>(row) + i, v);
+        return v;
+    }
+    __device__ __forceinline__ void next(int64_t n) {
+        noise += n * A;
+        outputs += n * K;
+    }
+};
+
+// T steps of env i under its MLP policy at w through head HEAD (rollout_mlp_head_kernel): rollout_mlp_env's loop,
+// written out again so that no pre-existing kernel changes, with MlpHeadActions in place of MlpActions; SUMMARY,
+// GLOBAL and ACT as rollout_mlp_env
+template <int KIND, bool SUMMARY, bool GLOBAL, int ACT, int HEAD>
+__device__ __forceinline__ void rollout_mlp_head_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                     const float *w, const MlpHeadArgs &p) {
+    using E = bgym::Env<KIND>;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D];
+    E::observe(s, o);
+    const MlpHeadActions<KIND, SUMMARY, GLOBAL, ACT, HEAD> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, p.bounds, o};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, SUMMARY> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                   o, ret, len, ended};
+    const float *act = reinterpret_cast<const float *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+    if constexpr (SUMMARY) {
+        p.mlp.returns[i] = ret;
+        p.mlp.lengths[i] = len;
+        p.mlp.ended[i] = ended ? 1 : 0;
+    }
+}
+
+// T steps of env i under its MLP policy at w with the caller's noise through head HEAD
+// (rollout_mlp_noisy_head_kernel): rollout_mlp_noisy_env's loop, written out again so that no pre-existing kernel
+// changes, with MlpNoisyHeadActions in place of MlpNoisyActions; GLOBAL and ACT as rollout_mlp_env
+template <int KIND, bool GLOBAL, int ACT, int HEAD>
+__device__ __forceinline__ void rollout_mlp_noisy_head_env(const StepArgs &a, int64_t i, int32_t T, float *last_obs,
+                                                           const float *w, const MlpHeadArgs &p) {
+    using E = bgym::Env<KIND>;
+    const int64_t n = a.n;
+    double s[E::S];
+#pragma unroll
+    for (int k = 0; k < E::S; k++) s[k] = a.state[k * n + i];
+    int32_t elapsed = a.elapsed[i];
+    float o[E::D];
+    E::observe(s, o);
+    MlpNoisyHeadActions<KIND, GLOBAL, ACT, HEAD> src{w, p.mlp.h1, p.mlp.h2, p.mlp.vec != 0, p.bounds, o, p.noise,
+                                                     p.outputs};
+    double ret = 0.0;
+    int32_t len = 0;
+    bool ended = false;
+    LinearSink<KIND, false> sink{{s, elapsed, a.obs, a.reward, a.terminated, a.truncated, a.final_obs, nullptr},
+                                 o, ret, len, ended};
+    const float *act = reinterpret_cast<const float *>(a.actions);
+    for (int32_t t = 0; t < T; t++) {
+        if (t == T - 1) sink.last = last_obs;
+        long long action_int = 0;
+        float a0 = 0.0f;
+        decode_action<KIND>(src.action(act, i), action_int, a0);
+        if (advance_env<KIND>(a, sink, i, s, elapsed, action_int, a0)) reset_env<KIND>(a, sink, i);
+        act += n;
+        src.next(n);
+        sink.next(n);
+    }
+#pragma unroll
+    for (int k = 0; k < E::S; k++) a.state[k * n + i] = s[k];
+    a.elapsed[i] = elapsed;
+}
+
 // ---- on-policy collection with a critic (b200gym_rollout_actor_critic) --------------------------------------------
 
 // The arguments of a b200gym_rollout_actor_critic launch: the actor and its noise and outputs (one actor shared by every

@@ -716,8 +716,8 @@ class B200VectorEnv:
                                                   int(per_env), T, *outs, vp(last.data_ptr()), vp(first.data_ptr()),
                                                   self._stream(), *norm, s, q)), moments)
 
-    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu", obs_norm=None, norm_epsilon=1e-8,
-                    clip_obs=None, obs_moments=False):
+    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu", head=None, obs_norm=None,
+                    norm_epsilon=1e-8, clip_obs=None, obs_moments=False):
         """T steps of an MLP policy in closed loop: ``rollout_linear()`` with the policy
         D -> hidden[0] (-> hidden[1]) -> K, the activation after every hidden layer and nothing after the last.
 
@@ -748,12 +748,34 @@ class B200VectorEnv:
             score = ret[ended].mean()                  # the mean first-episode return of the episodes that ended
 
         For Box kinds the action is the actor's mean output, unclipped, as ``rollout_linear()`` takes it (DESIGN.md
-        §4.19)."""
+        §4.19).
+
+        ``head`` (keyword only, Box kinds) is ``None`` (the default: the outputs are the action, as above),
+        ``"tanh"`` or ``"tanh_normal"``: the tanh-squashed actors of TD3 / DDPG and SAC.  With A = ``act_dim`` and the
+        action space's bounds, ``scale = float32(float32(high - low) / 2)`` and
+        ``bias = float32(float32(high + low) / 2)`` (2 and 0 for Pendulum, 1 and 0 for the other Box kinds), every
+        product and sum one rounded float32 operation, ``tanh`` as ``activation="tanh"`` and ``exp`` CUDA's ``expf``
+        (on the device the bits of ``torch.exp``, checked for every float32 input against the torch build of the
+        tests, DESIGN.md §4.21):
+
+        * ``"tanh"``: K = A outputs z and ``a = tanh(z) * scale + bias``, the action of CleanRL's TD3 / DDPG ``Actor``;
+        * ``"tanh_normal"``: K = 2A outputs, the mean ``m = z[:A]`` and the raw log-std ``z[A:]``, and
+          ``a = tanh(m) * scale + bias``, the deterministic action (``mean``) of CleanRL's SAC ``Actor.get_action``.
+
+        P counts K outputs; ``rollout_mlp_noisy()`` shows the packing of both actors.  The hidden widths stay 1 .. 64:
+        CleanRL's defaults are 256 wide, so those actors must be trained at widths <= 64 to run here.  ``head`` is
+        refused with ``obs_norm``, ``clip_obs`` or ``obs_moments`` and on Discrete kinds, before any CUDA call."""
         what = "rollout_mlp"
         captured = self._rollout_guards(what)
-        h1, h2, per_env, act = self._mlp_params(params, hidden, activation)
+        code = self._mlp_head(what, head, obs_norm, clip_obs, obs_moments)
+        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, head=head)
         norm, moments = self._policy_norm_args(what, summary, obs_norm, norm_epsilon, clip_obs, obs_moments)
         vp = ctypes.c_void_p
+        if code is not None:
+            return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first: (
+                self._lib.b200gym_rollout_mlp_head(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1,
+                                                   h2, T, *outs, vp(last.data_ptr()), vp(first.data_ptr()),
+                                                   self._stream(), act, code)))
         if norm is None:
             return self._policy_rollout(what, T, summary, captured, lambda T, outs, last, first: (
                 self._lib.b200gym_rollout_mlp_act(self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1,
@@ -764,8 +786,8 @@ class B200VectorEnv:
                                                T, *outs, vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act,
                                                *norm, s, q)), moments)
 
-    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu", obs_norm=None, norm_epsilon=1e-8,
-                          clip_obs=None):
+    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu", head=None, obs_norm=None,
+                          norm_epsilon=1e-8, clip_obs=None):
         """T steps of a stochastic MLP policy in closed loop, T = ``noise.shape[0]`` -> ``(actions, outputs, obs,
         rewards, terminateds, truncateds, infos)``: bit for bit what
         ``for t in range(T): z = mlp(obs); a = rule(z + noise[t]); obs, r, te, tr, info = self.step(a)`` returns,
@@ -819,15 +841,61 @@ class B200VectorEnv:
         never updates them) and need one shared policy: per-env ``params`` rows with ``obs_norm`` raise ``ValueError``,
         as does ``clip_obs`` without ``obs_norm``.  A captured graph reads the current contents of ``mean`` and
         ``var``; ``norm_epsilon`` and ``clip_obs`` are fixed at capture.  With the three keywords at their defaults the
-        call is the one above, unchanged (DESIGN.md §4.18)."""
+        call is the one above, unchanged (DESIGN.md §4.18).
+
+        ``head`` (keyword only, Box kinds) is ``rollout_mlp()``'s, with the noise going into the head: ``noise`` is
+        float32 (T, N, A) and ``outputs`` float32 (T, N, K), z before the head.  In the arithmetic of ``rollout_mlp()``:
+
+        * ``"tanh"``: ``a = clamp((tanh(z) * scale + bias) + noise[t], low, high)``, where a NaN stays NaN as in
+          ``torch.clamp``: CleanRL's TD3 / DDPG ``actor(obs) + noise`` and ``.clip(low, high)``;
+        * ``"tanh_normal"``: with ``m = z[..., :A]``, ``s = z[..., A:]`` and ``eps = noise[t]``,
+          ``ls = -5 + 3.5 * (tanh(s) + 1)``, ``x = m + eps * exp(ls)`` and ``a = tanh(x) * scale + bias``, unclipped:
+          CleanRL's SAC ``Actor.get_action`` (``LOG_STD_MIN = -5``, ``LOG_STD_MAX = 2``;
+          ``Normal(m, exp(ls)).rsample()`` is ``m + eps * exp(ls)``).  Its log-probabilities are recomputed from the
+          observations at update time.
+
+        A TD3 collection step of CleanRL's ``Actor`` (``fc1``, ``fc2``, ``fc_mu`` with ReLU; ``action_scale`` and
+        ``action_bias`` are buffers, so ``parameters()`` is the packing), trained at (64, 64), filling a replay buffer
+        with CleanRL's ``real_next_obs`` (the final observation where an episode ended)::
+
+            params = torch.nn.utils.parameters_to_vector(actor.parameters()).detach()
+            noise = torch.randn(T, N, A, device=dev) * (actor.action_scale * 0.1)        # exploration_noise = 0.1
+            a, z, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), noise, head="tanh")
+            prev = torch.cat([obs0[None], obs[:-1]])       # obs0: what the env returned before the call
+            done = info["_final_observation"]
+            real_next = torch.where(done[..., None], info["final_observation"], obs)
+            rb.add(prev.flatten(0, 1), real_next.flatten(0, 1), a.flatten(0, 1), r.flatten(), te.flatten())
+            obs0 = obs[-1]
+
+        and a SAC collection step of CleanRL's two-head ``Actor``, packed as one (2A, 64) output layer::
+
+            params = torch.cat([p.reshape(-1) for p in (actor.fc1.weight, actor.fc1.bias, actor.fc2.weight,
+                                actor.fc2.bias, actor.fc_mean.weight, actor.fc_logstd.weight, actor.fc_mean.bias,
+                                actor.fc_logstd.bias)]).detach()
+            a, z, obs, r, te, tr, info = envs.rollout_mlp_noisy(params, (64, 64), torch.randn(T, N, A, device=dev),
+                                                                head="tanh_normal")
+
+        with the same replay-buffer tuples.  The hidden widths stay 1 .. 64, so CleanRL's 256-wide defaults must be
+        trained at <= 64.  Capture and the refusals are as without a head; ``head`` is also refused with ``obs_norm``
+        or ``clip_obs`` and on Discrete kinds, before any CUDA call (DESIGN.md §4.21)."""
         what = "rollout_mlp_noisy"
         captured = self._rollout_guards(what)
-        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, what)
+        code = self._mlp_head(what, head, obs_norm, clip_obs)
+        h1, h2, per_env, act = self._mlp_params(params, hidden, activation, what, head=head)
         T = self._noise_steps(noise)
         norm = self._norm_args(what, obs_norm, norm_epsilon, clip_obs, per_env=per_env)
         self._refuse_box2d_capture(what)
-        outputs = _torch().empty_like(noise)
         vp = ctypes.c_void_p
+        if code is not None:
+            outputs = _torch().empty((T, self.num_envs, self._head_outputs(head)), dtype=noise.dtype,
+                                     device=self.device)
+            actions, obs, reward, term, trunc, infos = self._policy_rollout(
+                what, T, False, captured, lambda T, outs, last, first: self._lib.b200gym_rollout_mlp_noisy_head(
+                    self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T, vp(noise.data_ptr()),
+                    vp(outputs.data_ptr()), *outs[:6], vp(last.data_ptr()), vp(first.data_ptr()), self._stream(), act,
+                    code))
+            return actions, outputs, obs, reward, term, trunc, infos
+        outputs = _torch().empty_like(noise)
         if norm is None:
             launch = lambda T, outs, last, first: self._lib.b200gym_rollout_mlp_noisy_act(  # noqa: E731
                 self._handle, vp(params.data_ptr()), int(per_env), len(hidden), h1, h2, T, vp(noise.data_ptr()),
@@ -1279,7 +1347,8 @@ class B200VectorEnv:
 
     def _noise_steps(self, noise, what="rollout_mlp_noisy", n=None):
         """Check rollout_mlp_noisy()'s or rollout_actor_critic()'s noise without a CUDA call -> T.  n: the batch it
-        is drawn for (rollout_from_mlp()'s B), the env's num_envs when not given."""
+        is drawn for (rollout_from_mlp()'s B), the env's num_envs when not given.  Its last axis is the action space's
+        n or act_dim with or without a head= (a head's noise is A per env, whatever its K)."""
         n = self.num_envs if n is None else n
         torch = _torch()
         K = int(self.single_action_space.n if self.discrete else self.act_dim)
@@ -1360,10 +1429,29 @@ class B200VectorEnv:
                              f"{tuple(bias.shape)}")
         return per_env
 
-    def _mlp_params(self, params, hidden, activation, what="rollout_mlp", n=None):
+    def _mlp_head(self, what, head, obs_norm=None, clip_obs=None, obs_moments=False):
+        """Check rollout_mlp()'s or rollout_mlp_noisy()'s head= without a CUDA call -> None for no head, else the
+        b200gym_mlp_head code."""
+        if head is None:
+            return None
+        if not isinstance(head, str) or head not in _lib.MLP_HEADS:
+            raise ValueError(f"{what}() needs head None, 'tanh' or 'tanh_normal', got {head!r}")
+        if self.discrete:
+            raise ValueError(f"{what}() takes head= only for a Box action space, not "
+                             f"{self.single_action_space!r}")
+        if obs_norm is not None or clip_obs is not None or obs_moments:
+            raise ValueError(f"{what}() does not take head= together with obs_norm, clip_obs or obs_moments")
+        return _lib.MLP_HEADS[head]
+
+    def _head_outputs(self, head):
+        """K, the network outputs of head= (None, 'tanh' or 'tanh_normal') for a Box kind: act_dim, or 2 * act_dim
+        for the SAC head's mean and log-std."""
+        return int(self.act_dim) * (2 if head == "tanh_normal" else 1)
+
+    def _mlp_params(self, params, hidden, activation, what="rollout_mlp", n=None, head=None):
         """Check rollout_mlp()'s or rollout_mlp_noisy()'s parameters without a CUDA call -> (h1, h2 (0 for one hidden
         layer), per_env, the b200gym_mlp_activation code).  n: the number of per-env rows (rollout_from_mlp()'s B),
-        the env's num_envs when not given."""
+        the env's num_envs when not given.  head: a head= that _mlp_head() accepted; it sets K."""
         n = self.num_envs if n is None else n
         torch = _torch()
         if not isinstance(activation, str) or activation not in _lib.MLP_ACTIVATIONS:
@@ -1373,7 +1461,7 @@ class B200VectorEnv:
                 for h in hidden):
             raise ValueError(f"{what}() needs hidden as a tuple of one or two widths, each 1 .. 64, got {hidden!r}")
         widths = [int(h) for h in hidden]
-        K = self.single_action_space.n if self.discrete else self.act_dim
+        K = self.single_action_space.n if self.discrete else self._head_outputs(head)
         sizes = [self.obs_dim] + widths + [int(K)]
         P = sum(o * i + o for i, o in zip(sizes[:-1], sizes[1:]))
         if not isinstance(params, torch.Tensor):

@@ -69,14 +69,14 @@ class VectorWrapper:
                           "fused rollout of the wrapped env would skip it; call step() with the policy's actions T "
                           "times instead")
 
-    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu"):
+    def rollout_mlp(self, params, hidden, T, *, summary=False, activation="relu", head=None):
         """Refused, as rollout(): step the wrapper with the policy's actions instead."""
         from gym_b200 import error
         raise error.Error(f"{type(self).__name__} does not support rollout_mlp(): it acts after every step, and a "
                           "fused rollout of the wrapped env would skip it; call step() with the policy's actions T "
                           "times instead")
 
-    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu"):
+    def rollout_mlp_noisy(self, params, hidden, noise, *, activation="relu", head=None):
         """Refused, as rollout(): step the wrapper with the policy's actions instead."""
         from gym_b200 import error
         raise error.Error(f"{type(self).__name__} does not support rollout_mlp_noisy(): it acts after every step, and "

@@ -298,6 +298,40 @@ int b200gym_rollout_mlp_noisy_act(b200gym_t *h, const float *params_dev, int per
                                   int activation);
 
 /*
+ * The squashing head of b200gym_rollout_mlp_head / b200gym_rollout_mlp_noisy_head: how a Box kind's action of A
+ * dimensions comes from the network's K outputs z.  With the kind's action bounds [low, high] (Pendulum [-2, 2], the
+ * other Box kinds [-1, 1]), scale = float32(float32(high - low) / 2) and bias = float32(float32(high + low) / 2), every
+ * product and sum one rounded float32 operation, tanh = the B200GYM_MLP_TANH function and exp = CUDA's expf (on an H100
+ * the bits of torch.exp on a float32 CUDA tensor; see b200gym_selftest_exp):
+ */
+enum b200gym_mlp_head {
+    /* TD3 / DDPG actor, K = A.  Deterministic: a = tanh(z) * scale + bias.  With noise e (A per env and step):
+       a = clamp((tanh(z) * scale + bias) + e, low, high), where a NaN stays NaN */
+    B200GYM_HEAD_TANH = 1,
+    /* SAC actor, K = 2A: m = z[0 .. A-1] the mean, s = z[A .. 2A-1] the raw log-std.  Deterministic:
+       a = tanh(m) * scale + bias (s is computed and ignored).  With noise eps (A per env and step):
+       ls = -5 + 3.5 * (tanh(s) + 1);  x = m + eps * exp(ls);  a = tanh(x) * scale + bias */
+    B200GYM_HEAD_TANH_NORMAL = 2
+};
+
+/*
+ * b200gym_rollout_mlp_act and b200gym_rollout_mlp_noisy_act with the action taken from the outputs through `head`, a
+ * b200gym_mlp_head; any other value fails, and so does a Discrete kind.  The network has K = A (B200GYM_HEAD_TANH) or
+ * 2A (B200GYM_HEAD_TANH_NORMAL) outputs, and P counts them.  The noisy one reads noise_dev float32 [T][n][A] and writes
+ * outputs_dev float32 [T][n][K] (z, before the head) and the actions float32 [T][n][A].  Everything else is as there.
+ */
+int b200gym_rollout_mlp_head(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                             int32_t T, void *actions_out_dev, float *obs_dev, double *reward_dev,
+                             uint8_t *terminated_dev, uint8_t *truncated_dev, float *final_obs_dev, double *returns_dev,
+                             int32_t *lengths_dev, uint8_t *ended_dev, float *last_obs_dev, const float *first_obs_dev,
+                             void *stream, int activation, int head);
+int b200gym_rollout_mlp_noisy_head(b200gym_t *h, const float *params_dev, int per_env, int n_layers, int h1, int h2,
+                                   int32_t T, const float *noise_dev, float *outputs_dev, void *actions_out_dev,
+                                   float *obs_dev, double *reward_dev, uint8_t *terminated_dev, uint8_t *truncated_dev,
+                                   float *final_obs_dev, float *last_obs_dev, const float *first_obs_dev, void *stream,
+                                   int activation, int head);
+
+/*
  * b200gym_rollout_mlp_noisy_act with one actor shared by every env (actor_dev, P floats), plus a critic and the GAE
  * advantages: one on-policy collection step of PPO / A2C.
  *   critic_dev        the packed critic D -> h1 (-> h2) -> 1, the actor's widths and activation, b200gym_rollout_mlp's
@@ -825,6 +859,12 @@ int b200gym_selftest_trig(const double *x_dev, int64_t n, double *sin_dev, doubl
  * with torch.tanh on the same device).  Asynchronous.
  */
 int b200gym_selftest_tanh(const float *x_dev, int64_t n, float *y_dev, void *stream);
+/*
+ * Device self-test of the exp of the B200GYM_HEAD_TANH_NORMAL head: y_dev[k] = that exp of x_dev[k] for k < n,
+ * float32, computed by the same device function the policy kernels inline (the caller compares with torch.exp on the
+ * same device).  Asynchronous.
+ */
+int b200gym_selftest_exp(const float *x_dev, int64_t n, float *y_dev, void *stream);
 /*
  * Device self-test of the Box2D building blocks (csrc/b2probe.cuh): one thread per record runs `op` on in_dev[n][16]
  * float32 and writes out_dev[n][16].  op: 0 rot_of, 1 edge-polygon manifold, 2 box-polygon manifold, 3 edge ray cast,
