@@ -459,20 +459,23 @@ LD void joint_init(Joint &j, JTemp &t, const JointDef &d, const ShapeConst &A, c
     sB.w += iB * (crs(rB, P) + j.motorImpulse + j.imp[2]);
 }
 
+// the motor part of b2RevoluteJoint::SolveVelocityConstraints (skipped by the caller at an equal-limit joint)
+LD void joint_solve_motor(Joint &j, const JTemp &t, float iA, float iB, float &wA, float &wB, float dt) {
+    const float Cdot = wB - wA - j.motorSpeed;
+    float impulse = -t.motorMass * Cdot;
+    const float oldImpulse = j.motorImpulse, maxImpulse = dt * j.maxMotorTorque;
+    j.motorImpulse = clampf(oldImpulse + impulse, -maxImpulse, maxImpulse);
+    impulse = j.motorImpulse - oldImpulse;
+    wA -= iA * impulse;
+    wB += iB * impulse;
+}
+
 LD void joint_solve_velocity(Joint &j, const JTemp &t, const ShapeConst &A, const ShapeConst &B, BState &sA,
                                                   BState &sB, float dt) {
     const float mA = A.invMass, mB = B.invMass, iA = A.invI, iB = B.invI;
     v2 vA = sA.v, vB = sB.v;
     float wA = sA.w, wB = sB.w;
-    if (j.limitState != 3) {
-        const float Cdot = wB - wA - j.motorSpeed;
-        float impulse = -t.motorMass * Cdot;
-        const float oldImpulse = j.motorImpulse, maxImpulse = dt * j.maxMotorTorque;
-        j.motorImpulse = clampf(oldImpulse + impulse, -maxImpulse, maxImpulse);
-        impulse = j.motorImpulse - oldImpulse;
-        wA -= iA * impulse;
-        wB += iB * impulse;
-    }
+    if (j.limitState != 3) joint_solve_motor(j, t, iA, iB, wA, wB, dt);
     if (j.limitState != 0) {
         const v2 Cdot1 = sub(sub(add(vB, crs_sv(wB, t.rB)), vA), crs_sv(wA, t.rA));
         const float Cdot2 = wB - wA;
@@ -543,6 +546,204 @@ LD bool joint_solve_position(const Joint &j, const JointDef &d, const ShapeConst
     }
     sA.c = cA; sA.a = aA; sB.c = cB; sB.a = aB;
     return positionError <= kLinearSlop && angularError <= kAngularSlop;
+}
+
+// ---- contacts of a dynamic body (B) with the static ground (A, at the identity) ---------------------
+// b2ContactSolver::InitializeVelocityConstraints, per point: the normal and tangent masses at cp.rB
+LD void contact_point_masses(VCP &cp, v2 normal, float mB, float iB) {
+    const float rnB = crs(cp.rB, normal);
+    const float kN = mB + iB * rnB * rnB;
+    cp.normalMass = kN > 0.0f ? 1.0f / kN : 0.0f;
+    const v2 tangent = crs_vs(normal, 1.0f);
+    const float rtB = crs(cp.rB, tangent);
+    const float kT = mB + iB * rtB * rtB;
+    cp.tangentMass = kT > 0.0f ? 1.0f / kT : 0.0f;
+}
+
+// the 2-point block solver's K and its inverse; a K too ill-conditioned for it drops the second point
+LD void contact_block_k(VC &k, float mB, float iB) {
+    const float rn1B = crs(k.p[0].rB, k.normal), rn2B = crs(k.p[1].rB, k.normal);
+    const float k11 = mB + iB * rn1B * rn1B, k22 = mB + iB * rn2B * rn2B, k12 = mB + iB * rn1B * rn2B;
+    if (k11 * k11 < 1000.0f * (k11 * k22 - k12 * k12)) {
+        k.k11 = k11; k.k12 = k12; k.k22 = k22;
+        float det = k11 * k22 - k12 * k12;
+        if (det != 0.0f) det = 1.0f / det;
+        k.n11 = det * k22; k.n12 = -det * k12; k.n22 = det * k11;
+    } else k.pointCount = 1;
+}
+
+// b2WorldManifold::Initialize (world normal, points midway between the two surfaces) and the constraint's masses and
+// K, at body state sB
+LD void contact_init(VC &k, const ShapeConst &sh, const BState &sB) {
+    const float mB = sh.invMass, iB = sh.invI;
+    xform xfB;
+    xfB.q = rot_of(sB.a);
+    xfB.p = sub(sB.c, rmul(xfB.q, sh.localCenter));
+    v2 pts[2];
+    xform xfA;  // the ground body: identity transform (kept as explicit arithmetic, like Box2D does)
+    xfA.p = V(0.0f, 0.0f); xfA.q.s = 0.0f; xfA.q.c = 1.0f;
+    if (k.mType == 0) {  // e_faceA
+        k.normal = rmul(xfA.q, k.localNormal);
+        const v2 plane = xmul(xfA, k.localPoint);
+        for (int p = 0; p < k.pointCount; p++) {
+            const v2 clip = xmul(xfB, k.lp[p]);
+            const v2 cA = add(clip, scl(kPolygonRadius - dot(sub(clip, plane), k.normal), k.normal));
+            const v2 cB = sub(clip, scl(kPolygonRadius, k.normal));
+            pts[p] = scl(0.5f, add(cA, cB));
+        }
+    } else {             // e_faceB
+        v2 nrm = rmul(xfB.q, k.localNormal);
+        const v2 plane = xmul(xfB, k.localPoint);
+        for (int p = 0; p < k.pointCount; p++) {
+            const v2 clip = xmul(xfA, k.lp[p]);
+            const v2 cB = add(clip, scl(kPolygonRadius - dot(sub(clip, plane), nrm), nrm));
+            const v2 cA = sub(clip, scl(kPolygonRadius, nrm));
+            pts[p] = scl(0.5f, add(cA, cB));
+        }
+        k.normal = neg(nrm);
+    }
+    for (int p = 0; p < k.pointCount; p++) {
+        k.p[p].rB = sub(pts[p], sB.c);
+        contact_point_masses(k.p[p], k.normal, mB, iB);
+    }
+    if (k.pointCount == 2) contact_block_k(k, mB, iB);
+}
+
+// Which rule b2ContactSolver's 2-point block solver took: 1 both points pushing, 2 only the first, 3 only the second,
+// 4 neither; 0 when no case held (the impulses are left as they were), -1 for a 1-point constraint
+enum { kBlockNone = 0, kBlockBoth = 1, kBlockFirst = 2, kBlockSecond = 3, kBlockNeither = 4, kOnePoint = -1 };
+
+// One velocity iteration of one contact constraint on body B: friction at every point, then the normal impulse --
+// the 1-point solve or the 2-point block LCP.  Returns the block solver's case.
+LD int contact_solve_velocity(VC &k, const ShapeConst &sh, BState &sB) {
+    const float mB = sh.invMass, iB = sh.invI;
+    v2 vB = sB.v;
+    float wB = sB.w;
+    int kase = kOnePoint;
+    const v2 normal = k.normal, tangent = crs_vs(normal, 1.0f);
+    for (int p = 0; p < k.pointCount; p++) {
+        VCP &cp = k.p[p];
+        const v2 dv = add(vB, crs_sv(wB, cp.rB));
+        const float vt = dot(dv, tangent) - 0.0f;
+        float lambda = cp.tangentMass * (-vt);
+        const float maxF = k.friction * cp.nI;
+        const float newImp = clampf(cp.tI + lambda, -maxF, maxF);
+        lambda = newImp - cp.tI;
+        cp.tI = newImp;
+        const v2 P = scl(lambda, tangent);
+        vB = add(vB, scl(mB, P)); wB += iB * crs(cp.rB, P);
+    }
+    if (k.pointCount == 1) {
+        VCP &cp = k.p[0];
+        const v2 dv = add(vB, crs_sv(wB, cp.rB));
+        const float vn = dot(dv, normal);
+        float lambda = -cp.normalMass * (vn - 0.0f);
+        const float newImp = fmax_(cp.nI + lambda, 0.0f);
+        lambda = newImp - cp.nI;
+        cp.nI = newImp;
+        const v2 P = scl(lambda, normal);
+        vB = add(vB, scl(mB, P)); wB += iB * crs(cp.rB, P);
+    } else {
+        VCP &c1 = k.p[0], &c2 = k.p[1];
+        const v2 a = V(c1.nI, c2.nI);
+        const v2 dv1 = add(vB, crs_sv(wB, c1.rB)), dv2 = add(vB, crs_sv(wB, c2.rB));
+        float vn1 = dot(dv1, normal), vn2 = dot(dv2, normal);
+        v2 b = V(vn1 - 0.0f, vn2 - 0.0f);
+        b = sub(b, V(k.k11 * a.x + k.k12 * a.y, k.k12 * a.x + k.k22 * a.y));
+        v2 x;
+        bool solved = false;
+        kase = kBlockNone;
+        x = V(-(k.n11 * b.x + k.n12 * b.y), -(k.n12 * b.x + k.n22 * b.y));
+        if (x.x >= 0.0f && x.y >= 0.0f) { solved = true; kase = kBlockBoth; }
+        if (!solved) {
+            x.x = -c1.normalMass * b.x; x.y = 0.0f;
+            vn2 = k.k12 * x.x + b.y;
+            if (x.x >= 0.0f && vn2 >= 0.0f) { solved = true; kase = kBlockFirst; }
+        }
+        if (!solved) {
+            x.x = 0.0f; x.y = -c2.normalMass * b.y;
+            vn1 = k.k12 * x.y + b.x;
+            if (x.y >= 0.0f && vn1 >= 0.0f) { solved = true; kase = kBlockSecond; }
+        }
+        if (!solved) {
+            x.x = 0.0f; x.y = 0.0f;
+            if (b.x >= 0.0f && b.y >= 0.0f) { solved = true; kase = kBlockNeither; }
+        }
+        if (solved) {
+            const v2 d = sub(x, a);
+            const v2 P1 = scl(d.x, normal), P2 = scl(d.y, normal);
+            vB = add(vB, scl(mB, add(P1, P2)));
+            wB += iB * (crs(c1.rB, P1) + crs(c2.rB, P2));
+            c1.nI = x.x; c2.nI = x.y;
+        }
+    }
+    sB.v = vB; sB.w = wB;
+    return kase;
+}
+
+// One position iteration of one contact constraint (b2ContactSolver::SolvePositionConstraints) on body B, over the
+// manifold's points (mPointCount: the condition-number fallback does not apply here); folds every point's separation
+// before its correction into minSep
+LD void contact_solve_position(const VC &k, const ShapeConst &sh, BState &sB, float &minSep) {
+    const float mB = sh.invMass, iB = sh.invI;
+    v2 cB = sB.c;
+    float aB = sB.a;
+    for (int p = 0; p < k.mPointCount; p++) {
+        xform xfB;
+        xfB.q = rot_of(aB);
+        xfB.p = sub(cB, rmul(xfB.q, sh.localCenter));
+        v2 normal, point;
+        float separation;
+        if (k.mType == 0) {
+            normal = k.localNormal;
+            const v2 clip = xmul(xfB, k.lp[p]);
+            separation = dot(sub(clip, k.localPoint), normal) - kPolygonRadius - kPolygonRadius;
+            point = clip;
+        } else {
+            normal = rmul(xfB.q, k.localNormal);
+            const v2 plane = xmul(xfB, k.localPoint);
+            const v2 clip = k.lp[p];
+            separation = dot(sub(clip, plane), normal) - kPolygonRadius - kPolygonRadius;
+            point = clip;
+            normal = neg(normal);
+        }
+        const v2 rB = sub(point, cB);
+        minSep = fmin_(minSep, separation);
+        const float C = clampf(kBaumgarte * (separation + kLinearSlop), -kMaxLinearCorrection, 0.0f);
+        const float rnB = crs(rB, normal);
+        const float K = mB + iB * rnB * rnB;
+        const float impulse = K > 0.0f ? -C / K : 0.0f;
+        const v2 P = scl(impulse, normal);
+        cB = add(cB, scl(mB, P));
+        aB += iB * crs(rB, P);
+    }
+    sB.c = cB; sB.a = aB;
+}
+
+// ---- b2Island::Solve's integration (no damping) --------------------------------------------------
+// velocities: gravity plus the force and torque applied to the body before the step
+LD void integrate_velocity(BState &s, const ShapeConst &sh, v2 force, float torque, v2 gravity, float dt) {
+    v2 v = s.v;
+    float w = s.w;
+    v = add(v, scl(dt, add(gravity, scl(sh.invMass, force))));
+    w = w + dt * sh.invI * torque;
+    v = scl(1.0f / (1.0f + dt * 0.0f), v);
+    w = w * (1.0f / (1.0f + dt * 0.0f));
+    s.v = v; s.w = w;
+}
+
+// positions, after the velocity iterations: a step moves a body at most kMaxTranslation and turns it at most
+// kMaxRotation, the velocity scaled down to match
+LD void integrate_position(BState &s, float dt) {
+    v2 v = s.v;
+    float w = s.w;
+    const v2 tr = scl(dt, v);
+    if (dot(tr, tr) > kMaxTranslation * kMaxTranslation) { const float ratio = kMaxTranslation / sqrtf(dot(tr, tr)); v = scl(ratio, v); }
+    const float rotn = dt * w;
+    if (rotn * rotn > kMaxRotation * kMaxRotation) { const float ratio = kMaxRotation / fabsf(rotn); w *= ratio; }
+    s.c = add(s.c, scl(dt, v));
+    s.a = s.a + dt * w;
+    s.v = v; s.w = w;
 }
 
 #include "b2lite_toi.cuh"
@@ -664,15 +865,8 @@ __device__ __noinline__ void world_step(typename Scene::World &W, v2 force0, flo
     BState st[NB];
     static_for<0, NB>([&](auto I) {
         constexpr int i = decltype(I)::value;
-        const ShapeConst &sh = Scene::shape(i);
-        v2 v = W.b[i].v;
-        float w = W.b[i].w;
-        const v2 force = i == 0 ? force0 : V(0.0f, 0.0f);
-        v = add(v, scl(dt, add(gravity, scl(sh.invMass, force))));
-        w = w + dt * sh.invI * (i == 0 ? torque0 : 0.0f);
-        v = scl(1.0f / (1.0f + dt * 0.0f), v);
-        w = w * (1.0f / (1.0f + dt * 0.0f));
-        st[i].c = W.b[i].c; st[i].a = W.b[i].a; st[i].v = v; st[i].w = w;
+        st[i].c = W.b[i].c; st[i].a = W.b[i].a; st[i].v = W.b[i].v; st[i].w = W.b[i].w;
+        integrate_velocity(st[i], Scene::shape(i), i == 0 ? force0 : V(0.0f, 0.0f), i == 0 ? torque0 : 0.0f, gravity, dt);
     });
     Joint jn[NJ];
     static_for<0, NJ>([&](auto K) { constexpr int k = decltype(K)::value; jn[k] = W.j[k]; });
@@ -680,60 +874,11 @@ __device__ __noinline__ void world_step(typename Scene::World &W, v2 force0, flo
     uint32_t ids[kMaxVC][2];
     static_for<0, NB>([&](auto OI) {
         constexpr int oi = decltype(OI)::value, body = Scene::body_order(oi);
-        const ShapeConst &sh = Scene::shape(body);
-        const BState &sB = st[body];
-        const float mB = sh.invMass, iB = sh.invI;
         for (int ci = oi == 0 ? 0 : cend[oi == 0 ? 0 : oi - 1]; ci < cend[oi]; ci++) {
             VC &k = vc[ci];
             ids[ci][0] = __float_as_uint(k.p[0].normalMass);
             ids[ci][1] = k.pointCount > 1 ? __float_as_uint(k.p[1].normalMass) : 0u;
-            xform xfB;
-            xfB.q = rot_of(sB.a);
-            xfB.p = sub(sB.c, rmul(xfB.q, sh.localCenter));
-            v2 pts[2];
-            xform xfA;  // the ground body: identity transform (kept as explicit arithmetic, like Box2D does)
-            xfA.p = V(0.0f, 0.0f); xfA.q.s = 0.0f; xfA.q.c = 1.0f;
-            if (k.mType == 0) {  // b2WorldManifold::Initialize, e_faceA
-                k.normal = rmul(xfA.q, k.localNormal);
-                const v2 plane = xmul(xfA, k.localPoint);
-                for (int p = 0; p < k.pointCount; p++) {
-                    const v2 clip = xmul(xfB, k.lp[p]);
-                    const v2 cA = add(clip, scl(kPolygonRadius - dot(sub(clip, plane), k.normal), k.normal));
-                    const v2 cB = sub(clip, scl(kPolygonRadius, k.normal));
-                    pts[p] = scl(0.5f, add(cA, cB));
-                }
-            } else {             // e_faceB
-                v2 nrm = rmul(xfB.q, k.localNormal);
-                const v2 plane = xmul(xfB, k.localPoint);
-                for (int p = 0; p < k.pointCount; p++) {
-                    const v2 clip = xmul(xfA, k.lp[p]);
-                    const v2 cB = add(clip, scl(kPolygonRadius - dot(sub(clip, plane), nrm), nrm));
-                    const v2 cA = sub(clip, scl(kPolygonRadius, nrm));
-                    pts[p] = scl(0.5f, add(cA, cB));
-                }
-                k.normal = neg(nrm);
-            }
-            for (int p = 0; p < k.pointCount; p++) {
-                VCP &cp = k.p[p];
-                cp.rB = sub(pts[p], sB.c);
-                const float rnB = crs(cp.rB, k.normal);
-                const float kN = mB + iB * rnB * rnB;
-                cp.normalMass = kN > 0.0f ? 1.0f / kN : 0.0f;
-                const v2 tangent = crs_vs(k.normal, 1.0f);
-                const float rtB = crs(cp.rB, tangent);
-                const float kT = mB + iB * rtB * rtB;
-                cp.tangentMass = kT > 0.0f ? 1.0f / kT : 0.0f;
-            }
-            if (k.pointCount == 2) {
-                const float rn1B = crs(k.p[0].rB, k.normal), rn2B = crs(k.p[1].rB, k.normal);
-                const float k11 = mB + iB * rn1B * rn1B, k22 = mB + iB * rn2B * rn2B, k12 = mB + iB * rn1B * rn2B;
-                if (k11 * k11 < 1000.0f * (k11 * k22 - k12 * k12)) {
-                    k.k11 = k11; k.k12 = k12; k.k22 = k22;
-                    float det = k11 * k22 - k12 * k12;
-                    if (det != 0.0f) det = 1.0f / det;
-                    k.n11 = det * k22; k.n12 = -det * k12; k.n22 = det * k11;
-                } else k.pointCount = 1;
-            }
+            contact_init(k, Scene::shape(body), st[body]);
         }
     });
     // --- WarmStart
@@ -767,70 +912,8 @@ __device__ __noinline__ void world_step(typename Scene::World &W, v2 force0, flo
         });
         if (nvc != 0) static_for<0, NB>([&](auto OI) {
             constexpr int oi = decltype(OI)::value, body = Scene::body_order(oi);
-            const ShapeConst &sh = Scene::shape(body);
-            const float mB = sh.invMass, iB = sh.invI;
-            for (int ci = oi == 0 ? 0 : cend[oi == 0 ? 0 : oi - 1]; ci < cend[oi]; ci++) {
-                VC &k = vc[ci];
-                v2 vB = st[body].v;
-                float wB = st[body].w;
-                const v2 normal = k.normal, tangent = crs_vs(normal, 1.0f);
-                for (int p = 0; p < k.pointCount; p++) {
-                    VCP &cp = k.p[p];
-                    const v2 dv = add(vB, crs_sv(wB, cp.rB));
-                    const float vt = dot(dv, tangent) - 0.0f;
-                    float lambda = cp.tangentMass * (-vt);
-                    const float maxF = k.friction * cp.nI;
-                    const float newImp = clampf(cp.tI + lambda, -maxF, maxF);
-                    lambda = newImp - cp.tI;
-                    cp.tI = newImp;
-                    const v2 P = scl(lambda, tangent);
-                    vB = add(vB, scl(mB, P)); wB += iB * crs(cp.rB, P);
-                }
-                if (k.pointCount == 1) {
-                    VCP &cp = k.p[0];
-                    const v2 dv = add(vB, crs_sv(wB, cp.rB));
-                    const float vn = dot(dv, normal);
-                    float lambda = -cp.normalMass * (vn - 0.0f);
-                    const float newImp = fmax_(cp.nI + lambda, 0.0f);
-                    lambda = newImp - cp.nI;
-                    cp.nI = newImp;
-                    const v2 P = scl(lambda, normal);
-                    vB = add(vB, scl(mB, P)); wB += iB * crs(cp.rB, P);
-                } else {
-                    VCP &c1 = k.p[0], &c2 = k.p[1];
-                    const v2 a = V(c1.nI, c2.nI);
-                    const v2 dv1 = add(vB, crs_sv(wB, c1.rB)), dv2 = add(vB, crs_sv(wB, c2.rB));
-                    float vn1 = dot(dv1, normal), vn2 = dot(dv2, normal);
-                    v2 b = V(vn1 - 0.0f, vn2 - 0.0f);
-                    b = sub(b, V(k.k11 * a.x + k.k12 * a.y, k.k12 * a.x + k.k22 * a.y));
-                    v2 x;
-                    bool solved = false;
-                    x = V(-(k.n11 * b.x + k.n12 * b.y), -(k.n12 * b.x + k.n22 * b.y));
-                    if (x.x >= 0.0f && x.y >= 0.0f) solved = true;
-                    if (!solved) {
-                        x.x = -c1.normalMass * b.x; x.y = 0.0f;
-                        vn2 = k.k12 * x.x + b.y;
-                        if (x.x >= 0.0f && vn2 >= 0.0f) solved = true;
-                    }
-                    if (!solved) {
-                        x.x = 0.0f; x.y = -c2.normalMass * b.y;
-                        vn1 = k.k12 * x.y + b.x;
-                        if (x.y >= 0.0f && vn1 >= 0.0f) solved = true;
-                    }
-                    if (!solved) {
-                        x.x = 0.0f; x.y = 0.0f;
-                        if (b.x >= 0.0f && b.y >= 0.0f) solved = true;
-                    }
-                    if (solved) {
-                        const v2 d = sub(x, a);
-                        const v2 P1 = scl(d.x, normal), P2 = scl(d.y, normal);
-                        vB = add(vB, scl(mB, add(P1, P2)));
-                        wB += iB * (crs(c1.rB, P1) + crs(c2.rB, P2));
-                        c1.nI = x.x; c2.nI = x.y;
-                    }
-                }
-                st[body].v = vB; st[body].w = wB;
-            }
+            for (int ci = oi == 0 ? 0 : cend[oi == 0 ? 0 : oi - 1]; ci < cend[oi]; ci++)
+                contact_solve_velocity(vc[ci], Scene::shape(body), st[body]);
         });
     }
     // --- StoreImpulses: rebuild the warm-start store from this step's touching contacts
@@ -846,18 +929,7 @@ __device__ __noinline__ void world_step(typename Scene::World &W, v2 force0, flo
         }
     }
     // --- integrate positions
-    static_for<0, NB>([&](auto I) {
-        constexpr int i = decltype(I)::value;
-        v2 v = st[i].v;
-        float w = st[i].w;
-        const v2 tr = scl(dt, v);
-        if (dot(tr, tr) > kMaxTranslation * kMaxTranslation) { const float ratio = kMaxTranslation / sqrtf(dot(tr, tr)); v = scl(ratio, v); }
-        const float rotn = dt * w;
-        if (rotn * rotn > kMaxRotation * kMaxRotation) { const float ratio = kMaxRotation / fabsf(rotn); w *= ratio; }
-        st[i].c = add(st[i].c, scl(dt, v));
-        st[i].a = st[i].a + dt * w;
-        st[i].v = v; st[i].w = w;
-    });
+    static_for<0, NB>([&](auto I) { integrate_position(st[decltype(I)::value], dt); });
     // --- <= 60 position iterations
     bool positionSolved = false;
 #pragma unroll 1
@@ -866,43 +938,8 @@ __device__ __noinline__ void world_step(typename Scene::World &W, v2 force0, flo
         if (nvc != 0)
             static_for<0, NB>([&](auto OI) {
                 constexpr int oi = decltype(OI)::value, body = Scene::body_order(oi);
-                const ShapeConst &sh = Scene::shape(body);
-                const float mB = sh.invMass, iB = sh.invI;
-                for (int ci = oi == 0 ? 0 : cend[oi == 0 ? 0 : oi - 1]; ci < cend[oi]; ci++) {
-                    const VC &k = vc[ci];
-                    v2 cB = st[body].c;
-                    float aB = st[body].a;
-                    for (int p = 0; p < k.mPointCount; p++) {
-                        xform xfB;
-                        xfB.q = rot_of(aB);
-                        xfB.p = sub(cB, rmul(xfB.q, sh.localCenter));
-                        v2 normal, point;
-                        float separation;
-                        if (k.mType == 0) {
-                            normal = k.localNormal;
-                            const v2 clip = xmul(xfB, k.lp[p]);
-                            separation = dot(sub(clip, k.localPoint), normal) - kPolygonRadius - kPolygonRadius;
-                            point = clip;
-                        } else {
-                            normal = rmul(xfB.q, k.localNormal);
-                            const v2 plane = xmul(xfB, k.localPoint);
-                            const v2 clip = k.lp[p];
-                            separation = dot(sub(clip, plane), normal) - kPolygonRadius - kPolygonRadius;
-                            point = clip;
-                            normal = neg(normal);
-                        }
-                        const v2 rB = sub(point, cB);
-                        minSep = fmin_(minSep, separation);
-                        const float C = clampf(kBaumgarte * (separation + kLinearSlop), -kMaxLinearCorrection, 0.0f);
-                        const float rnB = crs(rB, normal);
-                        const float K = mB + iB * rnB * rnB;
-                        const float impulse = K > 0.0f ? -C / K : 0.0f;
-                        const v2 P = scl(impulse, normal);
-                        cB = add(cB, scl(mB, P));
-                        aB += iB * crs(rB, P);
-                    }
-                    st[body].c = cB; st[body].a = aB;
-                }
+                for (int ci = oi == 0 ? 0 : cend[oi == 0 ? 0 : oi - 1]; ci < cend[oi]; ci++)
+                    contact_solve_position(vc[ci], Scene::shape(body), st[body], minSep);
             });
         const bool contactsOkay = minSep >= -3.0f * kLinearSlop;
         bool jointsOkay = true;

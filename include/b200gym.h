@@ -868,8 +868,10 @@ int b200gym_selftest_exp(const float *x_dev, int64_t n, float *y_dev, void *stre
 /*
  * Device self-test of the Box2D building blocks (csrc/b2probe.cuh): one thread per record runs `op` on in_dev[n][16]
  * float32 and writes out_dev[n][16].  op: 0 rot_of, 1 edge-polygon manifold, 2 box-polygon manifold, 3 edge ray cast,
- * 4 box ray cast, 5 GJK distance, 6 time of impact, 7 solve22, 8 solve33; the record layouts are listed in
- * b2probe.cuh.  Loads the task polygons into constant memory as b200gym_create does, then launches asynchronously.
+ * 4 box ray cast, 5 GJK distance, 6 time of impact, 7 solve22, 8 solve33, 9 contact init, 10 one contact velocity
+ * iteration, 11 one contact position iteration, 12 joint init + one velocity iteration, 13 one joint position
+ * iteration, 14 integration, 15 the task constants; the record layouts are listed in b2probe.cuh.  Loads the task
+ * polygons and joints into constant memory as b200gym_create does, then launches asynchronously.
  */
 int b200gym_selftest_box2d(int op, const float *in_dev, int64_t n, float *out_dev, void *stream);
 
